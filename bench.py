@@ -1,10 +1,10 @@
 #!/usr/bin/env python
 """bench.py — reads/sec of the `coverm contig|genome --bam-files` coverage hot path (BASELINE.json).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config 2|ns|3]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config 2|ns|3] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
-Workloads (`--config`, all synthetic, SURVEY.md §8d; the default is BASELINE.json configs[1]):
+Workloads (`--config`, all synthetic; the default is BASELINE.json configs[1]):
   2    coverm contig -m mean trimmed_mean covered_fraction, 500 000 contigs / ~2.8 Gbp / ~10.5 M records
   ns   the north-star target: the same command on a ~5 Gbp / ~52 M-record BAM (906 000 contigs)
   3    coverm genome -s '~' -m mean trimmed_mean covered_fraction --min-read-percent-identity 95,
@@ -22,6 +22,12 @@ One "step" = one pass of the hot path over one sample.
   roofline / cpu_baseline as described in DESIGN.md (Measurement).
 `--impl reference` times the CPU restatement of the reference (oracle/, all host threads for BGZF inflate, the record loop
 single-threaded exactly as the reference's) on the SAME file and command; one step = one full run.
+`--dump-outputs DIR` writes what the last timed steps returned as float64 .npy files, so that two builds can be compared on
+the same seeded inputs: `rows_<field>.npy`, the per-contig table of the last device step (cmb_contig_stats, one value per
+contig), and `table_<column>.npy`, the numeric columns of the TSV the last e2e step printed.  Tables of more than
+DUMP_MAX_ROWS rows are reduced to a fixed seeded sample of rows whose indices are in `rows_index.npy` / `table_index.npy`.
+`rows_sum_identity_*` are f64 sums accumulated with atomics, so they may differ between runs in the last bits (relative
+1e-14); every other array is exact.
 """
 import argparse
 import json
@@ -71,7 +77,7 @@ def measured_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs, burst: K2 is timed as a single launch)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "H100 SXM data sheet, 3.35 TB/s HBM3 (not measured)"
 
 
 class ClockSampler(threading.Thread):
@@ -141,7 +147,7 @@ def workload_config(cfg, args, info, world, scaling):
                         f" on a synthetic reference-sorted BAM, {args.contigs} contigs / {info['bases']} bp / {info['records']} records",
             "config_id": args.config, "contigs": args.contigs, "reads": int(info["records"]), "bases": int(info["bases"]),
             "bam_bytes": int(info["bam_bytes"]), "seed": args.seed, "parallelism": par,
-            "l2": f"inputs larger than L2 (126 MB), no flush needed: {4 * info['bases'] / 1e9:.1f} GB delta arena (4 B per reference base) + "
+            "l2": f"inputs larger than L2 (50 MB), no flush needed: {4 * info['bases'] / 1e9:.1f} GB delta arena (4 B per reference base) + "
                   f"{48.5 * info['records'] / 1e6:.0f} MB tuples per step; e2e additionally streams the {info['bam_bytes'] / 1e9:.2f} GB file"}
 
 
@@ -168,6 +174,52 @@ def cpu_baseline_entry(records, sec, threads, runs, what):
             "seconds_per_run": sec}
 
 
+DUMP_MAX_ROWS = 200000  # 16 row fields + a few table columns at 8 B per value stay under 64 MB
+
+
+def dump_sample(n, seed):
+    """Indices of the rows to dump: all of them, or a fixed seeded sample of DUMP_MAX_ROWS in ascending order."""
+    import numpy as np
+    if n <= DUMP_MAX_ROWS:
+        return np.arange(n)
+    return np.sort(np.random.default_rng(seed).choice(n, DUMP_MAX_ROWS, replace=False))
+
+
+def fetch_rows(rows_ptr, n_contigs):
+    """The cmb_contig_stats table the device step left in HBM, as a numpy structured array."""
+    import numpy as np
+    import torch
+    from coverm_b200 import ContigStats
+    nbytes = n_contigs * C_sizeof(ContigStats)
+
+    class DeviceBytes:
+        __cuda_array_interface__ = {"shape": (nbytes,), "typestr": "|u1", "data": (rows_ptr, False), "version": 3}
+
+    torch.cuda.synchronize()
+    raw = torch.as_tensor(DeviceBytes(), device="cuda").cpu().numpy()
+    return raw.view(np.dtype(ContigStats))
+
+
+def dump_outputs(out_dir, rows, table, seed):
+    """Write the last device step's per-contig rows and the last e2e step's table as float64 .npy files."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    if rows is not None:  # --impl reference returns the table only
+        idx = dump_sample(len(rows), seed)
+        np.save(os.path.join(out_dir, "rows_index.npy"), idx.astype(np.float64))
+        for name in rows.dtype.names:
+            if name in ("hist_offset", "hist_count", "reserved"):  # buffer bookkeeping, not results
+                continue
+            np.save(os.path.join(out_dir, f"rows_{name}.npy"), rows[name][idx].astype(np.float64))
+    lines = table.splitlines()
+    header, body = lines[0].split("\t"), [l.split("\t") for l in lines[1:]]
+    idx = dump_sample(len(body), seed + 1)
+    np.save(os.path.join(out_dir, "table_index.npy"), idx.astype(np.float64))
+    for j, col in enumerate(header[1:], start=1):
+        name = col.split(" ", 1)[-1].strip().lower().replace(" ", "_")  # "<sample> Trimmed Mean" -> trimmed_mean
+        np.save(os.path.join(out_dir, f"table_{name}.npy"), np.array([float(body[i][j]) for i in idx], dtype=np.float64))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -186,7 +238,11 @@ def main():
     ap.add_argument("--scaling", default="strong", choices=["strong", "weak"],
                     help="N > 1: strong = one sample range-partitioned by contig over the N GPUs (default); weak = N samples, one per GPU")
     ap.add_argument("--workdir", default=os.environ.get("CMB_BENCH_DIR", "/tmp/coverm_b200_bench"))
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the outputs of the last timed steps to DIR/<name>.npy (float64; see the module docstring)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     cfg = CONFIGS[args.config]
     args.contigs = args.contigs or cfg["contigs"]
     args.reads = args.reads or cfg["reads"]
@@ -228,7 +284,10 @@ def main():
             est = max(times) if times else (elapsed if warm else 0.0)
             if times and elapsed + est > args.ref_budget_s:
                 break
-            times.append(run_oracle(cfg, bam, ncpu, 1, 0)[0])
+            sec_run, ref_out = run_oracle(cfg, bam, ncpu, 1, 0)
+            times.append(sec_run)
+        if args.dump_outputs:
+            dump_outputs(args.dump_outputs, None, ref_out, args.seed)
         steps = len(times)
         sec = sum(times) / steps
         cpu = cpu_baseline_entry(info["records"], sec, ncpu, steps, "the full workload file")
@@ -341,9 +400,10 @@ def main():
     def device_step():
         ctx.begin_sample()
         ctx.submit_device_batch(batch, n_rec, n_iv)
-        ctx.end_sample_device()  # K1c/K1b/K2/K3 + error check (stream-synchronous)
+        rows_ptr = ctx.end_sample_device()  # K1c/K1b/K2/K3 + error check (stream-synchronous)
         if strong:
             ctx.allgather_stats(cuts)  # the collective of the path, on the same stream (NCCL broadcasts of each rank's row range)
+        return rows_ptr
 
     sampler = ClockSampler(local_rank)
     n_warm = max(3, args.warmup)
@@ -360,7 +420,7 @@ def main():
         ev0.record()
     launches = 0
     for _ in range(args.steps):
-        device_step()
+        rows_ptr = device_step()
         tm = ctx.timing()
         k0_ms.append(tm["ms_zero"]); k1_ms.append(tm["ms_accumulate"]); k2_ms.append(tm["ms_scan"]); k3_ms.append(tm["ms_finalize"])
         dev_ms.append(tm["ms_total"])
@@ -380,11 +440,8 @@ def main():
     k2_mean = mean(k2_ms)
     algo_bytes = 4.0 * arena_elems
     achieved = algo_bytes / (k2_mean * 1e-3) / 1e9
-    traffic, traffic_src = None, None
-    tpath = os.path.join(ROOT, "profiles", "k2_traffic.json")
-    if os.path.exists(tpath) and args.config == "2" and world == 1:
-        tj = json.load(open(tpath))
-        traffic, traffic_src = tj.get("dram_bytes_per_launch"), tj.get("source", "profiles/k2_traffic.json (ncu --set full capture of this workload)")
+    # the e2e steps below reuse the context and overwrite its rows: keep the last device step's table now
+    dumped_rows = fetch_rows(rows_ptr, n_contigs) if args.dump_outputs and rank == 0 else None
 
     # ---------------------------------------------------------------- e2e arm: BAM bytes in host memory -> TSV
     e2e_steps = args.e2e_steps or args.steps
@@ -418,6 +475,8 @@ def main():
     d2h = row_bytes * world
     e2e_launches = s0["decode_launches"] + s0["k1_launches"] + 3 + s0["k2_launches"] + s0["k3_launches"]
     e2e_out = res.out  # the table of the last timed step (full file)
+    if dumped_rows is not None:
+        dump_outputs(args.dump_outputs, dumped_rows, e2e_out, args.seed)
     same_as_single = None
     if strong and rank == 0:
         same_as_single = e2e_out == single_out
@@ -479,7 +538,7 @@ def main():
                     "cold_cli": cold},
             "gpu_launches": int(launches),
             "roofline": {"bound": "hbm", "kernel": "k2_scan_reduce<HIST,CLEAN>", "achieved": achieved, "peak": peak, "unit": "GB/s",
-                         "frac": achieved / peak, "traffic": traffic, "traffic_source": traffic_src, "peak_source": peak_src,
+                         "frac": achieved / peak, "peak_source": peak_src,
                          "algorithmic_bytes_per_launch": algo_bytes, "avg_launch_ms": k2_mean,
                          "note": "rank 0's launch" + (" (1/N of the arena)" if strong else "")},
             "device_breakdown_ms_rank0": {"k0_zero": mean(k0_ms), "k1_filter_delta+carry": mean(k1_ms), "k2_scan_reduce": k2_mean,

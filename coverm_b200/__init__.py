@@ -1,6 +1,6 @@
-"""coverm_b200 — B200-native replacement for CoverM's per-contig coverage hot path.
+"""coverm_b200 — H100-native replacement for CoverM's per-contig coverage hot path.
 
-The product is the native library ``coverm_b200/libcoverm_b200.so`` (hand-written sm_100a CUDA kernels behind the C
+The product is the native library ``coverm_b200/libcoverm_b200.so`` (hand-written sm_90a CUDA kernels behind the C
 ABI declared in ``include/coverm_b200.h`` and ``include/coverm_b200_host.h``) plus the ``coverm_b200/bin/coverm``
 command-line binary.  This module is only a thin ctypes binding over that ABI for tests, ``bench.py`` and
 ``__graft_entry__.py``; there is no Python or CPU fallback — importing works anywhere, but every compute entry

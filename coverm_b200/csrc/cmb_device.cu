@@ -1,4 +1,4 @@
-// libcoverm_b200 — device side: hand-written sm_100a kernels + the C ABI of include/coverm_b200.h.
+// libcoverm_b200 — device side: hand-written sm_90a kernels + the C ABI of include/coverm_b200.h.
 //
 // Data layout in HBM (one cmb_ctx = one GPU = one contig shard):
 //   arena        i32[arena_elems]   all contigs' `ups_and_downs` (contig.rs:144-145) back to back; every contig
@@ -535,8 +535,8 @@ int cmb_create(const cmb_device_cfg* cfg, cmb_ctx** out) {
   CREATE_TRY(cudaSetDevice(c->device));
   cudaDeviceProp prop;
   CREATE_TRY(cudaGetDeviceProperties(&prop, c->device));
-  if (prop.major < 10) {
-    fail(c, CMB_E_CUDA, "cmb_create: device %d is sm_%d%d; this library is built for sm_100a only", c->device, prop.major, prop.minor);
+  if (prop.major != 9 || prop.minor != 0) {
+    fail(c, CMB_E_CUDA, "cmb_create: device %d is sm_%d%d; this library is built for sm_90a only", c->device, prop.major, prop.minor);
     return bail(CMB_E_CUDA);
   }
   c->sm_count = prop.multiProcessorCount;
@@ -1179,9 +1179,9 @@ constexpr uint64_t DEC_TAIL_BYTES = 4u << 20;  // ranged decode: inflated bytes 
 // Launch the inflate kernel over blocks [a.b0, a.b1).  CMB_INFLATE selects the first-pass kernel: t1 (default: one thread
 // per block + kd_crc32), g8 (four blocks per warp) or w1 (one block per warp, also the second pass over declined blocks).
 // First-pass inflate kernel: 0 = kd_inflate_t1 (a thread per block), 1 = kd_inflate_g8 (four blocks per warp), 2 = kd_inflate (a
-// warp per block).  t1 has the higher THROUGHPUT (its ~75 000 streams in flight need that many blocks) but every block takes
-// ~50 ms however few there are; g8 finishes a block in ~20 ms.  So the choice follows the number of blocks: a whole 10 M-read
-// file (46 000 blocks) goes to t1, a rank's share of it on 4 or 8 GPUs to g8.  CMB_INFLATE=t1|g8|w1 overrides.
+// warp per block).  t1 has the higher THROUGHPUT (its sm_count x 5 x 96 streams, 63 360 on 132 SMs, need that many blocks) but
+// each of its streams is slow, so a short list of blocks finishes sooner on g8.  The choice follows the number of blocks: a whole
+// 10 M-read file (46 000 blocks) goes to t1, a rank's share of it on 4 or 8 GPUs to g8.  CMB_INFLATE=t1|g8|w1 overrides.
 constexpr uint32_t T1_MIN_BLOCKS = 28000;
 int inflate_kind(uint32_t n_blocks) {
   static const int forced = [] {

@@ -1,5 +1,5 @@
 /*
- * coverm_b200.h — C ABI of libcoverm_b200.so: the B200 (sm_100a) replacement for
+ * coverm_b200.h — C ABI of libcoverm_b200.so: the H100 (sm_90a) replacement for
  * CoverM's per-contig coverage hot path.
  *
  * All citations are file:line under the reference tree (wwood/CoverM v0.8.0).

@@ -2,7 +2,7 @@
 //
 // Literal single-threaded CPU restatement of CoverM v0.8.0's coverage path.
 // Every function cites the reference file:line it follows (paths relative to
-// /root/reference/).  f32/f64 usage and operation order are kept exactly as in
+// the CoverM source tree).  f32/f64 usage and operation order are kept exactly as in
 // the reference; compile with -ffp-contract=off.
 #pragma once
 #include <charconv>

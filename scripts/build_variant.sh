@@ -5,7 +5,7 @@ set -e
 cd "$(dirname "$0")/../coverm_b200/csrc"
 name=$1; shift
 mkdir -p ../../variants build
-nvcc -gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC $* -c cmb_device.cu -o build/cmb_device_$name.o
+nvcc -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC $* -c cmb_device.cu -o build/cmb_device_$name.o
 [ -f build/host_api.o ] || make build/host_api.o
-nvcc -gencode arch=compute_100a,code=sm_100a -shared -o ../../variants/$name.so build/cmb_device_$name.o build/host_api.o -lnccl -lz -lpthread
+nvcc -gencode arch=compute_90a,code=sm_90a -shared -o ../../variants/$name.so build/cmb_device_$name.o build/host_api.o -lnccl -lz -lpthread
 echo built variants/$name.so

@@ -1,9 +1,9 @@
 """Golden vectors transcribed from the reference's own tests (wwood/CoverM v0.8.0).
 
-Every case cites the reference test it restates (file:line under /root/reference/).
+Every case cites the reference test it restates (file:line in wwood/CoverM v0.8.0).
 The expected strings are the literal strings asserted there.  Inputs are the
-reference's fixtures (copied as data files into tests/golden/data/ by
-tests/golden/copy_fixtures.py; they are test inputs, not source code).
+reference's fixtures, stored as data files in tests/golden/data/ (they are test
+inputs, not source code).
 
 A case is a dict:
   ref      reference file:line
@@ -478,6 +478,3 @@ OWN_GFF_FIXTURES = {  # GFF statements of the gene sets genes.rs's unit tests co
 CLI_CASES = CLI_CASES + GENE_CASES
 
 ALL_CASES = CASES + FILTER_CASES + CLI_CASES
-
-# fixtures (under /root/reference/tests/data) the cases above read
-FIXTURES = sorted({a.split("/", 1)[1] for c in ALL_CASES for a in c["argv"] if a.startswith("{D}/")} - set(OWN_GFF_FIXTURES))

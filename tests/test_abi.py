@@ -40,9 +40,9 @@ def test_abi_version_and_struct_sizes(lib):
     assert ctypes.sizeof(coverm_b200.ReadBatch) == 8 + 13 * 8
 
 
-def test_kernels_are_sm_100a_with_tma(lib):
+def test_kernels_are_sm_90a_with_tma(lib):
     out = subprocess.run(["cuobjdump", "-sass", coverm_b200.LIB_PATH], capture_output=True, text=True).stdout
-    assert "sm_100a" in out
+    assert "sm_90a" in out
     assert "UTMALDG" in out, "K2 must stage its tiles with TMA (cp.async.bulk.tensor)"
     for k in ("k1_filter_accumulate", "k1b_local", "k1b_apply", "k2_scan_reduce", "k3_finalize", "kd_inflate", "kd_inflate_g8", "kd_guess", "kd_walk",
               "kd_extract"):

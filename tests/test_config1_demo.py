@@ -1,5 +1,5 @@
 """BASELINE.json configs[0] -- "coverm contig -m mean on demo/ BAM (8 genomes, sample_1), plumbing only".  The reference's demo
-directory ships reads and genomes but no BAM and no mapper is available here, so (SURVEY.md 8d) the BAM is synthesised over the
+directory ships reads and genomes but no BAM and no mapper is available here, so the BAM is synthesised over the
 demo's own 1472 reference sequences (names and lengths in tests/golden/demo_contigs.tsv, extracted from demo/genome_*.fna by the
 snippet in that file's commit) with 100 000 reads; the product's table must equal the oracle's: CLI -> decode -> device -> printer."""
 import os

@@ -1,5 +1,5 @@
 """The CPU oracle against every golden vector the reference's own tests hold for
-the coverage path (SURVEY.md §8c).  Runs without a GPU."""
+the coverage path.  Runs without a GPU."""
 import os
 
 import pytest
