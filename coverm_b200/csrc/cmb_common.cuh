@@ -2,27 +2,21 @@
 #pragma once
 
 
-#ifndef CMB_SPAN
-#define CMB_SPAN 32
-#endif
-constexpr uint32_t SPAN = CMB_SPAN;             // elements per thread span; contig alignment (16 or 32)
-constexpr uint32_t K2_THREADS = 8192 / SPAN;
+constexpr uint32_t SPAN = 32;                   // elements per K2 thread span = one 128-B tile row; contig alignment
+constexpr uint32_t K2_THREADS = 256;
 constexpr uint32_t CHUNK = SPAN * K2_THREADS;   // 8192 elements = 32 KB
 constexpr uint32_t CHUNK_BYTES = CHUNK * 4;
 constexpr uint32_t CHUNK_SPANS = K2_THREADS;    // spans per chunk
-constexpr uint32_t ROW_ELEMS = 32;              // TMA row: 32 x i32 = 128 B
+constexpr uint32_t ROW_ELEMS = SPAN;            // TMA row: 32 x i32 = 128 B
 constexpr uint32_t CHUNK_ROWS = CHUNK / ROW_ELEMS;  // 256
 #ifndef CMB_K2_STAGES
 #define CMB_K2_STAGES 2
 #endif
 constexpr uint32_t K2_STAGES = CMB_K2_STAGES;
-constexpr uint32_t K2_WARPS = K2_THREADS / 32;  // 16
-#ifndef CMB_K2_COOP
-#define CMB_K2_COOP 0  // K2 experiment: warp-cooperative handling of the non-empty spans (measured SLOWER: 2.85 vs 2.66 ms on config 2)
-#endif
-#ifndef CMB_K2_STATIC
-#define CMB_K2_STATIC 1  // K2: static chunk schedule, chunk metadata requested an iteration ahead (0 = dynamic tickets; 2.64 vs 2.69 ms)
-#endif
+constexpr uint32_t K2_WARPS = K2_THREADS / 32;  // 8 = span-bitmap words per chunk
+// Span occupancy bitmap: one bit per span (K1 sets it for every event it adds), so one u32 word per warp of K2 spans.
+constexpr uint32_t BITMAP_SPANS_PER_WORD = 32;
+constexpr uint32_t BITMAP_ELEMS_PER_WORD = BITMAP_SPANS_PER_WORD * SPAN;  // 1024
 #ifndef CMB_HIST_SLOTS
 #define CMB_HIST_SLOTS 8
 #endif
@@ -75,6 +69,17 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* tma
       "l"(reinterpret_cast<uint64_t>(tmap)), "r"(x), "r"(y), "r"(bar)
       : "memory");
 }
+
+// Order this thread's earlier generic-proxy shared-memory accesses (and, after a CTA barrier, every thread's) before a later
+// async-proxy (TMA) write to the same bytes.
+__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// cp.async: 16 B global -> shared, L2 only; completion tracked per thread by commit / wait groups.
+__device__ __forceinline__ void cp_async_16(uint32_t dst, const void* src) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(src) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
 
 __device__ __forceinline__ uint64_t warp_sum_u64(uint64_t v) {
 #pragma unroll

@@ -4,6 +4,9 @@
 //   arena        i32[arena_elems]   all contigs' `ups_and_downs` (contig.rs:144-145) back to back; every contig
 //                                   starts on a 32-element span boundary (SPAN), the arena is a whole number of
 //                                   8192-element chunks (CHUNK).  4 B per reference base.
+//   span_bits    u32[arena_elems/1024]  one bit per 32-element span: set by K1 for every event it adds, read (and, when
+//                                   cleaning as it goes, cleared) by K2, which loads only the spans named there.
+//                                   Zero exactly when the arena is (zeroed together; K2 cleans both).
 //   off_span     u32[n_local+1]     padded contig offsets in span units; len u32[n_local]
 //   chunk_first  u32[n_chunks+1]    contig containing the first span of each chunk
 //   tail_sum     i32[n_chunks]      K1: sum of the deltas of the contig that continues past the chunk end
@@ -16,8 +19,9 @@
 //                             (lib.rs:59-79, filter.rs:243-336), per-contig read counters (contig.rs:157-211),
 //                             +1/-1 delta REDs into the arena (contig.rs:166-202), chunk tail sums.
 //   K1b k1b_chunk_carry       segmented scan of the per-chunk tail sums -> carry_in (so K2 needs no look-back).
-//   K2  k2_scan_reduce        persistent CTAs, TMA (cp.async.bulk.tensor, 128B swizzle) + mbarrier ring of 32 KB
-//                             chunks, blocked 32-element spans per thread, warp-shuffle segmented scan, then every
+//   K2  k2_scan_reduce        persistent CTAs, ring of 32 KB chunks: whole-tile TMA (cp.async.bulk.tensor, 128B swizzle)
+//                             + mbarrier for chunks with many non-empty spans, cp.async of just the non-empty 128-B rows
+//                             for the others; blocked 32-element spans per thread, warp-shuffle segmented scan, then every
 //                             O(L) reduction of EST:366-502 in one pass: sum/covered over the end-trimmed window,
 //                             covered over the full contig, window depth histogram into a shared-memory table that
 //                             is flushed as (depth,count) records; optionally re-zeroes the arena as it goes.
@@ -140,12 +144,14 @@ struct cmb_ctx {
   uint64_t arena_elems = 0;
   uint32_t n_chunks = 0;
   int32_t* d_arena = nullptr;
+  uint32_t* d_span_bits = nullptr;
   uint32_t *d_off_span = nullptr, *d_len = nullptr, *d_chunk_first = nullptr;
   int32_t *d_tail_sum = nullptr, *d_carry_in = nullptr;
   int2* d_block_agg = nullptr;
   cmb_contig_stats* d_rows = nullptr;
-  uint32_t* d_counters = nullptr;  // [0] error flags, [1] ticket, [2] rec_count, [3] ovf_count, [4..5] pair_count (u64),
-                                   // [6..7] kept tid range of the exclusive records (K1Args::kept_range)
+  uint32_t* d_counters = nullptr;  // [0] error flags, [2] rec_count, [3] ovf_count, [4..5] pair_count (u64),
+                                   // [6..7] kept tid range of the exclusive records (K1Args::kept_range), [8..9] gene mode
+                                   // kept primaries (u64), [10..11] K2 spans loaded / chunks loaded whole
   uint32_t kept_range[2] = {0, 0};  // host copy after cmb_end_sample*
   // multi-GPU (cmb_comm_*): one NCCL communicator per ctx, collectives on the ctx stream
   ncclComm_t comm = nullptr;
@@ -304,6 +310,8 @@ void carve_batch(void* slab, uint32_t nr, uint32_t ni, cmb_read_batch* b) {
 
 void free_reference(cmb_ctx* c) {
   cudaFree(c->d_arena);
+  cudaFree(c->d_span_bits);
+  c->d_span_bits = nullptr;
   cudaFree(c->d_off_span);
   cudaFree(c->d_len);
   cudaFree(c->d_chunk_first);
@@ -366,7 +374,7 @@ int launch_k1(cmb_ctx* c, const cmb_read_batch& b, uint32_t n_records, uint32_t 
     a.gene_first = c->d_gene_first; a.gene_start = c->d_gene_start; a.gene_end = c->d_gene_end; a.gene_maxlen = c->d_gene_maxlen;
     a.contig_len = c->d_contig_len32; a.contig_seen = c->d_contig_seen; a.kept_primary = (unsigned long long*)(c->d_counters + 8);
   }
-  a.arena = c->d_arena; a.tail_sum = c->d_tail_sum; a.rows = c->d_rows;
+  a.arena = c->d_arena; a.span_bits = c->d_span_bits; a.tail_sum = c->d_tail_sum; a.rows = c->d_rows;
   a.block_minmax = c->d_block_minmax + c->block_minmax_used;
   a.error_flags = c->d_counters + 0;
   a.block_xrange = c->comm_size > 1 || excl_n != 0xffffffffu ? c->d_block_xrange + c->block_minmax_used : nullptr;
@@ -428,7 +436,7 @@ int run_end_of_sample(cmb_ctx* c) {
   K2Args a{};
   a.off_span = c->d_off_span; a.len = c->d_len; a.chunk_first = c->d_chunk_first; a.carry_in = c->d_carry_in;
   a.rows = c->d_rows; a.tid_begin = c->tid_begin; a.n_local = c->n_local; a.n_chunks = c->n_chunks; a.excl = excl;
-  a.ticket = c->d_counters + 1; a.arena = c->d_arena;
+  a.arena = c->d_arena; a.span_bits = c->d_span_bits; a.load_stats = c->d_counters + 10;
   a.rec = c->d_rec; a.rec_capacity = c->rec_capacity; a.rec_count = c->d_counters + 2;
   a.warp_table = c->d_warp_table; a.ovf = c->d_ovf; a.ovf_head = c->d_ovf_head; a.ovf_capacity = c->ovf_capacity; a.ovf_count = c->d_counters + 3;
   a.error_flags = c->d_counters + 0;
@@ -460,13 +468,16 @@ int run_end_of_sample(cmb_ctx* c) {
 }
 
 int collect_errors_and_timing(cmb_ctx* c, uint32_t* counters_out) {
-  uint32_t h[8];
+  uint32_t h[12];
   CU_TRY(c, cudaMemcpyAsync(h, c->d_counters, sizeof h, cudaMemcpyDeviceToHost, c->stream));
   CU_TRY(c, cudaEventRecord(c->ev[6], c->stream));
   CU_TRY(c, cudaStreamSynchronize(c->stream));
   memcpy(counters_out, h, 6 * sizeof(uint32_t));
   c->kept_range[0] = h[6];
   c->kept_range[1] = h[7];
+  if (c->n_local && getenv("CMB_PIPELINE_STATS"))  // what K2 fetched: 128 B per span loaded + 32 B of bitmap per chunk
+    fprintf(stderr, "#k2_load\tspans_loaded=%u\tspans=%llu\tdense_chunks=%u\tchunks=%u\n", h[10],
+            (unsigned long long)c->n_chunks * CHUNK_SPANS, h[11], c->n_chunks);
   float ms = 0;
   cudaEventElapsedTime(&ms, c->ev[0], c->ev[1]); c->timing.ms_zero = ms;
   cudaEventElapsedTime(&ms, c->ev[3], c->ev[4]); c->timing.ms_scan = ms;
@@ -706,6 +717,7 @@ int cmb_set_reference(cmb_ctx* c, uint32_t n_contigs, const uint64_t* contig_len
     return CMB_OK;
   }
   CU_TRY(c, cudaMalloc(&c->d_arena, c->arena_elems * 4));
+  CU_TRY(c, cudaMalloc(&c->d_span_bits, c->arena_elems / BITMAP_ELEMS_PER_WORD * 4));
   CU_TRY(c, cudaMalloc(&c->d_off_span, 4ull * (c->n_local + 1)));
   CU_TRY(c, cudaMalloc(&c->d_len, 4ull * c->n_local));
   CU_TRY(c, cudaMalloc(&c->d_chunk_first, 4ull * (c->n_chunks + 1)));
@@ -773,7 +785,10 @@ int cmb_begin_sample(cmb_ctx* c) {
   c->n_records = c->n_intervals = 0;
   CU_TRY(c, cudaEventRecord(c->ev[0], c->stream));
   if (c->n_local) {
-    if (c->arena_dirty) CU_TRY(c, cudaMemsetAsync(c->d_arena, 0, c->arena_elems * 4, c->stream));
+    if (c->arena_dirty) {
+      CU_TRY(c, cudaMemsetAsync(c->d_arena, 0, c->arena_elems * 4, c->stream));
+      CU_TRY(c, cudaMemsetAsync(c->d_span_bits, 0, c->arena_elems / BITMAP_ELEMS_PER_WORD * 4, c->stream));
+    }
     CU_TRY(c, cudaMemsetAsync(c->d_tail_sum, 0, 4ull * c->n_chunks, c->stream));
   }
   CU_TRY(c, cudaMemsetAsync(c->d_rows, 0, sizeof(cmb_contig_stats) * (size_t)c->n_contigs, c->stream));

@@ -1,6 +1,7 @@
 #!/bin/bash
 # Build a kernel variant of libcoverm_b200.so into variants/<name>.so (for A/B runs: bench.py --lib variants/<name>.so).
 #   scripts/build_variant.sh <name> "<extra nvcc -D flags>"
+# Flags: CMB_K2_STAGES, CMB_K2_MINBLOCKS, CMB_K2_DENSE_SPANS, CMB_HIST_SLOTS, CMB_K1_PREFETCH, CMB_K1_MINBLOCKS.
 set -e
 cd "$(dirname "$0")/../coverm_b200/csrc"
 name=$1; shift
