@@ -18,7 +18,11 @@ CMBH_MAX_SAMPLES = 64
 
 
 class CmbError(RuntimeError):
-    pass
+    """A failed cmb_* / cmbh_* call; `code` is the negative CMB_E_* value when the call returned one."""
+
+    def __init__(self, msg, code=None):
+        super().__init__(msg)
+        self.code = code
 
 
 # ---------------------------------------------------------------------------------------------- device ABI structs
@@ -57,6 +61,14 @@ class ContigStats(C.Structure):
                 ("trim_min_index", C.c_uint64), ("trim_max_index", C.c_uint64), ("var_k", C.c_uint64),
                 ("var_ex", C.c_uint64), ("var_ex2", C.c_uint64), ("hist_offset", C.c_uint64),
                 ("hist_count", C.c_uint32), ("reserved", C.c_uint32)]
+
+
+class HistPair(C.Structure):
+    _fields_ = [("depth", C.c_uint32), ("count", C.c_uint32)]
+
+
+class Gene(C.Structure):
+    _fields_ = [("tid", C.c_uint32), ("start", C.c_uint32), ("end", C.c_uint32)]
 
 
 class SampleTiming(C.Structure):
@@ -174,6 +186,8 @@ def load_library(path=None):
     lib.cmb_submit_device_batch.argtypes = [C.c_void_p, C.POINTER(ReadBatch), C.c_uint32, C.c_uint32]
     lib.cmb_end_sample.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]
     lib.cmb_fetch_pairs.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64]
+    lib.cmb_set_genes.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(C.c_uint64), C.c_uint32, C.POINTER(Gene)]
+    lib.cmb_fetch_gene_extras.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64)]
     lib.cmb_end_sample_device.argtypes = [C.c_void_p, C.POINTER(C.c_void_p)]
     lib.cmb_get_timing.argtypes = [C.c_void_p, C.POINTER(SampleTiming)]
     lib.cmb_stream.argtypes = [C.c_void_p]
@@ -330,6 +344,7 @@ class DeviceContext:
         self._h = C.c_void_p()
         self._owned = borrowed is None
         self.n_contigs = 0
+        self.n_ref_contigs = 0
         if borrowed is not None:  # a cmb_ctx* owned by someone else (Session.device_context())
             self._h = C.c_void_p(borrowed)
             return
@@ -346,7 +361,7 @@ class DeviceContext:
 
     def _check(self, rc, what):
         if rc != 0:
-            raise CmbError(f"{what} failed ({rc}): " + self._lib.cmb_last_error(self._h).decode())
+            raise CmbError(f"{what} failed ({rc}): " + self._lib.cmb_last_error(self._h).decode(), rc)
 
     def set_reference(self, lens, tid_begin=0, tid_end=None):
         import numpy as np
@@ -355,6 +370,25 @@ class DeviceContext:
         tid_end = self.n_contigs if tid_end is None else tid_end
         self._check(self._lib.cmb_set_reference(self._h, self.n_contigs, lens.ctypes.data_as(C.POINTER(C.c_uint64)),
                                                 tid_begin, tid_end), "cmb_set_reference")
+
+    def set_genes(self, contig_lens, genes):
+        """Per-gene segments instead of contigs (cmb_set_genes): `genes` is a sequence of (tid, start, end) sorted by
+        (tid, start).  Result rows are then one per gene (one placeholder row when there are none)."""
+        import numpy as np
+        lens = np.ascontiguousarray(contig_lens, dtype=np.uint64)
+        arr = (Gene * max(1, len(genes)))(*[Gene(*g) for g in genes])
+        self._check(self._lib.cmb_set_genes(self._h, len(lens), lens.ctypes.data_as(C.POINTER(C.c_uint64)), len(genes), arr),
+                    "cmb_set_genes")
+        self.n_contigs = max(1, len(genes))
+        self.n_ref_contigs = len(lens)
+
+    def fetch_gene_extras(self):
+        """After end_sample in gene mode: (contig_seen as a uint8 array, kept primary records) (cmb_fetch_gene_extras)."""
+        import numpy as np
+        seen = np.zeros(max(1, self.n_ref_contigs), dtype=np.uint8)
+        kept = C.c_uint64()
+        self._check(self._lib.cmb_fetch_gene_extras(self._h, seen.ctypes.data, C.byref(kept)), "cmb_fetch_gene_extras")
+        return seen[:self.n_ref_contigs], kept.value
 
     def set_params(self, params):
         mode = FilterMode()
@@ -376,6 +410,38 @@ class DeviceContext:
     def submit_batch(self, n_records, n_intervals):
         self._check(self._lib.cmb_submit_batch(self._h, n_records, n_intervals), "cmb_submit_batch")
 
+    _RECORD_COLUMNS = [("tid", C.c_int32), ("pos", C.c_int32), ("flag", C.c_uint16), ("mapq", C.c_uint8),
+                       ("nm_state", C.c_uint8), ("nm", C.c_uint32), ("l_seq", C.c_uint32), ("aligned", C.c_uint32),
+                       ("del_", C.c_uint32), ("ins", C.c_uint32)]
+
+    def submit_columns(self, cols):
+        """Copy host columns into the pinned batches of acquire_batch() and submit them, in as many batches as their
+        capacity needs.  `cols` maps the cmb_read_batch field names (``del_`` for del) to array-likes; `iv_begin` has
+        n_records + 1 entries and indexes `iv_start` / `iv_len`."""
+        import numpy as np
+
+        def put(ptr, ctype, values):
+            if len(values):
+                np.ctypeslib.as_array(C.cast(ptr, C.POINTER(ctype)), (len(values),))[:] = values
+
+        n = len(cols["tid"])
+        ivb = np.asarray(cols["iv_begin"], dtype=np.int64)
+        r0 = 0
+        while r0 < n:
+            b = self.acquire_batch()
+            # as many records as fit both the record and the interval capacity of the batch
+            r1 = min(n, r0 + b.capacity_records, int(np.searchsorted(ivb, ivb[r0] + b.capacity_intervals, "right")) - 1)
+            if r1 <= r0:
+                raise CmbError(f"record {r0} has more intervals than a staging batch holds ({b.capacity_intervals})")
+            for name, ctype in self._RECORD_COLUMNS:
+                put(getattr(b, name), ctype, np.asarray(cols[name])[r0:r1])
+            i0, i1 = int(ivb[r0]), int(ivb[r1])
+            put(b.iv_begin, C.c_uint32, ivb[r0:r1 + 1] - i0)  # iv_begin[n] = n_intervals
+            put(b.iv_start, C.c_int32, np.asarray(cols["iv_start"])[i0:i1])
+            put(b.iv_len, C.c_int32, np.asarray(cols["iv_len"])[i0:i1])
+            self.submit_batch(r1 - r0, i1 - i0)
+            r0 = r1
+
     def end_sample_device(self):
         p = C.c_void_p()
         self._check(self._lib.cmb_end_sample_device(self._h, C.byref(p)), "cmb_end_sample_device")
@@ -386,12 +452,19 @@ class DeviceContext:
         cuts = (C.c_uint32 * len(tid_cuts))(*tid_cuts)
         self._check(self._lib.cmb_allgather_stats(self._h, cuts, None, None, None), "cmb_allgather_stats")
 
-    def end_sample(self):
+    def end_sample(self, want_pairs=False):
+        """(rows, number of CSR histogram pairs); with want_pairs (rows, pairs), the pairs fetched with cmb_fetch_pairs as a
+        HistPair array (row r's are pairs[hist_offset : hist_offset + hist_count])."""
         import numpy as np
         rows = np.zeros(self.n_contigs, dtype=np.dtype(ContigStats))
         n_pairs = C.c_uint64()
         self._check(self._lib.cmb_end_sample(self._h, rows.ctypes.data, None, 0, C.byref(n_pairs)), "cmb_end_sample")
-        return rows, n_pairs.value
+        if not want_pairs:
+            return rows, n_pairs.value
+        pairs = np.zeros(n_pairs.value, dtype=np.dtype(HistPair))
+        if n_pairs.value:
+            self._check(self._lib.cmb_fetch_pairs(self._h, pairs.ctypes.data, n_pairs.value), "cmb_fetch_pairs")
+        return rows, pairs
 
     def timing(self):
         t = SampleTiming()
