@@ -58,15 +58,8 @@
 // NVTX ranges around the entry points and the stages of the device decode (visible in Nsight Systems / `ncu --nvtx`; no-ops
 // without a tool attached: nvtx3 is header-only and resolves its injection library lazily).
 struct NvtxRange {
-  bool open = true;
   explicit NvtxRange(const char* name) { nvtxRangePushA(name); }
-  void end() {
-    if (open) {
-      nvtxRangePop();
-      open = false;
-    }
-  }
-  ~NvtxRange() { end(); }
+  ~NvtxRange() { nvtxRangePop(); }
   NvtxRange(const NvtxRange&) = delete;
   NvtxRange& operator=(const NvtxRange&) = delete;
 };
@@ -118,8 +111,46 @@ struct LocalBarrier {
   }
 };
 
+// The owner of one device allocation (PINNED: pinned host memory) of `cap` elements of T; it is freed with its owner.
+// ensure() only grows and does not keep the contents; the caller decides how much to allocate when it has to grow.
+template <class T, bool PINNED = false>
+struct Buf {
+  T* p = nullptr;
+  size_t cap = 0;
+  Buf() = default;
+  Buf(Buf&& o) noexcept : p(o.p), cap(o.cap) {
+    o.p = nullptr;
+    o.cap = 0;
+  }
+  Buf& operator=(Buf&& o) noexcept {
+    if (this != &o) {
+      release();
+      std::swap(p, o.p);
+      std::swap(cap, o.cap);
+    }
+    return *this;
+  }
+  ~Buf() { release(); }
+  operator T*() const { return p; }
+  void release() {
+    if (p) {
+      if (PINNED) cudaFreeHost(p);
+      else cudaFree(p);
+    }
+    p = nullptr;
+    cap = 0;
+  }
+  // room for `need` elements: allocates `alloc` (>= need) when there is less
+  int ensure(cmb_ctx* c, size_t need, size_t alloc);
+  int ensure(cmb_ctx* c, size_t n) { return ensure(c, n, n); }
+  // n elements, keeping the first `used` (copied on `st`, which is synchronised before the old allocation is freed)
+  int grow_keep(cmb_ctx* c, size_t used, size_t n, cudaStream_t st);
+};
+template <class T>
+using PinnedBuf = Buf<T, true>;
+
 struct DevBatch {  // device mirror of one staging batch
-  void* slab = nullptr;
+  Buf<uint8_t> slab;
   cmb_read_batch ptr{};
 };
 
@@ -132,7 +163,7 @@ struct cmb_ctx {
   cmb_device_cfg cfg{};
   int sm_count = 0;
   // staging
-  std::vector<void*> host_slab;
+  std::vector<PinnedBuf<uint8_t>> host_slab;
   std::vector<cmb_read_batch> host_batch;
   std::vector<DevBatch> dev_batch;
   std::vector<cudaEvent_t> batch_done;
@@ -143,41 +174,38 @@ struct cmb_ctx {
   uint32_t n_contigs = 0, tid_begin = 0, tid_end = 0, n_local = 0;
   uint64_t arena_elems = 0;
   uint32_t n_chunks = 0;
-  int32_t* d_arena = nullptr;
-  uint32_t* d_span_bits = nullptr;
-  uint32_t *d_off_span = nullptr, *d_len = nullptr, *d_chunk_first = nullptr;
-  int32_t *d_tail_sum = nullptr, *d_carry_in = nullptr;
-  int2* d_block_agg = nullptr;
-  cmb_contig_stats* d_rows = nullptr;
-  uint32_t* d_counters = nullptr;  // [0] error flags, [2] rec_count, [3] ovf_count, [4..5] pair_count (u64),
-                                   // [6..7] kept tid range of the exclusive records (K1Args::kept_range), [8..9] gene mode
-                                   // kept primaries (u64), [10..11] K2 spans loaded / chunks loaded whole
+  struct Reference {  // the buffers that live as long as one reference (cmb_set_reference / cmb_set_genes)
+    Buf<int32_t> d_arena;
+    Buf<uint32_t> d_span_bits;
+    Buf<uint32_t> d_off_span, d_len, d_chunk_first;
+    Buf<int32_t> d_tail_sum, d_carry_in;
+    Buf<int2> d_block_agg;
+    Buf<cmb_contig_stats> d_rows;
+    Buf<uint2> d_rec;  // K2 -> K3 histogram records; cap is the capacity K2 is given
+    Buf<uint2> d_warp_table;
+    Buf<uint4> d_ovf;
+    Buf<uint32_t> d_ovf_head;
+    Buf<cmb_hist_pair> d_pairs;  // CSR histogram pairs (CMB_WANT_HIST_CSR)
+    // gene mode (cmb_set_genes): segments are genes; records carry contig tids
+    Buf<uint32_t> d_gene_first, d_gene_start, d_gene_end, d_gene_maxlen, d_contig_len32;
+    Buf<uint8_t> d_contig_seen;
+  } ref;
+  Buf<uint32_t> d_counters;  // 16 words: [0] error flags, [2] rec_count, [3] ovf_count, [4..5] pair_count (u64),
+                             // [6..7] kept tid range of the exclusive records (K1Args::kept_range), [8..9] gene mode
+                             // kept primaries (u64), [10..11] K2 spans loaded / chunks loaded whole
   uint32_t kept_range[2] = {0, 0};  // host copy after cmb_end_sample*
   // multi-GPU (cmb_comm_*): one NCCL communicator per ctx, collectives on the ctx stream
   ncclComm_t comm = nullptr;
   int comm_rank = 0, comm_size = 1;
   std::shared_ptr<LocalBarrier> local_barrier;  // set when all ranks of the communicator live in this process
-  uint8_t* d_xchg = nullptr;  // staging of cmb_comm_allgather
-  size_t xchg_cap = 0;
-  cmb_hist_pair* d_pairs_all = nullptr;  // concatenated histogram pairs of all ranks (cmb_allgather_stats)
-  uint64_t pairs_all_capacity = 0;
-  uint2* d_rec = nullptr;
-  uint32_t rec_capacity = 0;
-  uint2* d_warp_table = nullptr;
-  uint4* d_ovf = nullptr;
-  uint32_t* d_ovf_head = nullptr;
-  uint32_t ovf_capacity = 0;
-  cmb_hist_pair* d_pairs = nullptr;
-  uint64_t pair_capacity = 0;
-  int2* d_block_minmax = nullptr;
-  int2* d_block_xrange = nullptr;  // same capacity as d_block_minmax
+  Buf<uint8_t> d_xchg;  // staging of cmb_comm_allgather
+  Buf<cmb_hist_pair> d_pairs_all;  // concatenated histogram pairs of all ranks (cmb_allgather_stats)
+  Buf<int2> d_block_minmax;
+  Buf<int2> d_block_xrange;  // same capacity as d_block_minmax
   bool have_xrange = false;
-  uint32_t block_minmax_capacity = 0, block_minmax_used = 0;
-  // gene mode (cmb_set_genes): segments are genes; records carry contig tids
+  uint32_t block_minmax_used = 0;
   bool gene_mode = false;
   uint32_t n_ref_contigs = 0;  // contigs of the BAM header (== n_contigs outside gene mode)
-  uint32_t *d_gene_first = nullptr, *d_gene_start = nullptr, *d_gene_end = nullptr, *d_gene_maxlen = nullptr, *d_contig_len32 = nullptr;
-  uint8_t* d_contig_seen = nullptr;
   CUtensorMap tmap{};
   bool arena_dirty = true;
   bool clean_as_you_go = true;
@@ -193,51 +221,37 @@ struct cmb_ctx {
   uint64_t n_records = 0, n_intervals = 0;
   // device-side decode (cmb_submit_bgzf); every buffer is grow-only and reused across samples
   struct Decode {
-    uint8_t* d_comp = nullptr;
-    size_t comp_cap = 0;
-    uint8_t* d_inflated = nullptr;
-    size_t infl_cap = 0;
-    uint64_t *d_coff = nullptr, *d_ustart = nullptr, *d_guess = nullptr, *d_exit = nullptr, *d_rec_base = nullptr, *d_cig_base = nullptr;
-    uint32_t *d_clen = nullptr, *d_isize = nullptr, *d_status = nullptr, *d_nrec = nullptr, *d_ncig = nullptr, *d_dirty = nullptr;
-    size_t blocks_cap = 0;
-    uint8_t* d_t1_scratch = nullptr;  // kd_inflate_t1: code-length scratch, 160 B per block
-    uint32_t* d_tickets = nullptr;  // [0] block ticket, [1 + w] window w has arrived
-    size_t tickets_cap = 0;
-    uint32_t* d_block_window = nullptr;
-    size_t block_window_cap = 0;
-    uint32_t* h_ones = nullptr;  // pinned source of the arrival flags
-    uint32_t* d_cnt = nullptr;  // [0] inflate failures [1] decode error bits [2] chain changed [4..5] n_primary [6..9] totals
-    uint64_t* d_rec_off = nullptr;
-    size_t rec_cap = 0;
-    void* d_tuple_slab = nullptr;
-    size_t tuple_slab_bytes = 0;
+    Buf<uint8_t> d_comp, d_inflated;
+    // per BGZF block
+    Buf<uint64_t> d_coff, d_ustart, d_guess, d_exit, d_rec_base, d_cig_base;
+    Buf<uint32_t> d_clen, d_isize, d_status, d_nrec, d_ncig, d_dirty;
+    Buf<uint8_t> d_t1_scratch;  // kd_inflate_t1: code-length scratch, T1_LENS_BYTES per block
+    Buf<uint32_t> d_tickets;  // [0] block ticket, [1 + w] window w has arrived
+    Buf<uint32_t> d_block_window;
+    PinnedBuf<uint32_t> h_ones;  // source of the arrival flags
+    Buf<uint32_t> d_cnt;  // 16 words: [0] inflate failures [1] decode error bits [2] chain changed [4..5] n_primary [6..9] totals
+    Buf<uint64_t> d_rec_off;
+    Buf<uint8_t> d_tuple_slab;
     uint32_t last_n_rec = 0, last_n_cig = 0;  // tuples of the last successful cmb_submit_bgzf (cmb_last_bgzf_batch)
     bool last_valid = false;
     // mate matching (cmb_pairs.cuh)
-    uint64_t* d_pair_key = nullptr;
-    int32_t* d_pair_mate = nullptr;
-    uint32_t* d_pair_next = nullptr;
-    size_t pair_rec_cap = 0;
-    unsigned long long* d_pair_tag = nullptr;
-    uint32_t* d_pair_head = nullptr;
-    size_t pair_table_cap = 0;
+    Buf<uint64_t> d_pair_key;
+    Buf<int32_t> d_pair_mate;
+    Buf<uint32_t> d_pair_next;
+    Buf<unsigned long long> d_pair_tag;
+    Buf<uint32_t> d_pair_head;
     const int32_t* last_mate = nullptr;
     uint32_t last_excl_n = 0xffffffffu;
     const uint8_t* last_infl_base = nullptr;  // biased base of the inflated stream of the last decode
     // coverm filter
-    unsigned long long* d_filter_anchor = nullptr;
-    uint8_t* d_filter_role = nullptr;
-    size_t filter_rec_cap = 0;
-    uint8_t* d_filter_out = nullptr;
-    size_t filter_out_cap = 0;
+    Buf<unsigned long long> d_filter_anchor;
+    Buf<uint8_t> d_filter_role;
+    Buf<uint8_t> d_filter_out;
     uint64_t filter_bytes = 0;
     bool filter_planned = false;
-    std::vector<void*> pinned;
+    std::vector<PinnedBuf<uint8_t>> pinned;  // two copy slots per copy stream
     std::vector<cudaStream_t> streams;
     std::vector<cudaEvent_t> slot_events, done_events;
-    std::vector<cudaStream_t> cstreams;      // per-window inflate launches (CMB_INFLATE=t1): kernels of different windows overlap
-    std::vector<cudaEvent_t> window_events;  // window w has been copied
-    std::vector<cudaEvent_t> cstream_done;
     cudaEvent_t ev[6]{};
     bool have_events = false;
   } dec;
@@ -262,6 +276,28 @@ int fail(cmb_ctx* ctx, int code, const char* fmt, ...) {
     if (e_ != cudaSuccess) return fail(ctx, e_ == cudaErrorMemoryAllocation ? CMB_E_NOMEM : CMB_E_CUDA,      \
                                        "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(e_), __FILE__, __LINE__); \
   } while (0)
+
+template <class T, bool PINNED>
+int Buf<T, PINNED>::ensure(cmb_ctx* c, size_t need, size_t alloc) {
+  if (p && cap >= need) return CMB_OK;
+  release();
+  if (PINNED) CU_TRY(c, cudaHostAlloc((void**)&p, sizeof(T) * alloc, cudaHostAllocDefault));
+  else CU_TRY(c, cudaMalloc((void**)&p, sizeof(T) * alloc));
+  cap = alloc;
+  return CMB_OK;
+}
+
+template <class T, bool PINNED>
+int Buf<T, PINNED>::grow_keep(cmb_ctx* c, size_t used, size_t n, cudaStream_t st) {
+  Buf b;
+  if (int rc = b.ensure(c, n)) return rc;
+  if (used) CU_TRY(c, cudaMemcpyAsync(b.p, p, sizeof(T) * used, cudaMemcpyDeviceToDevice, st));
+  CU_TRY(c, cudaStreamSynchronize(st));
+  *this = std::move(b);
+  return CMB_OK;
+}
+
+size_t with_slack(size_t n) { return n + n / 8 + 16; }  // grow-only buffers sized by the data
 
 size_t batch_slab_bytes(uint32_t nr, uint32_t ni, size_t* offs) {
   // column order: tid,pos,nm,l_seq,aligned,del,ins,iv_begin(nr+1),iv_start(ni),iv_len(ni),flag(u16),mapq(u8),nm_state(u8)
@@ -309,72 +345,33 @@ void carve_batch(void* slab, uint32_t nr, uint32_t ni, cmb_read_batch* b) {
 }
 
 void free_reference(cmb_ctx* c) {
-  cudaFree(c->d_arena);
-  cudaFree(c->d_span_bits);
-  c->d_span_bits = nullptr;
-  cudaFree(c->d_off_span);
-  cudaFree(c->d_len);
-  cudaFree(c->d_chunk_first);
-  cudaFree(c->d_tail_sum);
-  cudaFree(c->d_carry_in);
-  cudaFree(c->d_block_agg);
-  c->d_block_agg = nullptr;
-  cudaFree(c->d_rows);
-  cudaFree(c->d_rec);
-  cudaFree(c->d_warp_table);
-  cudaFree(c->d_ovf);
-  cudaFree(c->d_ovf_head);
-  c->d_ovf_head = nullptr;
-  cudaFree(c->d_pairs);
-  cudaFree(c->d_gene_first); cudaFree(c->d_gene_start); cudaFree(c->d_gene_end); cudaFree(c->d_gene_maxlen); cudaFree(c->d_contig_len32);
-  cudaFree(c->d_contig_seen);
-  c->d_gene_first = c->d_gene_start = c->d_gene_end = c->d_gene_maxlen = c->d_contig_len32 = nullptr;
-  c->d_contig_seen = nullptr;
+  c->ref = {};
   c->gene_mode = false;
-  c->d_arena = nullptr;
-  c->d_off_span = c->d_len = c->d_chunk_first = nullptr;
-  c->d_tail_sum = c->d_carry_in = nullptr;
-  c->d_rows = nullptr;
-  c->d_rec = nullptr;
-  c->d_warp_table = nullptr;
-  c->d_ovf = nullptr;
-  c->d_pairs = nullptr;
-  c->pair_capacity = 0;
 }
 
 int launch_k1(cmb_ctx* c, const cmb_read_batch& b, uint32_t n_records, uint32_t n_intervals, uint32_t excl_n = 0xffffffffu,
               const int32_t* mate = nullptr) {
   if (n_records == 0) return CMB_OK;
   const uint32_t blocks = (n_records + K1_THREADS - 1) / K1_THREADS;
-  if (c->block_minmax_used + blocks > c->block_minmax_capacity) {
-    // grow (rare): allocate a larger array and copy what is there
-    uint32_t ncap = std::max(c->block_minmax_capacity * 2, c->block_minmax_used + blocks + 4096);
-    int2 *nd = nullptr, *nx = nullptr;
-    CU_TRY(c, cudaMalloc(&nd, sizeof(int2) * (size_t)ncap));
-    CU_TRY(c, cudaMalloc(&nx, sizeof(int2) * (size_t)ncap));
-    if (c->block_minmax_used) {
-      CU_TRY(c, cudaMemcpyAsync(nd, c->d_block_minmax, sizeof(int2) * (size_t)c->block_minmax_used, cudaMemcpyDeviceToDevice, c->stream));
-      CU_TRY(c, cudaMemcpyAsync(nx, c->d_block_xrange, sizeof(int2) * (size_t)c->block_minmax_used, cudaMemcpyDeviceToDevice, c->stream));
-    }
-    CU_TRY(c, cudaStreamSynchronize(c->stream));
-    cudaFree(c->d_block_minmax);
-    cudaFree(c->d_block_xrange);
-    c->d_block_minmax = nd;
-    c->d_block_xrange = nx;
-    c->block_minmax_capacity = ncap;
+  if (c->block_minmax_used + blocks > c->d_block_minmax.cap) {
+    // grow (rare): allocate larger arrays and copy what is there
+    const size_t ncap = std::max<size_t>(c->d_block_minmax.cap * 2, c->block_minmax_used + blocks + 4096);
+    if (int rc = c->d_block_minmax.grow_keep(c, c->block_minmax_used, ncap, c->stream)) return rc;
+    if (int rc = c->d_block_xrange.grow_keep(c, c->block_minmax_used, ncap, c->stream)) return rc;
   }
+  const auto& r = c->ref;
   K1Args a{};
   a.tid = b.tid; a.pos = b.pos; a.flag = b.flag; a.mapq = b.mapq; a.nm_state = b.nm_state; a.nm = b.nm;
   a.l_seq = b.l_seq; a.aligned = b.aligned; a.del = b.del; a.ins = b.ins; a.iv_begin = b.iv_begin;
   a.iv_start = b.iv_start; a.iv_len = b.iv_len;
   a.n = n_records;
-  a.off_span = c->d_off_span; a.len = c->d_len;
+  a.off_span = r.d_off_span; a.len = r.d_len;
   a.n_contigs = c->gene_mode ? c->n_ref_contigs : c->n_contigs; a.tid_begin = c->tid_begin; a.tid_end = c->tid_end;
   if (c->gene_mode) {
-    a.gene_first = c->d_gene_first; a.gene_start = c->d_gene_start; a.gene_end = c->d_gene_end; a.gene_maxlen = c->d_gene_maxlen;
-    a.contig_len = c->d_contig_len32; a.contig_seen = c->d_contig_seen; a.kept_primary = (unsigned long long*)(c->d_counters + 8);
+    a.gene_first = r.d_gene_first; a.gene_start = r.d_gene_start; a.gene_end = r.d_gene_end; a.gene_maxlen = r.d_gene_maxlen;
+    a.contig_len = r.d_contig_len32; a.contig_seen = r.d_contig_seen; a.kept_primary = (unsigned long long*)(c->d_counters + 8);
   }
-  a.arena = c->d_arena; a.span_bits = c->d_span_bits; a.tail_sum = c->d_tail_sum; a.rows = c->d_rows;
+  a.arena = r.d_arena; a.span_bits = r.d_span_bits; a.tail_sum = r.d_tail_sum; a.rows = r.d_rows;
   a.block_minmax = c->d_block_minmax + c->block_minmax_used;
   a.error_flags = c->d_counters + 0;
   a.block_xrange = c->comm_size > 1 || excl_n != 0xffffffffu ? c->d_block_xrange + c->block_minmax_used : nullptr;
@@ -420,27 +417,28 @@ int run_end_of_sample(cmb_ctx* c) {
   const bool hist = c->params.want & (CMB_WANT_HIST | CMB_WANT_HIST_CSR);
   const bool csr = c->params.want & CMB_WANT_HIST_CSR;
   const uint32_t excl = (uint32_t)std::min<uint64_t>(c->params.contig_end_exclusion, 0x7fffffffu);
+  const auto& r = c->ref;
   CU_TRY(c, cudaEventRecord(c->ev[2], c->stream));
   if (c->block_minmax_used) {
     k1c_check_sorted<<<1, 1024, 0, c->stream>>>(c->d_block_minmax, c->block_minmax_used, c->d_counters + 0,
-                                                c->have_xrange ? c->d_block_xrange : nullptr, c->d_counters + 6);
+                                                c->have_xrange ? c->d_block_xrange.p : nullptr, c->d_counters + 6);
     CU_TRY(c, cudaGetLastError());
   }
   {
     const uint32_t blocks = (c->n_chunks + K1B_BLOCK - 1) / K1B_BLOCK;
-    k1b_local<<<blocks, K1B_THREADS, 0, c->stream>>>(c->d_tail_sum, c->d_chunk_first, c->d_off_span, c->n_chunks, c->d_carry_in, c->d_block_agg);
+    k1b_local<<<blocks, K1B_THREADS, 0, c->stream>>>(r.d_tail_sum, r.d_chunk_first, r.d_off_span, c->n_chunks, r.d_carry_in, r.d_block_agg);
     CU_TRY(c, cudaGetLastError());
-    k1b_apply<<<blocks, K1B_THREADS, 0, c->stream>>>(c->d_tail_sum, c->d_block_agg, c->n_chunks, c->d_carry_in);
+    k1b_apply<<<blocks, K1B_THREADS, 0, c->stream>>>(r.d_tail_sum, r.d_block_agg, c->n_chunks, r.d_carry_in);
     CU_TRY(c, cudaGetLastError());
   }
   K2Args a{};
-  a.off_span = c->d_off_span; a.len = c->d_len; a.chunk_first = c->d_chunk_first; a.carry_in = c->d_carry_in;
-  a.rows = c->d_rows; a.tid_begin = c->tid_begin; a.n_local = c->n_local; a.n_chunks = c->n_chunks; a.excl = excl;
-  a.arena = c->d_arena; a.span_bits = c->d_span_bits; a.load_stats = c->d_counters + 10;
-  a.rec = c->d_rec; a.rec_capacity = c->rec_capacity; a.rec_count = c->d_counters + 2;
-  a.warp_table = c->d_warp_table; a.ovf = c->d_ovf; a.ovf_head = c->d_ovf_head; a.ovf_capacity = c->ovf_capacity; a.ovf_count = c->d_counters + 3;
+  a.off_span = r.d_off_span; a.len = r.d_len; a.chunk_first = r.d_chunk_first; a.carry_in = r.d_carry_in;
+  a.rows = r.d_rows; a.tid_begin = c->tid_begin; a.n_local = c->n_local; a.n_chunks = c->n_chunks; a.excl = excl;
+  a.arena = r.d_arena; a.span_bits = r.d_span_bits; a.load_stats = c->d_counters + 10;
+  a.rec = r.d_rec; a.rec_capacity = (uint32_t)r.d_rec.cap; a.rec_count = c->d_counters + 2;
+  a.warp_table = r.d_warp_table; a.ovf = r.d_ovf; a.ovf_head = r.d_ovf_head; a.ovf_capacity = (uint32_t)r.d_ovf.cap; a.ovf_count = c->d_counters + 3;
   a.error_flags = c->d_counters + 0;
-  if (hist) CU_TRY(c, cudaMemsetAsync(c->d_ovf_head, 0xff, 4ull * c->n_chunks, c->stream));
+  if (hist) CU_TRY(c, cudaMemsetAsync(r.d_ovf_head, 0xff, 4ull * c->n_chunks, c->stream));
   CU_TRY(c, cudaEventRecord(c->ev[3], c->stream));
   int rc;
   if (hist) rc = c->clean_as_you_go ? launch_k2_variant<true, true>(c, a) : launch_k2_variant<true, false>(c, a);
@@ -451,12 +449,12 @@ int run_end_of_sample(cmb_ctx* c) {
   CU_TRY(c, cudaEventRecord(c->ev[4], c->stream));
   if (hist) {
     K3Args k{};
-    k.off_span = c->d_off_span; k.len = c->d_len; k.chunk_first = c->d_chunk_first; k.rows = c->d_rows;
+    k.off_span = r.d_off_span; k.len = r.d_len; k.chunk_first = r.d_chunk_first; k.rows = r.d_rows;
     k.tid_begin = c->tid_begin; k.n_local = c->n_local; k.excl = excl;
     k.trim_min = c->params.trim_min; k.trim_max = c->params.trim_max;
-    k.rec = c->d_rec; k.warp_table = c->d_warp_table; k.ovf = c->d_ovf; k.ovf_head = c->d_ovf_head;
-    k.ovf_capacity = c->ovf_capacity;
-    k.pairs = c->d_pairs; k.pair_count = (unsigned long long*)(c->d_counters + 4); k.pair_capacity = c->pair_capacity;
+    k.rec = r.d_rec; k.warp_table = r.d_warp_table; k.ovf = r.d_ovf; k.ovf_head = r.d_ovf_head;
+    k.ovf_capacity = (uint32_t)r.d_ovf.cap;
+    k.pairs = r.d_pairs; k.pair_count = (unsigned long long*)(c->d_counters + 4); k.pair_capacity = r.d_pairs.cap;
     k.want_csr = csr; k.all_rows = c->gene_mode ? 1u : 0u; k.error_flags = c->d_counters + 0;
     const uint32_t grid = (c->n_local + K3_WARPS - 1) / K3_WARPS;  // one warp per contig
     k3_finalize<<<grid, K3_THREADS, 0, c->stream>>>(k);
@@ -556,26 +554,25 @@ int cmb_create(const cmb_device_cfg* cfg, cmb_ctx** out) {
   size_t offs[13];
   const size_t slab = batch_slab_bytes(c->cfg.batch_records, c->cfg.batch_intervals, offs);
   for (uint32_t i = 0; i < c->cfg.n_staging; ++i) {
-    void* h = nullptr;
-    CREATE_TRY(cudaHostAlloc(&h, slab, cudaHostAllocDefault));
-    c->host_slab.push_back(h);
+    PinnedBuf<uint8_t> h;
+    if (int rc = h.ensure(c, slab)) return bail(rc);
     cmb_read_batch hb;
     carve_batch(h, c->cfg.batch_records, c->cfg.batch_intervals, &hb);
+    c->host_slab.push_back(std::move(h));
     c->host_batch.push_back(hb);
     DevBatch db;
-    CREATE_TRY(cudaMalloc(&db.slab, slab));
+    if (int rc = db.slab.ensure(c, slab)) return bail(rc);
     carve_batch(db.slab, c->cfg.batch_records, c->cfg.batch_intervals, &db.ptr);
-    c->dev_batch.push_back(db);
+    c->dev_batch.push_back(std::move(db));
     cudaEvent_t ev;
     CREATE_TRY(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
     c->batch_done.push_back(ev);
     c->batch_busy.push_back(false);
   }
-  CREATE_TRY(cudaMalloc(&c->d_counters, 64));
+  if (int rc = c->d_counters.ensure(c, 16)) return bail(rc);
   CREATE_TRY(cudaMemset(c->d_counters, 0, 64));
-  c->block_minmax_capacity = 1u << 16;
-  CREATE_TRY(cudaMalloc(&c->d_block_minmax, sizeof(int2) * (size_t)c->block_minmax_capacity));
-  CREATE_TRY(cudaMalloc(&c->d_block_xrange, sizeof(int2) * (size_t)c->block_minmax_capacity));
+  if (int rc = c->d_block_minmax.ensure(c, 1u << 16)) return bail(rc);
+  if (int rc = c->d_block_xrange.ensure(c, 1u << 16)) return bail(rc);
   const char* env = getenv("CMB_CLEAN_AS_YOU_GO");
   if (env && env[0] == '0') c->clean_as_you_go = false;
   *out = c;
@@ -586,9 +583,6 @@ void cmb_destroy(cmb_ctx* c) {
   if (!c) return;
   cudaSetDevice(c->device);
   if (c->stream) cudaStreamSynchronize(c->stream);
-  free_reference(c);
-  for (auto h : c->host_slab) cudaFreeHost(h);
-  for (auto& d : c->dev_batch) cudaFree(d.slab);
   for (auto e : c->batch_done) cudaEventDestroy(e);
   for (auto& e : c->k1_events) {
     cudaEventDestroy(e.first);
@@ -596,31 +590,17 @@ void cmb_destroy(cmb_ctx* c) {
   }
   for (auto e : c->ev)
     if (e) cudaEventDestroy(e);
-  cudaFree(c->d_counters);
-  cudaFree(c->d_block_minmax);
-  cudaFree(c->d_block_xrange);
   cmb_comm_destroy(c);
-  cudaFree(c->d_xchg);
-  cudaFree(c->d_pairs_all);
   {
     auto& d = c->dec;
-    cudaFree(d.d_comp); cudaFree(d.d_inflated); cudaFree(d.d_coff); cudaFree(d.d_ustart); cudaFree(d.d_guess); cudaFree(d.d_exit);
-    cudaFree(d.d_rec_base); cudaFree(d.d_cig_base); cudaFree(d.d_clen); cudaFree(d.d_isize); cudaFree(d.d_status); cudaFree(d.d_nrec);
-    cudaFree(d.d_filter_anchor); cudaFree(d.d_filter_role); cudaFree(d.d_filter_out);
-    cudaFree(d.d_pair_key); cudaFree(d.d_pair_mate); cudaFree(d.d_pair_next); cudaFree(d.d_pair_tag); cudaFree(d.d_pair_head);
-    cudaFree(d.d_ncig); cudaFree(d.d_dirty); cudaFree(d.d_tickets); cudaFree(d.d_t1_scratch); cudaFree(d.d_block_window); if (d.h_ones) cudaFreeHost(d.h_ones); cudaFree(d.d_cnt); cudaFree(d.d_rec_off); cudaFree(d.d_tuple_slab);
-    for (auto p : d.pinned) cudaFreeHost(p);
     for (auto st : d.streams) cudaStreamDestroy(st);
     for (auto e : d.slot_events) cudaEventDestroy(e);
     for (auto e : d.done_events) cudaEventDestroy(e);
-    for (auto st : d.cstreams) cudaStreamDestroy(st);
-    for (auto e : d.window_events) cudaEventDestroy(e);
-    for (auto e : d.cstream_done) cudaEventDestroy(e);
     if (d.have_events)
       for (auto e : d.ev) cudaEventDestroy(e);
   }
   if (c->stream) cudaStreamDestroy(c->stream);
-  delete c;
+  delete c;  // frees every buffer (the device is still current)
 }
 
 int cmb_set_genes(cmb_ctx* c, uint32_t n_contigs, const uint64_t* contig_len, uint32_t n_genes, const cmb_gene* genes) {
@@ -651,17 +631,16 @@ int cmb_set_genes(cmb_ctx* c, uint32_t n_contigs, const uint64_t* contig_len, ui
   if (rc) return rc;
   c->gene_mode = true;
   c->n_ref_contigs = n_contigs;
-  CU_TRY(c, cudaMalloc(&c->d_gene_first, 4ull * (n_contigs + 1)));
-  CU_TRY(c, cudaMalloc(&c->d_gene_start, 4ull * n_seg));
-  CU_TRY(c, cudaMalloc(&c->d_gene_end, 4ull * n_seg));
-  CU_TRY(c, cudaMalloc(&c->d_gene_maxlen, 4ull * std::max<uint32_t>(1, n_contigs)));
-  CU_TRY(c, cudaMalloc(&c->d_contig_len32, 4ull * std::max<uint32_t>(1, n_contigs)));
-  CU_TRY(c, cudaMalloc(&c->d_contig_seen, std::max<size_t>(1, n_contigs)));
-  CU_TRY(c, cudaMemcpyAsync(c->d_gene_first, first.data(), 4ull * (n_contigs + 1), cudaMemcpyHostToDevice, c->stream));
-  CU_TRY(c, cudaMemcpyAsync(c->d_gene_start, gs.data(), 4ull * n_seg, cudaMemcpyHostToDevice, c->stream));
-  CU_TRY(c, cudaMemcpyAsync(c->d_gene_end, ge.data(), 4ull * n_seg, cudaMemcpyHostToDevice, c->stream));
-  CU_TRY(c, cudaMemcpyAsync(c->d_gene_maxlen, maxlen.data(), 4ull * std::max<uint32_t>(1, n_contigs), cudaMemcpyHostToDevice, c->stream));
-  CU_TRY(c, cudaMemcpyAsync(c->d_contig_len32, clen.data(), 4ull * std::max<uint32_t>(1, n_contigs), cudaMemcpyHostToDevice, c->stream));
+  auto& r = c->ref;
+  const size_t n_ctg = std::max<uint32_t>(1, n_contigs);
+  if ((rc = r.d_gene_first.ensure(c, (size_t)n_contigs + 1)) || (rc = r.d_gene_start.ensure(c, n_seg)) || (rc = r.d_gene_end.ensure(c, n_seg)) ||
+      (rc = r.d_gene_maxlen.ensure(c, n_ctg)) || (rc = r.d_contig_len32.ensure(c, n_ctg)) || (rc = r.d_contig_seen.ensure(c, n_ctg)))
+    return rc;
+  CU_TRY(c, cudaMemcpyAsync(r.d_gene_first, first.data(), 4ull * (n_contigs + 1), cudaMemcpyHostToDevice, c->stream));
+  CU_TRY(c, cudaMemcpyAsync(r.d_gene_start, gs.data(), 4ull * n_seg, cudaMemcpyHostToDevice, c->stream));
+  CU_TRY(c, cudaMemcpyAsync(r.d_gene_end, ge.data(), 4ull * n_seg, cudaMemcpyHostToDevice, c->stream));
+  CU_TRY(c, cudaMemcpyAsync(r.d_gene_maxlen, maxlen.data(), 4 * n_ctg, cudaMemcpyHostToDevice, c->stream));
+  CU_TRY(c, cudaMemcpyAsync(r.d_contig_len32, clen.data(), 4 * n_ctg, cudaMemcpyHostToDevice, c->stream));
   CU_TRY(c, cudaStreamSynchronize(c->stream));
   return CMB_OK;
 }
@@ -671,7 +650,7 @@ int cmb_fetch_gene_extras(cmb_ctx* c, uint8_t* contig_seen, uint64_t* n_kept_pri
   if (!c->gene_mode || !c->ended) return fail(c, CMB_E_ARG, "cmb_fetch_gene_extras: no ended sample in gene mode");
   CU_TRY(c, cudaSetDevice(c->device));
   unsigned long long kp = 0;
-  if (c->n_ref_contigs) CU_TRY(c, cudaMemcpyAsync(contig_seen, c->d_contig_seen, c->n_ref_contigs, cudaMemcpyDeviceToHost, c->stream));
+  if (c->n_ref_contigs) CU_TRY(c, cudaMemcpyAsync(contig_seen, c->ref.d_contig_seen, c->n_ref_contigs, cudaMemcpyDeviceToHost, c->stream));
   CU_TRY(c, cudaMemcpyAsync(&kp, c->d_counters + 8, 8, cudaMemcpyDeviceToHost, c->stream));
   CU_TRY(c, cudaStreamSynchronize(c->stream));
   *n_kept_primary = kp;
@@ -712,34 +691,30 @@ int cmb_set_reference(cmb_ctx* c, uint32_t n_contigs, const uint64_t* contig_len
     }
     chunk_first[c->n_chunks] = c->n_local ? c->n_local - 1 : 0;
   }
-  if (c->n_local == 0) {  // empty shard: nothing to allocate beyond the rows
-    CU_TRY(c, cudaMalloc(&c->d_rows, sizeof(cmb_contig_stats) * std::max<size_t>(1, n_contigs)));
-    return CMB_OK;
-  }
-  CU_TRY(c, cudaMalloc(&c->d_arena, c->arena_elems * 4));
-  CU_TRY(c, cudaMalloc(&c->d_span_bits, c->arena_elems / BITMAP_ELEMS_PER_WORD * 4));
-  CU_TRY(c, cudaMalloc(&c->d_off_span, 4ull * (c->n_local + 1)));
-  CU_TRY(c, cudaMalloc(&c->d_len, 4ull * c->n_local));
-  CU_TRY(c, cudaMalloc(&c->d_chunk_first, 4ull * (c->n_chunks + 1)));
-  CU_TRY(c, cudaMalloc(&c->d_tail_sum, 4ull * c->n_chunks));
-  CU_TRY(c, cudaMalloc(&c->d_carry_in, 4ull * c->n_chunks));
-  CU_TRY(c, cudaMalloc(&c->d_block_agg, sizeof(int2) * ((size_t)c->n_chunks / K1B_BLOCK + 1)));
-  CU_TRY(c, cudaMalloc(&c->d_rows, sizeof(cmb_contig_stats) * (size_t)n_contigs));
-  CU_TRY(c, cudaMemcpyAsync(c->d_off_span, off_span.data(), 4ull * (c->n_local + 1), cudaMemcpyHostToDevice, c->stream));
-  CU_TRY(c, cudaMemcpyAsync(c->d_len, len.data(), 4ull * c->n_local, cudaMemcpyHostToDevice, c->stream));
-  CU_TRY(c, cudaMemcpyAsync(c->d_chunk_first, chunk_first.data(), 4ull * (c->n_chunks + 1), cudaMemcpyHostToDevice, c->stream));
+  auto& r = c->ref;
+  int rc;
+  if (c->n_local == 0)  // empty shard: nothing to allocate beyond the rows
+    return r.d_rows.ensure(c, std::max<size_t>(1, n_contigs));
+  if ((rc = r.d_arena.ensure(c, c->arena_elems)) || (rc = r.d_span_bits.ensure(c, c->arena_elems / BITMAP_ELEMS_PER_WORD)) ||
+      (rc = r.d_off_span.ensure(c, (size_t)c->n_local + 1)) || (rc = r.d_len.ensure(c, c->n_local)) ||
+      (rc = r.d_chunk_first.ensure(c, (size_t)c->n_chunks + 1)) || (rc = r.d_tail_sum.ensure(c, c->n_chunks)) ||
+      (rc = r.d_carry_in.ensure(c, c->n_chunks)) || (rc = r.d_block_agg.ensure(c, (size_t)c->n_chunks / K1B_BLOCK + 1)) ||
+      (rc = r.d_rows.ensure(c, n_contigs)))
+    return rc;
+  CU_TRY(c, cudaMemcpyAsync(r.d_off_span, off_span.data(), 4ull * (c->n_local + 1), cudaMemcpyHostToDevice, c->stream));
+  CU_TRY(c, cudaMemcpyAsync(r.d_len, len.data(), 4ull * c->n_local, cudaMemcpyHostToDevice, c->stream));
+  CU_TRY(c, cudaMemcpyAsync(r.d_chunk_first, chunk_first.data(), 4ull * (c->n_chunks + 1), cudaMemcpyHostToDevice, c->stream));
   CU_TRY(c, cudaStreamSynchronize(c->stream));
   // histogram record buffers: one 8 B record per 8 arena elements is far above anything a real sample produces
-  c->rec_capacity = (uint32_t)std::min<uint64_t>(0xfffffff0ull, std::max<uint64_t>(1u << 20, c->arena_elems / 8));
-  c->ovf_capacity = (uint32_t)std::min<uint64_t>(1u << 26, std::max<uint64_t>(1u << 20, c->arena_elems / 64));
+  uint64_t rec_cap = std::min<uint64_t>(0xfffffff0ull, std::max<uint64_t>(1u << 20, c->arena_elems / 8));
+  uint64_t ovf_cap = std::min<uint64_t>(1u << 26, std::max<uint64_t>(1u << 20, c->arena_elems / 64));
   if (getenv("CMB_TEST_SMALL_HIST")) {  // testing aid: buffers that overflow at once (cmb_grow_buffers path)
-    c->rec_capacity = 256;
-    c->ovf_capacity = 64;
+    rec_cap = 256;
+    ovf_cap = 64;
   }
-  CU_TRY(c, cudaMalloc(&c->d_rec, 8ull * c->rec_capacity));
-  CU_TRY(c, cudaMalloc(&c->d_warp_table, 8ull * c->n_chunks * HIST_SLOTS));
-  CU_TRY(c, cudaMalloc(&c->d_ovf, 16ull * c->ovf_capacity));
-  CU_TRY(c, cudaMalloc(&c->d_ovf_head, 4ull * c->n_chunks));
+  if ((rc = r.d_rec.ensure(c, rec_cap)) || (rc = r.d_warp_table.ensure(c, (size_t)c->n_chunks * HIST_SLOTS)) ||
+      (rc = r.d_ovf.ensure(c, ovf_cap)) || (rc = r.d_ovf_head.ensure(c, c->n_chunks)))
+    return rc;
   c->arena_dirty = true;
   // TMA descriptor: the arena as [rows][32] i32, box = one chunk (256 rows x 128 B), 128B swizzle
   PFN_encodeTiled encode = nullptr;
@@ -750,9 +725,9 @@ int cmb_set_reference(cmb_ctx* c, uint32_t n_contigs, const uint64_t* contig_len
   cuuint64_t gstride[1] = {ROW_ELEMS * 4};
   cuuint32_t box[2] = {ROW_ELEMS, CHUNK_ROWS};
   cuuint32_t estr[2] = {1, 1};
-  CUresult r = encode(&c->tmap, CU_TENSOR_MAP_DATA_TYPE_INT32, 2, c->d_arena, gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                      CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return fail(c, CMB_E_CUDA, "cuTensorMapEncodeTiled failed with CUresult %d", (int)r);
+  CUresult res = encode(&c->tmap, CU_TENSOR_MAP_DATA_TYPE_INT32, 2, r.d_arena.p, gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                        CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (res != CUDA_SUCCESS) return fail(c, CMB_E_CUDA, "cuTensorMapEncodeTiled failed with CUresult %d", (int)res);
   return CMB_OK;
 }
 
@@ -775,7 +750,7 @@ int cmb_set_params(cmb_ctx* c, const cmb_params* p, cmb_filter_mode* mode_out) {
 int cmb_begin_sample(cmb_ctx* c) {
   NvtxRange nvtx_fn("cmb_begin_sample");
   if (!c) return CMB_E_ARG;
-  if (!c->d_rows || !c->have_params) return fail(c, CMB_E_ARG, "cmb_begin_sample: set_reference and set_params first");
+  if (!c->ref.d_rows || !c->have_params) return fail(c, CMB_E_ARG, "cmb_begin_sample: set_reference and set_params first");
   if (c->in_sample) return fail(c, CMB_E_ARG, "cmb_begin_sample: previous sample not ended");
   CU_TRY(c, cudaSetDevice(c->device));
   c->timing = cmb_sample_timing{};
@@ -786,26 +761,20 @@ int cmb_begin_sample(cmb_ctx* c) {
   CU_TRY(c, cudaEventRecord(c->ev[0], c->stream));
   if (c->n_local) {
     if (c->arena_dirty) {
-      CU_TRY(c, cudaMemsetAsync(c->d_arena, 0, c->arena_elems * 4, c->stream));
-      CU_TRY(c, cudaMemsetAsync(c->d_span_bits, 0, c->arena_elems / BITMAP_ELEMS_PER_WORD * 4, c->stream));
+      CU_TRY(c, cudaMemsetAsync(c->ref.d_arena, 0, c->arena_elems * 4, c->stream));
+      CU_TRY(c, cudaMemsetAsync(c->ref.d_span_bits, 0, c->arena_elems / BITMAP_ELEMS_PER_WORD * 4, c->stream));
     }
-    CU_TRY(c, cudaMemsetAsync(c->d_tail_sum, 0, 4ull * c->n_chunks, c->stream));
+    CU_TRY(c, cudaMemsetAsync(c->ref.d_tail_sum, 0, 4ull * c->n_chunks, c->stream));
   }
-  CU_TRY(c, cudaMemsetAsync(c->d_rows, 0, sizeof(cmb_contig_stats) * (size_t)c->n_contigs, c->stream));
+  CU_TRY(c, cudaMemsetAsync(c->ref.d_rows, 0, sizeof(cmb_contig_stats) * (size_t)c->n_contigs, c->stream));
   CU_TRY(c, cudaMemsetAsync(c->d_counters, 0, 64, c->stream));
-  if (c->gene_mode) CU_TRY(c, cudaMemsetAsync(c->d_contig_seen, 0, std::max<size_t>(1, c->n_ref_contigs), c->stream));
+  if (c->gene_mode) CU_TRY(c, cudaMemsetAsync(c->ref.d_contig_seen, 0, std::max<size_t>(1, c->n_ref_contigs), c->stream));
   CU_TRY(c, cudaEventRecord(c->ev[1], c->stream));
   c->arena_dirty = true;  // until K2 has cleaned it
   if ((c->params.want & CMB_WANT_HIST_CSR) && c->n_local) {
     uint64_t want = std::max<uint64_t>(1u << 20, c->arena_elems / 16);
     if (getenv("CMB_TEST_SMALL_HIST")) want = 64;  // testing aid: start with buffers that overflow at once (cmb_grow_buffers path)
-    if (c->pair_capacity < want) {
-      cudaFree(c->d_pairs);
-      c->d_pairs = nullptr;
-      c->pair_capacity = 0;
-      CU_TRY(c, cudaMalloc(&c->d_pairs, sizeof(cmb_hist_pair) * want));
-      c->pair_capacity = want;
-    }
+    if (int rc = c->ref.d_pairs.ensure(c, want)) return rc;
   }
   c->in_sample = true;
   c->ended = false;
@@ -893,7 +862,7 @@ int cmb_end_sample_device(cmb_ctx* c, const cmb_contig_stats** dev_stats) {
   int rc = collect_errors_and_timing(c, counters);
   if (rc) return rc;
   c->ended = true;
-  if (dev_stats) *dev_stats = c->d_rows;
+  if (dev_stats) *dev_stats = c->ref.d_rows;
   return CMB_OK;
 }
 
@@ -902,17 +871,17 @@ int cmb_end_sample(cmb_ctx* c, cmb_contig_stats* stats, cmb_hist_pair* pairs, ui
   if (!c) return fail(c, CMB_E_ARG, "cmb_end_sample: null argument");
   int rc = cmb_end_sample_device(c, nullptr);
   if (rc) return rc;
-  if (stats) CU_TRY(c, cudaMemcpyAsync(stats, c->d_rows, sizeof(cmb_contig_stats) * (size_t)c->n_contigs, cudaMemcpyDeviceToHost, c->stream));
+  if (stats) CU_TRY(c, cudaMemcpyAsync(stats, c->ref.d_rows, sizeof(cmb_contig_stats) * (size_t)c->n_contigs, cudaMemcpyDeviceToHost, c->stream));
   uint64_t np = 0;
   if ((c->params.want & CMB_WANT_HIST_CSR) && c->n_local) {
     unsigned long long cnt = 0;
     CU_TRY(c, cudaMemcpyAsync(&cnt, c->d_counters + 4, 8, cudaMemcpyDeviceToHost, c->stream));
     CU_TRY(c, cudaStreamSynchronize(c->stream));
     np = cnt;
-    if (np > c->pair_capacity) return fail(c, CMB_E_CAPACITY, "device histogram pair buffer overflowed");
+    if (np > c->ref.d_pairs.cap) return fail(c, CMB_E_CAPACITY, "device histogram pair buffer overflowed");
     if (pairs) {
       if (np > pairs_capacity) return fail(c, CMB_E_CAPACITY, "cmb_end_sample: caller's pair buffer too small (%llu needed)", (unsigned long long)np);
-      if (np) CU_TRY(c, cudaMemcpyAsync(pairs, c->d_pairs, sizeof(cmb_hist_pair) * np, cudaMemcpyDeviceToHost, c->stream));
+      if (np) CU_TRY(c, cudaMemcpyAsync(pairs, c->ref.d_pairs, sizeof(cmb_hist_pair) * np, cudaMemcpyDeviceToHost, c->stream));
     }
   }
   CU_TRY(c, cudaStreamSynchronize(c->stream));
@@ -923,39 +892,27 @@ int cmb_end_sample(cmb_ctx* c, cmb_contig_stats* stats, cmb_hist_pair* pairs, ui
 int cmb_fetch_pairs(cmb_ctx* c, cmb_hist_pair* pairs, uint64_t n_pairs) {
   if (!c || (!pairs && n_pairs)) return fail(c, CMB_E_ARG, "cmb_fetch_pairs: null argument");
   if (!c->ended) return fail(c, CMB_E_ARG, "cmb_fetch_pairs: no ended sample");
-  if (n_pairs > c->pair_capacity) return fail(c, CMB_E_ARG, "cmb_fetch_pairs: more pairs requested than produced");
+  if (n_pairs > c->ref.d_pairs.cap) return fail(c, CMB_E_ARG, "cmb_fetch_pairs: more pairs requested than produced");
   if (n_pairs) {
     CU_TRY(c, cudaSetDevice(c->device));
-    CU_TRY(c, cudaMemcpyAsync(pairs, c->d_pairs, sizeof(cmb_hist_pair) * n_pairs, cudaMemcpyDeviceToHost, c->stream));
+    CU_TRY(c, cudaMemcpyAsync(pairs, c->ref.d_pairs, sizeof(cmb_hist_pair) * n_pairs, cudaMemcpyDeviceToHost, c->stream));
     CU_TRY(c, cudaStreamSynchronize(c->stream));
   }
   return CMB_OK;
 }
 
 int cmb_grow_buffers(cmb_ctx* c) {
-  if (!c || !c->d_rows) return fail(c, CMB_E_ARG, "cmb_grow_buffers: no reference set");
+  if (!c || !c->ref.d_rows) return fail(c, CMB_E_ARG, "cmb_grow_buffers: no reference set");
   if (c->in_sample) return fail(c, CMB_E_ARG, "cmb_grow_buffers: a sample is in progress");
   if (c->n_local == 0) return CMB_OK;
   CU_TRY(c, cudaSetDevice(c->device));
   CU_TRY(c, cudaStreamSynchronize(c->stream));
-  const uint64_t rec = std::min<uint64_t>(0xfffffff0ull, (uint64_t)c->rec_capacity * 4);
-  const uint64_t ovf = std::min<uint64_t>(1ull << 30, (uint64_t)c->ovf_capacity * 4);
-  cudaFree(c->d_rec);
-  cudaFree(c->d_ovf);
-  c->d_rec = nullptr;
-  c->d_ovf = nullptr;
-  CU_TRY(c, cudaMalloc(&c->d_rec, 8ull * rec));
-  CU_TRY(c, cudaMalloc(&c->d_ovf, 16ull * ovf));
-  c->rec_capacity = (uint32_t)rec;
-  c->ovf_capacity = (uint32_t)ovf;
-  if (c->d_pairs) {
-    const uint64_t want = c->pair_capacity * 4;
-    cudaFree(c->d_pairs);
-    c->d_pairs = nullptr;
-    c->pair_capacity = 0;
-    CU_TRY(c, cudaMalloc(&c->d_pairs, sizeof(cmb_hist_pair) * want));
-    c->pair_capacity = want;
-  }
+  auto& r = c->ref;  // the next sample rebuilds what these hold
+  int rc;
+  if ((rc = r.d_rec.ensure(c, std::min<uint64_t>(0xfffffff0ull, (uint64_t)r.d_rec.cap * 4))) ||
+      (rc = r.d_ovf.ensure(c, std::min<uint64_t>(1ull << 30, (uint64_t)r.d_ovf.cap * 4))) ||
+      (r.d_pairs && (rc = r.d_pairs.ensure(c, r.d_pairs.cap * 4))))
+    return rc;
   c->arena_dirty = true;
   return CMB_OK;
 }
@@ -1078,13 +1035,7 @@ int cmb_comm_allgather(cmb_ctx* c, const void* send, void* recv, size_t bytes) {
   if (!c->comm) return fail(c, CMB_E_ARG, "cmb_comm_allgather: no communicator (cmb_comm_init first)");
   CU_TRY(c, cudaSetDevice(c->device));
   const size_t need = bytes * (size_t)(c->comm_size + 1);
-  if (c->xchg_cap < need) {
-    cudaFree(c->d_xchg);
-    c->d_xchg = nullptr;
-    c->xchg_cap = 0;
-    CU_TRY(c, cudaMalloc(&c->d_xchg, need + 4096));
-    c->xchg_cap = need + 4096;
-  }
+  if (int rc = c->d_xchg.ensure(c, need, need + 4096)) return rc;
   uint8_t* d_send = c->d_xchg;
   uint8_t* d_recv = c->d_xchg + bytes;
   if (c->local_barrier) c->local_barrier->arrive_and_wait();
@@ -1099,7 +1050,7 @@ int cmb_allgather_stats(cmb_ctx* c, const uint32_t* tid_cuts, const uint64_t* pa
   NvtxRange nvtx_fn("cmb_allgather_stats: NCCL gather");
   if (!c || !tid_cuts) return fail(c, CMB_E_ARG, "cmb_allgather_stats: null argument");
   if (!c->comm) return fail(c, CMB_E_ARG, "cmb_allgather_stats: no communicator (cmb_comm_init first)");
-  if (!c->ended || !c->d_rows) return fail(c, CMB_E_ARG, "cmb_allgather_stats: no ended sample");
+  if (!c->ended || !c->ref.d_rows) return fail(c, CMB_E_ARG, "cmb_allgather_stats: no ended sample");
   const int N = c->comm_size, me = c->comm_rank;
   if (tid_cuts[0] != 0 || tid_cuts[N] != c->n_contigs || tid_cuts[me] != c->tid_begin || tid_cuts[me + 1] != c->tid_end)
     return fail(c, CMB_E_ARG, "cmb_allgather_stats: tid_cuts do not match this context's shard");
@@ -1109,18 +1060,11 @@ int cmb_allgather_stats(cmb_ctx* c, const uint32_t* tid_cuts, const uint64_t* pa
   const bool csr = pair_base && (c->params.want & CMB_WANT_HIST_CSR);
   if (csr) {
     const uint64_t total = pair_base[N];
-    if (pair_base[me + 1] - pair_base[me] > c->pair_capacity) return fail(c, CMB_E_ARG, "cmb_allgather_stats: pair_base exceeds this rank's pairs");
-    if (c->pairs_all_capacity < total || !c->d_pairs_all) {
-      cudaFree(c->d_pairs_all);
-      c->d_pairs_all = nullptr;
-      c->pairs_all_capacity = 0;
-      const uint64_t want = total + total / 8 + 1024;
-      CU_TRY(c, cudaMalloc(&c->d_pairs_all, sizeof(cmb_hist_pair) * want));
-      c->pairs_all_capacity = want;
-    }
+    if (pair_base[me + 1] - pair_base[me] > c->ref.d_pairs.cap) return fail(c, CMB_E_ARG, "cmb_allgather_stats: pair_base exceeds this rank's pairs");
+    if (int rc = c->d_pairs_all.ensure(c, total, total + total / 8 + 1024)) return rc;
     const uint32_t n_own = c->tid_end - c->tid_begin;
     if (n_own && pair_base[me]) {
-      k_rebase_hist_offsets<<<(n_own + 255) / 256, 256, 0, c->stream>>>(c->d_rows + c->tid_begin, n_own, pair_base[me]);
+      k_rebase_hist_offsets<<<(n_own + 255) / 256, 256, 0, c->stream>>>(c->ref.d_rows + c->tid_begin, n_own, pair_base[me]);
       CU_TRY(c, cudaGetLastError());
     }
   }
@@ -1130,18 +1074,18 @@ int cmb_allgather_stats(cmb_ctx* c, const uint32_t* tid_cuts, const uint64_t* pa
   for (int r = 0; r < N; ++r) {
     const size_t n = (size_t)(tid_cuts[r + 1] - tid_cuts[r]) * sizeof(cmb_contig_stats);
     if (!n) continue;
-    cmb_contig_stats* p = c->d_rows + tid_cuts[r];
+    cmb_contig_stats* p = c->ref.d_rows + tid_cuts[r];
     NCCL_TRY(c, ncclBroadcast(p, p, n, ncclChar, r, c->comm, c->stream));
   }
   if (csr) {
     for (int r = 0; r < N; ++r) {
       const size_t n = (size_t)(pair_base[r + 1] - pair_base[r]) * sizeof(cmb_hist_pair);
       if (!n) continue;
-      NCCL_TRY(c, ncclBroadcast(c->d_pairs, c->d_pairs_all + pair_base[r], n, ncclChar, r, c->comm, c->stream));
+      NCCL_TRY(c, ncclBroadcast(c->ref.d_pairs, c->d_pairs_all + pair_base[r], n, ncclChar, r, c->comm, c->stream));
     }
   }
   NCCL_TRY(c, ncclGroupEnd());
-  if (stats) CU_TRY(c, cudaMemcpyAsync(stats, c->d_rows, sizeof(cmb_contig_stats) * (size_t)c->n_contigs, cudaMemcpyDeviceToHost, c->stream));
+  if (stats) CU_TRY(c, cudaMemcpyAsync(stats, c->ref.d_rows, sizeof(cmb_contig_stats) * (size_t)c->n_contigs, cudaMemcpyDeviceToHost, c->stream));
   if (csr && pairs && pair_base[N])
     CU_TRY(c, cudaMemcpyAsync(pairs, c->d_pairs_all, sizeof(cmb_hist_pair) * pair_base[N], cudaMemcpyDeviceToHost, c->stream));
   CU_TRY(c, cudaStreamSynchronize(c->stream));
@@ -1191,12 +1135,11 @@ constexpr size_t DEC_SLACK = 1024;
 constexpr size_t DEC_FRONT = 256;              // readable bytes in front of the first uploaded block (the bit readers align down)
 constexpr uint64_t DEC_TAIL_BYTES = 4u << 20;  // ranged decode: inflated bytes kept beyond the range for its last straddling record
 
-// Launch the inflate kernel over blocks [a.b0, a.b1).  CMB_INFLATE selects the first-pass kernel: t1 (default: one thread
-// per block + kd_crc32), g8 (four blocks per warp) or w1 (one block per warp, also the second pass over declined blocks).
-// First-pass inflate kernel: 0 = kd_inflate_t1 (a thread per block), 1 = kd_inflate_g8 (four blocks per warp), 2 = kd_inflate (a
-// warp per block).  t1 has the higher THROUGHPUT (its sm_count x 5 x 96 streams, 63 360 on 132 SMs, need that many blocks) but
-// each of its streams is slow, so a short list of blocks finishes sooner on g8.  The choice follows the number of blocks: a whole
-// 10 M-read file (46 000 blocks) goes to t1, a rank's share of it on 4 or 8 GPUs to g8.  CMB_INFLATE=t1|g8|w1 overrides.
+// First-pass inflate kernel: 0 = kd_inflate_t1 (a thread per block + kd_crc32), 1 = kd_inflate_g8 (four blocks per warp), 2 =
+// kd_inflate (a warp per block, also the second pass over declined blocks).  t1 has the higher THROUGHPUT (its sm_count x 5 x 96
+// streams, 63 360 on 132 SMs, need that many blocks) but each of its streams is slow, so a short list of blocks finishes sooner
+// on g8.  The choice follows the number of blocks: a whole 10 M-read file (46 000 blocks) goes to t1, a rank's share of it on 4
+// or 8 GPUs to g8.  CMB_INFLATE=t1|g8|w1 overrides.
 constexpr uint32_t T1_MIN_BLOCKS = 28000;
 int inflate_kind(uint32_t n_blocks) {
   static const int forced = [] {
@@ -1204,24 +1147,13 @@ int inflate_kind(uint32_t n_blocks) {
     if (e && !strcmp(e, "t1")) return 0;
     if (e && !strcmp(e, "g8")) return 1;
     if (e && !strcmp(e, "w1")) return 2;
-    if (getenv("CMB_INFLATE_G8") && getenv("CMB_INFLATE_G8")[0] == '0') return 2;
     return -1;
   }();
   if (forced >= 0) return forced;
-  static const uint32_t min_blocks = [] {
-    const char* e = getenv("CMB_T1_MIN_BLOCKS");  // experiment knob
-    return e ? (uint32_t)atol(e) : T1_MIN_BLOCKS;
-  }();
-  return n_blocks >= min_blocks ? 0 : 1;
+  return n_blocks >= T1_MIN_BLOCKS ? 0 : 1;
 }
 // Default: ONE persistent launch whose threads poll the windows' arrival flags (bounded wait), so that every SM has work as soon
-// as the first window is in.  CMB_INFLATE_WINDOWS=1 (t1 only) launches per copied window instead, stream-ordered behind the
-// window's copy -- nothing on the device then waits for data, which tools that serialise streams (ncu, compute-sanitizer)
-// need; with the default 8 hardware queues (CUDA_DEVICE_MAX_CONNECTIONS) those launches overlap poorly, hence not the default.
-bool inflate_per_window() {
-  static const bool v = getenv("CMB_INFLATE_WINDOWS") && getenv("CMB_INFLATE_WINDOWS")[0] == '1';
-  return v;
-}
+// as the first window is in.
 // Serial mode: copy everything, then ONE inflate launch ordered behind the copies on the context stream -- no flags, nothing on
 // the device waits for anything.  Used for files of a single window (nothing to overlap), on request (CMB_INFLATE_SERIAL=1),
 // and when a CUDA tool is injected into the process (ncu, compute-sanitizer: they serialise kernels against the other streams,
@@ -1243,29 +1175,21 @@ int launch_crc32(cmb_ctx* c, const InflateArgs& a, cudaStream_t st) {
   CU_TRY(c, cudaGetLastError());
   return CMB_OK;
 }
+// Launch the inflate kernel over blocks [a.b0, a.b1), or over a.block_list[a.b0, a.b1) with kd_inflate (the second pass).
 // *crc_pending (when given) is set instead of launching kd_crc32: the caller launches it once nothing else has to get past it
 // in the hardware queue (a kernel waiting for its predecessor blocks the queue for every stream that shares it).
-int launch_inflate(cmb_ctx* c, const InflateArgs& a, cudaStream_t st, bool first_pass = true, bool* crc_pending = nullptr) {
-  const int which = inflate_kind(a.b1 - a.b0);
-  const int k = (first_pass && !a.block_list) ? which : 2;
+int launch_inflate(cmb_ctx* c, const InflateArgs& a, cudaStream_t st, bool* crc_pending = nullptr) {
   const uint32_t nb = a.b1 - a.b0;
+  const int k = a.block_list ? 2 : inflate_kind(nb);
   if (k == 0) {
     CU_TRY(c, cudaFuncSetAttribute(kd_inflate_t1, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)T1_SMEM_BYTES));
     // every resident warp takes part; with fewer blocks than lanes, each warp works with its first `lanes` lanes only
     const uint32_t max_grid = (uint32_t)c->sm_count * 5, warps = max_grid * (T1_THREADS / 32);
-    uint32_t lanes = std::min<uint32_t>(32, std::max<uint32_t>(1, (nb + warps - 1) / warps));
-    static const int lanes_forced = [] { const char* e = getenv("CMB_T1_LANES"); return e ? atoi(e) : 0; }();  // experiment knob
-    if (lanes_forced > 0) lanes = std::min<uint32_t>(32, (uint32_t)lanes_forced);
+    const uint32_t lanes = std::min<uint32_t>(32, std::max<uint32_t>(1, (nb + warps - 1) / warps));
     const uint32_t per_cta = lanes * (T1_THREADS / 32);
-    uint32_t grid = std::min<uint32_t>((nb + per_cta - 1) / per_cta, max_grid);
-    if (const char* cap = getenv("CMB_T1_MAX_CTAS")) grid = std::max<uint32_t>(1, std::min<uint32_t>(grid, (uint32_t)atoi(cap)));  // experiment knob: fewer live streams
+    const uint32_t grid = std::min<uint32_t>((nb + per_cta - 1) / per_cta, max_grid);
     InflateArgs at = a;
     at.lane_limit = lanes;
-    // experiment knob, measured and left off: dealing the first round out column-wise (a warp's lanes hold blocks spread over
-    // the file) does not shorten the tail of a streamed file (94 vs 93 ms on config 2) and costs locality when the file is
-    // resident (82 vs 49 ms)
-    static const bool columns = getenv("CMB_T1_COLUMNS") && getenv("CMB_T1_COLUMNS")[0] == '1';
-    at.static_first = (!a.block_list && columns) ? 1u : 0u;
     kd_inflate_t1<<<grid, T1_THREADS, T1_SMEM_BYTES, st>>>(at);
     CU_TRY(c, cudaGetLastError());
     if (crc_pending) *crc_pending = true;
@@ -1284,147 +1208,68 @@ int launch_inflate(cmb_ctx* c, const InflateArgs& a, cudaStream_t st, bool first
   return CMB_OK;
 }
 
-template <class T>
-int dec_grow(cmb_ctx* c, T*& p, size_t& cap, size_t need, size_t extra_bytes = 0) {
-  if (cap >= need && p) return CMB_OK;
-  cudaFree(p);
-  p = nullptr;
-  cap = 0;
-  const size_t want = need + need / 8 + 16;
-  CU_TRY(c, cudaMalloc(&p, want * sizeof(T) + extra_bytes));
-  cap = want;
-  return CMB_OK;
-}
-}  // namespace
-
-namespace {
-int submit_bgzf_impl(cmb_ctx* c, const cmb_bgzf_input* in, cmb_bgzf_result* out, bool decode_only);
-}
-// Device memory for the decode buffers (compressed file + inflated stream + tuples) is requested before anything is
-// accumulated, so running out of it simply declines the sample: the host decoder needs only the staging batches.
-extern "C" int cmb_last_bgzf_batch(cmb_ctx* c, cmb_read_batch* dev_batch, uint32_t* n_records, uint32_t* n_intervals) {
-  if (!c || !dev_batch || !n_records || !n_intervals) return fail(c, CMB_E_ARG, "cmb_last_bgzf_batch: null argument");
-  if (!c->dec.last_valid || !c->dec.d_tuple_slab) return fail(c, CMB_E_ARG, "cmb_last_bgzf_batch: no device-decoded sample is resident");
-  carve_batch(c->dec.d_tuple_slab, c->dec.last_n_rec, c->dec.last_n_cig, dev_batch);
-  *n_records = c->dec.last_n_rec;
-  *n_intervals = c->dec.last_n_cig;
-  return CMB_OK;
+// zlib's inflate of BGZF block b into buf[0, isize), checked against the block's length and CRC-32 footer
+bool host_inflate_block(const cmb_bgzf_input* in, uint32_t b, std::vector<uint8_t>& buf) {
+  const uint32_t isz = in->block_isize[b];
+  if (buf.size() < (size_t)isz + 64) buf.resize((size_t)isz + 64);
+  z_stream zs;
+  memset(&zs, 0, sizeof zs);
+  if (inflateInit2(&zs, -15) != Z_OK) return false;
+  zs.next_in = const_cast<Bytef*>(in->data + in->block_coffset[b]);
+  zs.avail_in = in->block_clen[b];
+  zs.next_out = buf.data();
+  zs.avail_out = isz;
+  const bool ok = inflate(&zs, Z_FINISH) == Z_STREAM_END && zs.avail_out == 0;
+  inflateEnd(&zs);
+  uint32_t want_crc;
+  memcpy(&want_crc, in->data + in->block_coffset[b] + in->block_clen[b], 4);
+  return ok && (uint32_t)crc32(0, buf.data(), isz) == want_crc;
 }
 
-namespace {
-int bgzf_entry(cmb_ctx* c, const cmb_bgzf_input* in, cmb_bgzf_result* out, bool decode_only);
-}
-extern "C" int cmb_submit_bgzf(cmb_ctx* c, const cmb_bgzf_input* in, cmb_bgzf_result* out) { return bgzf_entry(c, in, out, false); }
-extern "C" int cmb_decode_bgzf(cmb_ctx* c, const cmb_bgzf_input* in, cmb_bgzf_result* out) { return bgzf_entry(c, in, out, true); }
+// One cmb_submit_bgzf / cmb_decode_bgzf call, handed from stage to stage.
+struct BgzfCall {
+  cmb_ctx* c;
+  cmb_ctx::Decode& d;
+  const cmb_bgzf_input* in;
+  cmb_bgzf_result* out;
+  bool decode_only;
+  uint32_t nb;
+  bool nothing_to_decode = true;  // header only, or an empty share of a ranged decode
+  std::vector<uint64_t> ustart;   // offset of every block in the inflated stream; [nb] = its length
+  // Blocks: records starting in [first_block, walk_end) are decoded; [first_block, data_end) are uploaded and inflated (the tail
+  // beyond walk_end only supplies the bytes of a record that straddles out of the range).  Whole file: walk_end = data_end = nb.
+  // Blocks before first_block are header text the host has already read: not inflated here.
+  uint32_t first_block = 0, walk_end = 0, data_end = 0;
+  // Device buffers hold only [byte_lo, byte_hi) of the file and [u_lo, total) of the inflated stream; the kernels index both
+  // with absolute offsets through biased base pointers.
+  uint64_t byte_lo = 0, byte_hi = 0, u_lo = 0, total = 0;
+  uint8_t* comp_base = nullptr;
+  uint8_t* infl_base = nullptr;
+  struct Window { uint32_t b0, b1; uint64_t byte0, byte1; };
+  std::vector<Window> windows;  // whole blocks, ~DEC_WINDOW_BYTES of file each
+  uint32_t n_copy_threads = 0;
+  bool src_pinned = false;
+  uint64_t n_rec = 0, n_cig = 0;
 
-extern "C" int cmb_filter_plan(cmb_ctx* c, int inverse, uint64_t* n_records, uint64_t* n_bytes) {
-  if (!c || !n_records || !n_bytes) return fail(c, CMB_E_ARG, "cmb_filter_plan: null argument");
-  auto& d = c->dec;
-  if (!d.last_valid || !d.d_tuple_slab || !c->have_params) return fail(c, CMB_E_ARG, "cmb_filter_plan: no device-decoded sample is resident (cmb_decode_bgzf first)");
-  CU_TRY(c, cudaSetDevice(c->device));
-  *n_records = 0;
-  *n_bytes = 0;
-  d.filter_planned = false;
-  const uint32_t n = d.last_n_rec;
-  if (n == 0) {
-    d.filter_bytes = 0;
-    d.filter_planned = true;
-    return CMB_OK;
-  }
-  const bool pair_path = !(c->mode.filter_single_reads && !c->mode.filter_pairs);
-  if (pair_path && !d.last_mate) return fail(c, CMB_E_ARG, "cmb_filter_plan: the sample was decoded without mate matching (set the parameters before cmb_decode_bgzf)");
-  if (d.filter_rec_cap < (size_t)n + 1 || !d.d_filter_anchor) {
-    cudaFree(d.d_filter_anchor); cudaFree(d.d_filter_role);
-    d.d_filter_anchor = nullptr; d.d_filter_role = nullptr; d.filter_rec_cap = 0;
-    const size_t want = (size_t)n + n / 8 + 16;
-    CU_TRY(c, cudaMalloc(&d.d_filter_anchor, 8 * want));
-    CU_TRY(c, cudaMalloc(&d.d_filter_role, want));
-    d.filter_rec_cap = want;
-  }
-  cmb_read_batch tb;
-  carve_batch(d.d_tuple_slab, d.last_n_rec, d.last_n_cig, &tb);
-  FilterArgs a{};
-  a.data = d.last_infl_base; a.rec_off = d.d_rec_off; a.n = n; a.flag = tb.flag; a.mapq = tb.mapq; a.nm_state = tb.nm_state; a.nm = tb.nm;
-  a.l_seq = tb.l_seq; a.aligned = tb.aligned; a.del = tb.del; a.mate = pair_path ? d.last_mate : nullptr; a.p = c->params;
-  a.filter_single = c->mode.filter_single_reads; a.pair_path = pair_path; a.filter_out = inverse ? 0 : 1;
-  a.anchor_bytes = d.d_filter_anchor; a.role = d.d_filter_role; a.error_flags = d.d_cnt + 12; a.n_emit = (unsigned long long*)(d.d_cnt + 14);
-  CU_TRY(c, cudaMemsetAsync(d.d_cnt + 12, 0, 16, c->stream));
-  kf_decide<<<(n + 255) / 256, 256, 0, c->stream>>>(a);
-  kf_scan<<<1, 1024, 0, c->stream>>>(d.d_filter_anchor, n);
-  CU_TRY(c, cudaGetLastError());
-  uint32_t h[4];
-  unsigned long long total = 0;
-  CU_TRY(c, cudaMemcpyAsync(h, d.d_cnt + 12, 16, cudaMemcpyDeviceToHost, c->stream));
-  CU_TRY(c, cudaMemcpyAsync(&total, d.d_filter_anchor + n, 8, cudaMemcpyDeviceToHost, c->stream));
-  CU_TRY(c, cudaStreamSynchronize(c->stream));
-  if (h[0] & ERR_NM)
-    return fail(c, CMB_E_NM, "Mapping record encountered that does not have an 'NM' auxiliary tag in the SAM/BAM format. This is required to work out some coverage statistics");
-  unsigned long long n_emit;
-  memcpy(&n_emit, h + 2, 8);
-  if (d.filter_out_cap < total || !d.d_filter_out) {
-    cudaFree(d.d_filter_out);
-    d.d_filter_out = nullptr;
-    d.filter_out_cap = 0;
-    const size_t want = (size_t)total + (size_t)total / 8 + 4096;
-    CU_TRY(c, cudaMalloc(&d.d_filter_out, want));
-    d.filter_out_cap = want;
-  }
-  a.out = d.d_filter_out;
-  kf_gather<<<(n + 7) / 8, 256, 0, c->stream>>>(a);
-  CU_TRY(c, cudaGetLastError());
-  d.filter_bytes = total;
-  d.filter_planned = true;
-  *n_records = n_emit;
-  *n_bytes = total;
-  return CMB_OK;
+  InflateArgs inflate_args(uint32_t b0, uint32_t b1) const;
+  int prepare();
+  int copy_inflate();
+  int declined();
+  int chain();
+  int extract();
+};
+
+// The inflate kernels' arguments over blocks [b0, b1) of the call
+InflateArgs BgzfCall::inflate_args(uint32_t b0, uint32_t b1) const {
+  InflateArgs a{};
+  a.comp = comp_base; a.coff = d.d_coff; a.clen = d.d_clen; a.isize = d.d_isize; a.uoff = d.d_ustart; a.scratch = d.d_t1_scratch;
+  a.b0 = b0; a.b1 = b1; a.out = infl_base; a.status = d.d_status; a.ticket = d.d_tickets; a.fail_count = d.d_cnt + 0;
+  return a;
 }
 
-extern "C" int cmb_filter_fetch(cmb_ctx* c, uint8_t* records, uint64_t n_bytes) {
-  if (!c || (!records && n_bytes)) return fail(c, CMB_E_ARG, "cmb_filter_fetch: null argument");
-  auto& d = c->dec;
-  if (!d.filter_planned || n_bytes != d.filter_bytes) return fail(c, CMB_E_ARG, "cmb_filter_fetch: call cmb_filter_plan first and pass the size it reported");
-  CU_TRY(c, cudaSetDevice(c->device));
-  if (n_bytes) CU_TRY(c, cudaMemcpyAsync(records, d.d_filter_out, n_bytes, cudaMemcpyDeviceToHost, c->stream));
-  CU_TRY(c, cudaStreamSynchronize(c->stream));
-  return CMB_OK;
-}
-
-namespace {
-int bgzf_entry(cmb_ctx* c, const cmb_bgzf_input* in, cmb_bgzf_result* out, bool decode_only) {
-  if (c) {
-    c->dec.last_valid = false;
-    c->dec.filter_planned = false;
-  }
-  const auto t_call0 = std::chrono::steady_clock::now();
-  const int rc = submit_bgzf_impl(c, in, out, decode_only);
-  if (out) out->ms_host_wall = (float)std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_call0).count();
-  if (rc == CMB_E_NOMEM) {
-    cudaGetLastError();
-    auto& d = c->dec;  // give the big buffers back so that the rest of the sample has room
-    cudaFree(d.d_comp); d.d_comp = nullptr; d.comp_cap = 0;
-    cudaFree(d.d_inflated); d.d_inflated = nullptr; d.infl_cap = 0;
-    cudaFree(d.d_tuple_slab); d.d_tuple_slab = nullptr; d.tuple_slab_bytes = 0;
-    cudaFree(d.d_rec_off); d.d_rec_off = nullptr; d.rec_cap = 0;
-    return fail(c, CMB_E_DECLINED, "cmb_submit_bgzf: not enough device memory for device-side decode");
-  }
-  return rc;
-}
-}  // namespace
-namespace {
-int submit_bgzf_impl(cmb_ctx* c, const cmb_bgzf_input* in, cmb_bgzf_result* out, bool decode_only) {
-  NvtxRange nvtx_fn("cmb_submit_bgzf");
-  if (!c || !in || !out || !in->data || !in->block_coffset || !in->block_clen || !in->block_isize)
-    return fail(c, CMB_E_ARG, "cmb_submit_bgzf: null argument");
-  if (!decode_only && !c->in_sample) return fail(c, CMB_E_ARG, "cmb_submit_bgzf: no sample in progress");
-  if (decode_only && (c->in_sample || !c->have_params)) return fail(c, CMB_E_ARG, "cmb_decode_bgzf: set the parameters first; not inside a sample");
-  if (c->n_acquired) return fail(c, CMB_E_ARG, "cmb_submit_bgzf: a staging batch is still acquired");
-  *out = cmb_bgzf_result{};
-  const uint32_t nb = in->n_blocks;
-  if (nb == 0) return CMB_OK;
-  CU_TRY(c, cudaSetDevice(c->device));
-  auto& d = c->dec;
-  // ---- host block table
-  std::vector<uint64_t> ustart((size_t)nb + 1, 0);
+// Stage 1: the block table, the blocks this call decodes, its copy windows, and every buffer, stream and copy slot it needs.
+int BgzfCall::prepare() {
+  ustart.assign((size_t)nb + 1, 0);
   for (uint32_t b = 0; b < nb; ++b) {
     if (in->block_coffset[b] + in->block_clen[b] + 8 > in->size) return fail(c, CMB_E_ARG, "cmb_submit_bgzf: block %u lies outside the data", b);
     ustart[b + 1] = ustart[b] + in->block_isize[b];
@@ -1432,10 +1277,8 @@ int submit_bgzf_impl(cmb_ctx* c, const cmb_bgzf_input* in, cmb_bgzf_result* out,
   const uint64_t stream_total = ustart[nb];
   if (in->records_at > stream_total) return fail(c, CMB_E_ARG, "cmb_submit_bgzf: records_at beyond the end of the stream");
   if (in->records_at == stream_total) return CMB_OK;  // header only
-  // Blocks: records starting in [first_block, walk_end) are decoded; [first_block, data_end) are uploaded and inflated (the tail
-  // beyond walk_end only supplies the bytes of a record that straddles out of the range).  Whole file: walk_end = data_end = nb.
-  uint32_t first_block = (uint32_t)(std::upper_bound(ustart.begin(), ustart.end(), in->records_at) - ustart.begin()) - 1;
-  uint32_t walk_end = nb, data_end = nb;
+  first_block = (uint32_t)(std::upper_bound(ustart.begin(), ustart.end(), in->records_at) - ustart.begin()) - 1;
+  walk_end = data_end = nb;
   if (in->ranged) {
     if (in->walk_begin_block != first_block || in->walk_end_block > nb || in->walk_end_block < in->walk_begin_block)
       return fail(c, CMB_E_ARG, "cmb_submit_bgzf: inconsistent block range");
@@ -1445,48 +1288,33 @@ int submit_bgzf_impl(cmb_ctx* c, const cmb_bgzf_input* in, cmb_bgzf_result* out,
     uint64_t tail = 0;
     while (data_end < nb && tail < DEC_TAIL_BYTES) tail += in->block_isize[data_end++];
   }
-  // Device buffers hold only [byte_lo, byte_hi) of the file and [u_lo, total) of the inflated stream; the kernels index both
-  // with absolute offsets through biased base pointers.
-  const uint64_t byte_lo = in->block_coffset[first_block];
-  const uint64_t byte_hi = data_end == nb ? in->size : in->block_coffset[data_end - 1] + in->block_clen[data_end - 1] + 8;
-  const uint64_t u_lo = ustart[first_block];
-  const uint64_t total = ustart[data_end];  // end of the inflated bytes available to this call
+  nothing_to_decode = false;
+  byte_lo = in->block_coffset[first_block];
+  byte_hi = data_end == nb ? in->size : in->block_coffset[data_end - 1] + in->block_clen[data_end - 1] + 8;
+  u_lo = ustart[first_block];
+  total = ustart[data_end];  // end of the inflated bytes available to this call
   // ---- buffers
   if (const char* lim = getenv("CMB_DECODE_MEM_LIMIT_MB")) {  // testing aid: behave as if the device had this much room
     if (((byte_hi - byte_lo) + (total - u_lo)) >> 20 > strtoull(lim, nullptr, 10)) return CMB_E_NOMEM;
   }
-  size_t dummy_cap;
   int rc;
-  if ((rc = dec_grow(c, d.d_comp, d.comp_cap, (size_t)(byte_hi - byte_lo) + DEC_FRONT + DEC_SLACK))) return rc;
-  if ((rc = dec_grow(c, d.d_inflated, d.infl_cap, (size_t)(total - u_lo) + DEC_SLACK))) return rc;
-  uint8_t* const comp_base = reinterpret_cast<uint8_t*>(reinterpret_cast<uintptr_t>(d.d_comp) + DEC_FRONT - byte_lo);
-  uint8_t* const infl_base = reinterpret_cast<uint8_t*>(reinterpret_cast<uintptr_t>(d.d_inflated) - u_lo);
-  if (d.blocks_cap < (size_t)nb + 1 || !d.d_coff) {
-    const size_t want = (size_t)nb + nb / 8 + 64;
-    cudaFree(d.d_coff); cudaFree(d.d_ustart); cudaFree(d.d_guess); cudaFree(d.d_exit); cudaFree(d.d_rec_base); cudaFree(d.d_cig_base);
-    cudaFree(d.d_clen); cudaFree(d.d_isize); cudaFree(d.d_status); cudaFree(d.d_nrec); cudaFree(d.d_ncig); cudaFree(d.d_dirty);
-    d.d_coff = d.d_ustart = d.d_guess = d.d_exit = d.d_rec_base = d.d_cig_base = nullptr;
-    d.d_clen = d.d_isize = d.d_status = d.d_nrec = d.d_ncig = d.d_dirty = nullptr;
-    d.blocks_cap = 0;
-    CU_TRY(c, cudaMalloc(&d.d_coff, 8 * want)); CU_TRY(c, cudaMalloc(&d.d_ustart, 8 * want)); CU_TRY(c, cudaMalloc(&d.d_guess, 8 * want));
-    CU_TRY(c, cudaMalloc(&d.d_exit, 8 * want)); CU_TRY(c, cudaMalloc(&d.d_rec_base, 8 * want)); CU_TRY(c, cudaMalloc(&d.d_cig_base, 8 * want));
-    CU_TRY(c, cudaMalloc(&d.d_clen, 4 * want)); CU_TRY(c, cudaMalloc(&d.d_isize, 4 * want)); CU_TRY(c, cudaMalloc(&d.d_status, 4 * want));
-    CU_TRY(c, cudaMalloc(&d.d_nrec, 4 * want)); CU_TRY(c, cudaMalloc(&d.d_ncig, 4 * want)); CU_TRY(c, cudaMalloc(&d.d_dirty, 4 * want));
-    cudaFree(d.d_t1_scratch);
-    d.d_t1_scratch = nullptr;
-    CU_TRY(c, cudaMalloc(&d.d_t1_scratch, (size_t)T1_LENS_BYTES * want));
-    d.blocks_cap = want;
-  }
-  if (!d.d_cnt) CU_TRY(c, cudaMalloc(&d.d_cnt, 64));
+  const size_t comp_need = (size_t)(byte_hi - byte_lo) + DEC_FRONT + DEC_SLACK, infl_need = (size_t)(total - u_lo) + DEC_SLACK;
+  if ((rc = d.d_comp.ensure(c, comp_need, with_slack(comp_need))) || (rc = d.d_inflated.ensure(c, infl_need, with_slack(infl_need))))
+    return rc;
+  comp_base = reinterpret_cast<uint8_t*>(reinterpret_cast<uintptr_t>(d.d_comp.p) + DEC_FRONT - byte_lo);
+  infl_base = reinterpret_cast<uint8_t*>(reinterpret_cast<uintptr_t>(d.d_inflated.p) - u_lo);
+  const size_t blocks_need = (size_t)nb + 1, blocks_want = (size_t)nb + nb / 8 + 64;
+  for (auto* b : {&d.d_coff, &d.d_ustart, &d.d_guess, &d.d_exit, &d.d_rec_base, &d.d_cig_base})
+    if ((rc = b->ensure(c, blocks_need, blocks_want))) return rc;
+  for (auto* b : {&d.d_clen, &d.d_isize, &d.d_status, &d.d_nrec, &d.d_ncig, &d.d_dirty})
+    if ((rc = b->ensure(c, blocks_need, blocks_want))) return rc;
+  if ((rc = d.d_t1_scratch.ensure(c, blocks_need * T1_LENS_BYTES, blocks_want * T1_LENS_BYTES))) return rc;
+  if ((rc = d.d_cnt.ensure(c, 16))) return rc;
   if (!d.have_events) {
     for (auto& e : d.ev) CU_TRY(c, cudaEventCreate(&e));
     d.have_events = true;
   }
-  (void)dummy_cap;
-  NvtxRange nvtx_copy("bgzf: H2D copy + inflate");
-  // ---- windows of whole blocks, ~DEC_WINDOW_BYTES of file each
-  struct Window { uint32_t b0, b1; uint64_t byte0, byte1; };
-  std::vector<Window> windows;
+  // ---- windows
   {
     uint32_t b = first_block;
     uint64_t byte0 = byte_lo;
@@ -1503,28 +1331,19 @@ int submit_bgzf_impl(cmb_ctx* c, const cmb_bgzf_input* in, cmb_bgzf_result* out,
       byte0 = byte1;
     }
   }
-  if (d.tickets_cap < windows.size() + 8 || !d.d_tickets) {  // [0] block ticket, [1, 1 + W) arrival flags
-    cudaFree(d.d_tickets);
-    d.d_tickets = nullptr;
-    d.tickets_cap = 0;
-    const size_t want = windows.size() * 3 + 64;
-    CU_TRY(c, cudaMalloc(&d.d_tickets, 4 * want));
-    d.tickets_cap = want;
-  }
-  if ((rc = dec_grow(c, d.d_block_window, d.block_window_cap, (size_t)nb))) return rc;
+  const size_t n_windows = windows.size();
+  if ((rc = d.d_tickets.ensure(c, n_windows + 8, n_windows * 3 + 64))) return rc;  // [0] block ticket, [1, 1 + W) arrival flags
+  if ((rc = d.d_block_window.ensure(c, nb, with_slack(nb)))) return rc;
   if (!d.h_ones) {
-    CU_TRY(c, cudaHostAlloc((void**)&d.h_ones, 64, cudaHostAllocDefault));
-    for (int k = 0; k < 16; ++k) d.h_ones[k] = 1;
+    if ((rc = d.h_ones.ensure(c, 16))) return rc;
+    for (int k = 0; k < 16; ++k) d.h_ones.p[k] = 1;
   }
-  std::vector<uint32_t> block_window(nb, 0);
-  for (size_t w = 0; w < windows.size(); ++w)
-    for (uint32_t b = windows[w].b0; b < windows[w].b1; ++b) block_window[b] = (uint32_t)w;
   // ---- copy threads, their streams and pinned slots
   cudaPointerAttributes attr{};
-  const bool src_pinned = cudaPointerGetAttributes(&attr, in->data) == cudaSuccess && attr.type == cudaMemoryTypeHost;
+  src_pinned = cudaPointerGetAttributes(&attr, in->data) == cudaSuccess && attr.type == cudaMemoryTypeHost;
   cudaGetLastError();  // cudaPointerGetAttributes on pageable memory may leave a sticky-free error code
-  uint32_t T = in->copy_threads ? in->copy_threads : 4;
-  T = std::min<uint32_t>(std::min<uint32_t>(T, 16), (uint32_t)windows.size());
+  const uint32_t T = std::min<uint32_t>(std::min<uint32_t>(in->copy_threads ? in->copy_threads : 4, 16), (uint32_t)n_windows);
+  n_copy_threads = T;
   while (d.streams.size() < T) {
     cudaStream_t st;
     CU_TRY(c, cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
@@ -1535,11 +1354,23 @@ int submit_bgzf_impl(cmb_ctx* c, const cmb_bgzf_input* in, cmb_bgzf_result* out,
     for (int k = 0; k < 2; ++k) {
       CU_TRY(c, cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
       d.slot_events.push_back(e);
-      void* p = nullptr;
-      CU_TRY(c, cudaHostAlloc(&p, DEC_COPY_CHUNK, cudaHostAllocDefault));
-      d.pinned.push_back(p);
+      PinnedBuf<uint8_t> slot;
+      if ((rc = slot.ensure(c, DEC_COPY_CHUNK))) return rc;
+      d.pinned.push_back(std::move(slot));
     }
   }
+  return CMB_OK;
+}
+
+// Stage 2: the block table goes up on the context stream, the windows on the copy streams (one host thread each, a 4-byte
+// arrival flag after each window), and the inflate kernel runs: one persistent launch before the copies whose threads wait for
+// their window's flag, or (serial) one launch behind all the copies.
+int BgzfCall::copy_inflate() {
+  NvtxRange nvtx("bgzf: H2D copy + inflate");
+  const uint32_t T = n_copy_threads;
+  std::vector<uint32_t> block_window(nb, 0);
+  for (size_t w = 0; w < windows.size(); ++w)
+    for (uint32_t b = windows[w].b0; b < windows[w].b1; ++b) block_window[b] = (uint32_t)w;
   // ---- upload the block table, reset counters (ctx stream), then let the copy streams start after it
   CU_TRY(c, cudaEventRecord(d.ev[0], c->stream));
   CU_TRY(c, cudaMemcpyAsync(d.d_coff, in->block_coffset, 8ull * nb, cudaMemcpyHostToDevice, c->stream));
@@ -1555,35 +1386,14 @@ int submit_bgzf_impl(cmb_ctx* c, const cmb_bgzf_input* in, cmb_bgzf_result* out,
   CU_TRY(c, cudaMemsetAsync(d.d_comp, 0, DEC_FRONT, c->stream));
   CU_TRY(c, cudaEventRecord(d.ev[1], c->stream));
   for (uint32_t t = 0; t < T; ++t) CU_TRY(c, cudaStreamWaitEvent(d.streams[t], d.ev[1], 0));
-  const bool serial = !inflate_per_window() && (windows.size() <= 1 || inflate_serial_requested());
-  const bool per_window = !serial && inflate_per_window();
-  const uint32_t NCS = 64;  // compute streams for the per-window launches
+  const bool serial = windows.size() <= 1 || inflate_serial_requested();
   bool crc_pending = false;
-  InflateArgs persistent_args{};
-  if (per_window) {
-    CU_TRY(c, cudaFuncSetAttribute(kd_inflate_t1, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)T1_SMEM_BYTES));
-    while (d.cstreams.size() < std::min<size_t>(NCS, windows.size())) {
-      cudaStream_t cs;
-      CU_TRY(c, cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking));
-      d.cstreams.push_back(cs);
-      cudaEvent_t e;
-      CU_TRY(c, cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-      d.cstream_done.push_back(e);
-    }
-    while (d.window_events.size() < windows.size()) {
-      cudaEvent_t e;
-      CU_TRY(c, cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-      d.window_events.push_back(e);
-    }
-    for (size_t k = 0; k < std::min<size_t>(NCS, windows.size()); ++k) CU_TRY(c, cudaStreamWaitEvent(d.cstreams[k], d.ev[1], 0));
-  } else if (!serial) {  // one persistent launch over every block; its warps wait for their block's window to arrive
-    InflateArgs a{};
-    a.comp = comp_base; a.coff = d.d_coff; a.clen = d.d_clen; a.isize = d.d_isize; a.uoff = d.d_ustart; a.scratch = d.d_t1_scratch;
-    // blocks before the one holding the first record are header text the host has already read: not inflated here
-    a.b0 = first_block; a.b1 = data_end; a.out = infl_base; a.status = d.d_status; a.ticket = d.d_tickets; a.fail_count = d.d_cnt + 0;
-    a.block_window = d.d_block_window; a.ready = d.d_tickets + 1;
-    persistent_args = a;
-    if ((rc = launch_inflate(c, a, c->stream, true, &crc_pending))) return rc;
+  InflateArgs persistent = inflate_args(first_block, data_end);
+  int rc;
+  if (!serial) {  // one persistent launch over every block; its warps wait for their block's window to arrive
+    persistent.block_window = d.d_block_window;
+    persistent.ready = d.d_tickets + 1;
+    if ((rc = launch_inflate(c, persistent, c->stream, &crc_pending))) return rc;
   }
   std::atomic<size_t> next_window{0};
   std::atomic<int> first_err{0};
@@ -1617,22 +1427,7 @@ int submit_bgzf_impl(cmb_ctx* c, const cmb_bgzf_input* in, cmb_bgzf_result* out,
           slot ^= 1;
         }
       }
-      if (per_window) {
-        // the window's blocks are inflated by their own launch, ordered behind the copy by an event; many windows' launches
-        // are in flight at once on the compute streams.  d_tickets[1 + w] (zeroed above) is that launch's block ticket.
-        cudaStream_t cs = d.cstreams[w % d.cstreams.size()];
-        if (!check(cudaEventRecord(d.window_events[w], st))) break;
-        if (!check(cudaStreamWaitEvent(cs, d.window_events[w], 0))) break;
-        InflateArgs a{};
-        a.comp = comp_base; a.coff = d.d_coff; a.clen = d.d_clen; a.isize = d.d_isize; a.uoff = d.d_ustart; a.scratch = d.d_t1_scratch;
-        a.b0 = win.b0; a.b1 = win.b1; a.out = infl_base; a.status = d.d_status; a.ticket = d.d_tickets + 1 + w; a.fail_count = d.d_cnt + 0;
-        const uint32_t nbw = win.b1 - win.b0;
-        kd_inflate_t1<<<(nbw + T1_THREADS - 1) / T1_THREADS, T1_THREADS, T1_SMEM_BYTES, cs>>>(a);
-        kd_crc32<<<std::max<uint32_t>(1, (nbw + 7) / 8), 256, 0, cs>>>(a);
-        if (!check(cudaGetLastError())) break;
-      } else if (!check(cudaMemcpyAsync(d.d_tickets + 1 + w, d.h_ones, 4, cudaMemcpyHostToDevice, st))) {  // window w has arrived
-        break;
-      }
+      if (!check(cudaMemcpyAsync(d.d_tickets + 1 + w, d.h_ones, 4, cudaMemcpyHostToDevice, st))) break;  // window w has arrived
     }
     check(cudaEventRecord(d.done_events[t], st));
   };
@@ -1645,13 +1440,10 @@ int submit_bgzf_impl(cmb_ctx* c, const cmb_bgzf_input* in, cmb_bgzf_result* out,
   }
   const double copy_wall_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - copy_t0).count();
   out->ms_copy_enqueue_wall = (float)copy_wall_ms;
-  if (crc_pending && (rc = launch_crc32(c, persistent_args, c->stream))) return rc;  // every copy is enqueued: nothing left to hold up
+  if (crc_pending && (rc = launch_crc32(c, persistent, c->stream))) return rc;  // every copy is enqueued: nothing left to hold up
   if (serial && !first_err.load()) {
     for (uint32_t t = 0; t < T; ++t) CU_TRY(c, cudaStreamWaitEvent(c->stream, d.done_events[t], 0));
-    InflateArgs a{};
-    a.comp = comp_base; a.coff = d.d_coff; a.clen = d.d_clen; a.isize = d.d_isize; a.uoff = d.d_ustart; a.scratch = d.d_t1_scratch;
-    a.b0 = first_block; a.b1 = data_end; a.out = infl_base; a.status = d.d_status; a.ticket = d.d_tickets; a.fail_count = d.d_cnt + 0;
-    if ((rc = launch_inflate(c, a, c->stream))) return rc;
+    if ((rc = launch_inflate(c, inflate_args(first_block, data_end), c->stream))) return rc;
   }
   if (first_err.load()) {  // release the warps still waiting for windows that will never arrive
     cudaMemsetAsync(d.d_tickets + 1, 1, 4 * windows.size(), d.streams[0]);
@@ -1669,12 +1461,6 @@ int submit_bgzf_impl(cmb_ctx* c, const cmb_bgzf_input* in, cmb_bgzf_result* out,
     fprintf(stderr, "#decode_h2d\twindows=%zu\tbytes=%llu\tcopy_streams_done_after_ms=%.1f (host clock from the end of the enqueue; enqueue took %.1f ms)\n",
             windows.size(), (unsigned long long)(byte_hi - byte_lo), wait_ms, copy_wall_ms);
   }
-  if (per_window) {
-    for (size_t k = 0; k < std::min<size_t>(NCS, windows.size()); ++k) {
-      CU_TRY(c, cudaEventRecord(d.cstream_done[k], d.cstreams[k]));
-      CU_TRY(c, cudaStreamWaitEvent(c->stream, d.cstream_done[k], 0));
-    }
-  }
   CU_TRY(c, cudaEventRecord(d.ev[2], c->stream));
   if (getenv("CMB_DECODE_PROFILE")) {  // debugging aid: the inflate kernel alone, all blocks resident, one launch
     CU_TRY(c, cudaStreamSynchronize(c->stream));
@@ -1682,9 +1468,8 @@ int submit_bgzf_impl(cmb_ctx* c, const cmb_bgzf_input* in, cmb_bgzf_result* out,
     cudaEventCreate(&p0);
     cudaEventCreate(&p1);
     CU_TRY(c, cudaMemsetAsync(d.d_tickets, 0, 4, c->stream));
-    InflateArgs a{};
-    a.comp = comp_base; a.coff = d.d_coff; a.clen = d.d_clen; a.isize = d.d_isize; a.uoff = d.d_ustart; a.scratch = d.d_t1_scratch;
-    a.b0 = first_block; a.b1 = data_end; a.out = infl_base; a.status = d.d_status; a.ticket = d.d_tickets; a.fail_count = d.d_cnt + 8;
+    InflateArgs a = inflate_args(first_block, data_end);
+    a.fail_count = d.d_cnt + 8;
     cudaEventRecord(p0, c->stream);
     if ((rc = launch_inflate(c, a, c->stream))) return rc;
     cudaEventRecord(p1, c->stream);
@@ -1696,12 +1481,16 @@ int submit_bgzf_impl(cmb_ctx* c, const cmb_bgzf_input* in, cmb_bgzf_result* out,
     cudaEventDestroy(p0);
     cudaEventDestroy(p1);
   }
-  nvtx_copy.end();
-  NvtxRange nvtx_declined("bgzf: declined blocks (second pass, host zlib)");
-  // ---- blocks the device declined: zlib on the host, patched into the inflated stream
+  return CMB_OK;
+}
+
+// Stage 3: blocks the first pass declined get a second device pass, then zlib on the host, patched into the inflated stream.
+int BgzfCall::declined() {
+  NvtxRange nvtx("bgzf: declined blocks (second pass, host zlib)");
   uint32_t h_cnt[16];
   CU_TRY(c, cudaMemcpyAsync(h_cnt, d.d_cnt, 64, cudaMemcpyDeviceToHost, c->stream));
   CU_TRY(c, cudaStreamSynchronize(c->stream));
+  std::vector<uint8_t> tmp;
   if (h_cnt[0] || getenv("CMB_DECODE_RETRY_TEST")) {
     std::vector<uint32_t> status(nb);
     CU_TRY(c, cudaMemcpy(status.data(), d.d_status, 4ull * nb, cudaMemcpyDeviceToHost));
@@ -1717,83 +1506,56 @@ int submit_bgzf_impl(cmb_ctx* c, const cmb_bgzf_input* in, cmb_bgzf_result* out,
     }
     // Second chance on the device: the one-stream-per-warp kernel has larger Huffman tables (10-bit roots, 128 long-code
     // prefixes) than the four-streams-per-warp one, so most blocks the first pass declined for table space fit there.
-    {
-      std::vector<uint32_t> again;
-      for (uint32_t b = first_block; b < data_end; ++b)
-        if (status[b] != INF_OK) again.push_back(b);
-      out->n_blocks_second_pass = (uint32_t)again.size();
-      if (!again.empty()) {
-        uint32_t* d_list = d.d_dirty;  // free until the record chain starts (nb entries)
-        CU_TRY(c, cudaMemcpyAsync(d_list, again.data(), 4ull * again.size(), cudaMemcpyHostToDevice, c->stream));
-        CU_TRY(c, cudaMemsetAsync(d.d_tickets, 0, 4, c->stream));
-        CU_TRY(c, cudaMemsetAsync(d.d_cnt, 0, 4, c->stream));
-        InflateArgs a2{};
-        a2.comp = comp_base; a2.coff = d.d_coff; a2.clen = d.d_clen; a2.isize = d.d_isize; a2.uoff = d.d_ustart; a2.scratch = d.d_t1_scratch;
-        a2.b0 = 0; a2.b1 = (uint32_t)again.size(); a2.out = infl_base; a2.status = d.d_status; a2.ticket = d.d_tickets;
-        a2.fail_count = d.d_cnt + 0; a2.block_list = d_list;
-        if ((rc = launch_inflate(c, a2, c->stream, false))) return rc;
-        out->n_launches += 1;
-        for (uint32_t b : again) status[b] = INF_OK;  // refreshed from the device below
-        std::vector<uint32_t> st2(nb);
-        CU_TRY(c, cudaMemcpyAsync(st2.data(), d.d_status, 4ull * nb, cudaMemcpyDeviceToHost, c->stream));
-        CU_TRY(c, cudaStreamSynchronize(c->stream));
-        for (uint32_t b : again) status[b] = st2[b];
-      }
+    std::vector<uint32_t> again;
+    for (uint32_t b = first_block; b < data_end; ++b)
+      if (status[b] != INF_OK) again.push_back(b);
+    out->n_blocks_second_pass = (uint32_t)again.size();
+    if (!again.empty()) {
+      uint32_t* d_list = d.d_dirty;  // free until the record chain starts (nb entries)
+      CU_TRY(c, cudaMemcpyAsync(d_list, again.data(), 4ull * again.size(), cudaMemcpyHostToDevice, c->stream));
+      CU_TRY(c, cudaMemsetAsync(d.d_tickets, 0, 4, c->stream));
+      CU_TRY(c, cudaMemsetAsync(d.d_cnt, 0, 4, c->stream));
+      InflateArgs a = inflate_args(0, (uint32_t)again.size());
+      a.block_list = d_list;
+      if (int rc = launch_inflate(c, a, c->stream)) return rc;
+      out->n_launches += 1;
+      std::vector<uint32_t> st2(nb);
+      CU_TRY(c, cudaMemcpyAsync(st2.data(), d.d_status, 4ull * nb, cudaMemcpyDeviceToHost, c->stream));
+      CU_TRY(c, cudaStreamSynchronize(c->stream));
+      for (uint32_t b : again) status[b] = st2[b];
     }
-    std::vector<uint8_t> tmp(65536 + 64);
-    z_stream zs;
-    memset(&zs, 0, sizeof zs);
-    if (inflateInit2(&zs, -15) != Z_OK) return fail(c, CMB_E_NOMEM, "zlib init failed");
     for (uint32_t b = first_block; b < data_end; ++b) {
       if (status[b] == INF_OK) continue;
-      const uint32_t isz = in->block_isize[b];
-      if (tmp.size() < isz) tmp.resize(isz);
-      inflateReset(&zs);
-      zs.next_in = const_cast<Bytef*>(in->data + in->block_coffset[b]);
-      zs.avail_in = in->block_clen[b];
-      zs.next_out = tmp.data();
-      zs.avail_out = isz;
-      uint32_t want_crc;
-      memcpy(&want_crc, in->data + in->block_coffset[b] + in->block_clen[b], 4);
-      if (inflate(&zs, Z_FINISH) != Z_STREAM_END || zs.avail_out != 0 || (uint32_t)crc32(0, tmp.data(), isz) != want_crc) {
-        inflateEnd(&zs);
-        return fail(c, CMB_E_DECLINED, "cmb_submit_bgzf: BGZF block %u does not inflate", b);
-      }
-      CU_TRY(c, cudaMemcpy(infl_base + ustart[b], tmp.data(), isz, cudaMemcpyHostToDevice));
+      if (!host_inflate_block(in, b, tmp)) return fail(c, CMB_E_DECLINED, "cmb_submit_bgzf: BGZF block %u does not inflate", b);
+      CU_TRY(c, cudaMemcpy(infl_base + ustart[b], tmp.data(), in->block_isize[b], cudaMemcpyHostToDevice));
       out->n_blocks_host += 1;
     }
-    inflateEnd(&zs);
   }
   if (getenv("CMB_DECODE_VERIFY")) {  // debugging aid: compare every device-inflated block with zlib's output
-    std::vector<uint8_t> dev(total - u_lo), tmp(65536 + 64);
+    std::vector<uint8_t> dev(total - u_lo);
     CU_TRY(c, cudaMemcpy(dev.data(), d.d_inflated, total - u_lo, cudaMemcpyDeviceToHost));
-    z_stream zs;
-    memset(&zs, 0, sizeof zs);
-    inflateInit2(&zs, -15);
     uint32_t bad = 0;
     for (uint32_t b = first_block; b < data_end; ++b) {
       const uint32_t isz = in->block_isize[b];
       if (!isz) continue;
-      if (tmp.size() < isz) tmp.resize(isz);
-      inflateReset(&zs);
-      zs.next_in = const_cast<Bytef*>(in->data + in->block_coffset[b]);
-      zs.avail_in = in->block_clen[b];
-      zs.next_out = tmp.data();
-      zs.avail_out = isz;
-      const int zr = inflate(&zs, Z_FINISH);
-      if (zr != Z_STREAM_END || memcmp(tmp.data(), dev.data() + (ustart[b] - u_lo), isz) != 0) {
+      const uint8_t* got = dev.data() + (ustart[b] - u_lo);
+      const bool zlib_ok = host_inflate_block(in, b, tmp);
+      if (!zlib_ok || memcmp(tmp.data(), got, isz) != 0) {
         uint32_t k = 0;
-        while (k < isz && tmp[k] == dev[ustart[b] - u_lo + k]) ++k;
-        if (bad < 8) fprintf(stderr, "#decode_verify\tblock %u (clen %u isize %u): zlib rc %d, first difference at byte %u\n", b, in->block_clen[b], isz, zr, k);
+        while (k < isz && tmp[k] == got[k]) ++k;
+        if (bad < 8) fprintf(stderr, "#decode_verify\tblock %u (clen %u isize %u): zlib %s, first difference at byte %u\n", b, in->block_clen[b], isz, zlib_ok ? "ok" : "failed", k);
         ++bad;
       }
     }
-    inflateEnd(&zs);
     fprintf(stderr, "#decode_verify\t%u of %u blocks differ from zlib; %u inflated on the host\n", bad, data_end - first_block, out->n_blocks_host);
   }
-  nvtx_declined.end();
-  NvtxRange nvtx_chain("bgzf: record chain (guess, walk, verify, offsets)");
-  // ---- record chain
+  return CMB_OK;
+}
+
+// Stage 4: the record chain -- a guessed first record per block, walked to the block's end, verified against the neighbour's
+// guess (repaired and re-walked until it settles), then the record and CIGAR bases of every block.
+int BgzfCall::chain() {
+  NvtxRange nvtx("bgzf: record chain (guess, walk, verify, offsets)");
   WalkArgs wa{};
   // The chain is walked over [first_block, walk_hi): one block past the range when there is one, so that the range's last
   // record boundary is also checked against an independent guess.
@@ -1807,6 +1569,7 @@ int submit_bgzf_impl(cmb_ctx* c, const cmb_bgzf_input* in, cmb_bgzf_result* out,
   kd_walk<<<(nwb + 127) / 128, 128, 0, c->stream>>>(wa);
   CU_TRY(c, cudaGetLastError());
   out->n_launches += 2;
+  uint32_t h_cnt[16];
   uint64_t h_exit = 0;
   for (uint32_t round = 0;; ++round) {
     if (nwb > 1) {
@@ -1826,7 +1589,7 @@ int submit_bgzf_impl(cmb_ctx* c, const cmb_bgzf_input* in, cmb_bgzf_result* out,
     kd_walk<<<(nwb + 127) / 128, 128, 0, c->stream>>>(wa);
     CU_TRY(c, cudaGetLastError());
   }
-  if (walk_end == nb ? h_exit != stream_total : (h_exit == WALK_UNKNOWN || h_exit > total))
+  if (walk_end == nb ? h_exit != ustart[nb] : (h_exit == WALK_UNKNOWN || h_exit > total))
     return fail(c, CMB_E_DECLINED, walk_end == nb ? "cmb_submit_bgzf: record chain does not end at the end of the stream"
                                                   : "cmb_submit_bgzf: a record runs past the inflated tail of the block range");
   kd_scan_items<<<1, 1024, 0, c->stream>>>(d.d_nrec, d.d_ncig, first_block, walk_end, d.d_rec_base, d.d_cig_base, (uint64_t*)(d.d_cnt + 6));
@@ -1836,112 +1599,122 @@ int submit_bgzf_impl(cmb_ctx* c, const cmb_bgzf_input* in, cmb_bgzf_result* out,
   CU_TRY(c, cudaMemcpyAsync(totals, d.d_cnt + 6, 16, cudaMemcpyDeviceToHost, c->stream));
   CU_TRY(c, cudaStreamSynchronize(c->stream));
   CU_TRY(c, cudaEventRecord(d.ev[3], c->stream));
-  nvtx_chain.end();
-  NvtxRange nvtx_extract("bgzf: extract, mate matching, K1");
-  const uint64_t n_rec = totals[0], n_cig = totals[1];
+  n_rec = totals[0];
+  n_cig = totals[1];
+  return CMB_OK;
+}
+
+// Stage 5: the per-record tuples, mate matching when a pair filter needs it, and K1 over the tuples (not for cmb_decode_bgzf).
+int BgzfCall::extract() {
+  NvtxRange nvtx("bgzf: extract, mate matching, K1");
   if (n_rec >= 0xffffff00ull || n_cig >= 0xffffff00ull) return fail(c, CMB_E_DECLINED, "cmb_submit_bgzf: more than 2^32 records or cigar operations");
   out->n_records = n_rec;
   out->n_intervals = n_cig;
-  if (n_rec) {
-    if ((rc = dec_grow(c, d.d_rec_off, d.rec_cap, (size_t)n_rec))) return rc;
-    size_t offs[13];
-    const size_t need = batch_slab_bytes((uint32_t)n_rec, (uint32_t)n_cig, offs);
-    if (d.tuple_slab_bytes < need || !d.d_tuple_slab) {
-      cudaFree(d.d_tuple_slab);
-      d.d_tuple_slab = nullptr;
-      d.tuple_slab_bytes = 0;
-      const size_t want = need + need / 8;
-      CU_TRY(c, cudaMalloc(&d.d_tuple_slab, want));
-      d.tuple_slab_bytes = want;
+  if (!n_rec) {
+    CU_TRY(c, cudaEventRecord(d.ev[4], c->stream));
+    CU_TRY(c, cudaEventRecord(d.ev[5], c->stream));
+    return CMB_OK;
+  }
+  int rc;
+  size_t offs[13];
+  const size_t slab_need = batch_slab_bytes((uint32_t)n_rec, (uint32_t)n_cig, offs);
+  if ((rc = d.d_rec_off.ensure(c, n_rec, with_slack(n_rec))) || (rc = d.d_tuple_slab.ensure(c, slab_need, slab_need + slab_need / 8)))
+    return rc;
+  cmb_read_batch tb;
+  carve_batch(d.d_tuple_slab, (uint32_t)n_rec, (uint32_t)n_cig, &tb);
+  d.last_n_rec = (uint32_t)n_rec;
+  d.last_n_cig = (uint32_t)n_cig;
+  OffsetArgs oa{};
+  oa.data = infl_base; oa.ustart = d.d_ustart; oa.guess = d.d_guess; oa.rec_base = d.d_rec_base; oa.cig_base = d.d_cig_base;
+  oa.first_block = first_block; oa.n_blocks = walk_end; oa.rec_off = d.d_rec_off; oa.iv_begin = tb.iv_begin; oa.n_records = n_rec; oa.n_cig_total = n_cig;
+  kd_offsets<<<(walk_end - first_block + 127) / 128, 128, 0, c->stream>>>(oa);
+  CU_TRY(c, cudaGetLastError());
+  ExtractArgs ea{};
+  ea.data = infl_base; ea.rec_off = d.d_rec_off; ea.n_records = n_rec;
+  ea.own_lo = in->ranged ? in->own_tid_begin : INT_MIN; ea.own_hi = in->ranged ? in->own_tid_end : INT_MAX;
+  ea.own_unplaced = in->ranged ? in->own_unplaced : 1u; ea.n_owned = (unsigned long long*)(d.d_cnt + 10);
+  ea.tid = tb.tid; ea.pos = tb.pos; ea.flag = tb.flag; ea.mapq = tb.mapq; ea.nm_state = tb.nm_state; ea.nm = tb.nm; ea.l_seq = tb.l_seq;
+  ea.aligned = tb.aligned; ea.del = tb.del; ea.ins = tb.ins; ea.iv_begin = tb.iv_begin; ea.iv_start = tb.iv_start; ea.iv_len = tb.iv_len;
+  ea.n_primary = (unsigned long long*)(d.d_cnt + 4); ea.flags = d.d_cnt + 1;
+  kd_extract<<<(uint32_t)((n_rec + 255) / 256), 256, 0, c->stream>>>(ea);
+  CU_TRY(c, cudaGetLastError());
+  out->n_launches += 2;
+  uint32_t h_cnt[16];
+  CU_TRY(c, cudaMemcpyAsync(h_cnt, d.d_cnt, 64, cudaMemcpyDeviceToHost, c->stream));
+  CU_TRY(c, cudaStreamSynchronize(c->stream));
+  if (h_cnt[1]) return fail(c, CMB_E_DECLINED, "cmb_submit_bgzf: malformed alignment record (flags %u)", h_cnt[1]);
+  memcpy(&out->n_primary, h_cnt + 4, 8);
+  memcpy(&out->n_records, h_cnt + 10, 8);  // records this call owns (all of them unless ranged)
+  d.last_valid = true;
+  d.last_mate = nullptr;
+  d.last_infl_base = infl_base;
+  // mate matching on the device (filter.rs:117-233; cmb_pairs.cuh): for coverage when the pair thresholds apply; for
+  // `coverm filter` whenever the filter's pair path runs (everything but "single-read thresholds only", filter.rs:88)
+  const bool need_mates = decode_only ? !(c->mode.filter_single_reads && !c->mode.filter_pairs) : (bool)c->mode.filter_pairs;
+  if (need_mates) {
+    if (d.d_pair_key.cap < n_rec) {  // growing: give the filter's buffers back first (cmb_filter_plan sizes them again)
+      d.d_filter_anchor.release();
+      d.d_filter_role.release();
+      d.d_filter_out.release();
     }
-    cmb_read_batch tb;
-    carve_batch(d.d_tuple_slab, (uint32_t)n_rec, (uint32_t)n_cig, &tb);
-    d.last_n_rec = (uint32_t)n_rec;
-    d.last_n_cig = (uint32_t)n_cig;
-    OffsetArgs oa{};
-    oa.data = infl_base; oa.ustart = d.d_ustart; oa.guess = d.d_guess; oa.rec_base = d.d_rec_base; oa.cig_base = d.d_cig_base;
-    oa.first_block = first_block; oa.n_blocks = walk_end; oa.rec_off = d.d_rec_off; oa.iv_begin = tb.iv_begin; oa.n_records = n_rec; oa.n_cig_total = n_cig;
-    kd_offsets<<<(walk_end - first_block + 127) / 128, 128, 0, c->stream>>>(oa);
+    const size_t want = with_slack(n_rec);
+    if ((rc = d.d_pair_key.ensure(c, n_rec, want)) || (rc = d.d_pair_mate.ensure(c, n_rec, want)) || (rc = d.d_pair_next.ensure(c, n_rec, want)))
+      return rc;
+    size_t table = 1u << 16;
+    while (table < 2 * (size_t)n_rec) table <<= 1;
+    if ((rc = d.d_pair_tag.ensure(c, table)) || (rc = d.d_pair_head.ensure(c, table))) return rc;
+    CU_TRY(c, cudaMemsetAsync(d.d_pair_tag, 0, 8 * table, c->stream));
+    CU_TRY(c, cudaMemsetAsync(d.d_pair_head, 0xff, 4 * table, c->stream));
+    PairArgs pa{};
+    pa.data = infl_base; pa.rec_off = d.d_rec_off; pa.n_records = (uint32_t)n_rec; pa.key = d.d_pair_key; pa.mate = d.d_pair_mate;
+    pa.next = d.d_pair_next; pa.slot_tag = d.d_pair_tag; pa.slot_head = d.d_pair_head; pa.table_mask = (uint32_t)(table - 1);
+    pa.flags = d.d_cnt + 1;
+    const uint32_t gr = (uint32_t)((n_rec + 255) / 256);
+    kd_pair_keys<<<gr, 256, 0, c->stream>>>(pa);
+    kd_pair_insert<<<gr, 256, 0, c->stream>>>(pa);
+    kd_pair_resolve<<<(uint32_t)((table + 255) / 256), 256, 0, c->stream>>>(pa);
     CU_TRY(c, cudaGetLastError());
-    ExtractArgs ea{};
-    ea.data = infl_base; ea.rec_off = d.d_rec_off; ea.n_records = n_rec;
-    ea.own_lo = in->ranged ? in->own_tid_begin : INT_MIN; ea.own_hi = in->ranged ? in->own_tid_end : INT_MAX;
-    ea.own_unplaced = in->ranged ? in->own_unplaced : 1u; ea.n_owned = (unsigned long long*)(d.d_cnt + 10);
-    ea.tid = tb.tid; ea.pos = tb.pos; ea.flag = tb.flag; ea.mapq = tb.mapq; ea.nm_state = tb.nm_state; ea.nm = tb.nm; ea.l_seq = tb.l_seq;
-    ea.aligned = tb.aligned; ea.del = tb.del; ea.ins = tb.ins; ea.iv_begin = tb.iv_begin; ea.iv_start = tb.iv_start; ea.iv_len = tb.iv_len;
-    ea.n_primary = (unsigned long long*)(d.d_cnt + 4); ea.flags = d.d_cnt + 1;
-    kd_extract<<<(uint32_t)((n_rec + 255) / 256), 256, 0, c->stream>>>(ea);
-    CU_TRY(c, cudaGetLastError());
-    out->n_launches += 2;
+    out->n_launches += 3;
     CU_TRY(c, cudaMemcpyAsync(h_cnt, d.d_cnt, 64, cudaMemcpyDeviceToHost, c->stream));
     CU_TRY(c, cudaStreamSynchronize(c->stream));
-    if (h_cnt[1]) return fail(c, CMB_E_DECLINED, "cmb_submit_bgzf: malformed alignment record (flags %u)", h_cnt[1]);
-    memcpy(&out->n_primary, h_cnt + 4, 8);
-    memcpy(&out->n_records, h_cnt + 10, 8);  // records this call owns (all of them unless ranged)
-    d.last_valid = true;
-    d.last_mate = nullptr;
-    d.last_infl_base = infl_base;
-    // mate matching on the device (filter.rs:117-233; cmb_pairs.cuh): for coverage when the pair thresholds apply; for
-    // `coverm filter` whenever the filter's pair path runs (everything but "single-read thresholds only", filter.rs:88)
-    const bool need_mates = decode_only ? !(c->mode.filter_single_reads && !c->mode.filter_pairs) : (bool)c->mode.filter_pairs;
-    if (need_mates) {
-      if (d.pair_rec_cap < (size_t)n_rec || !d.d_pair_key) {
-        cudaFree(d.d_filter_anchor); cudaFree(d.d_filter_role); cudaFree(d.d_filter_out);
-    cudaFree(d.d_pair_key); cudaFree(d.d_pair_mate); cudaFree(d.d_pair_next);
-        d.d_pair_key = nullptr; d.d_pair_mate = nullptr; d.d_pair_next = nullptr; d.pair_rec_cap = 0;
-        const size_t want = (size_t)n_rec + (size_t)n_rec / 8 + 16;
-        CU_TRY(c, cudaMalloc(&d.d_pair_key, 8 * want));
-        CU_TRY(c, cudaMalloc(&d.d_pair_mate, 4 * want));
-        CU_TRY(c, cudaMalloc(&d.d_pair_next, 4 * want));
-        d.pair_rec_cap = want;
+    if (h_cnt[1]) return fail(c, CMB_E_DECLINED, "cmb_submit_bgzf: mate matching gave up (flags %u)", h_cnt[1]);
+    d.last_mate = d.d_pair_mate;
+  }
+  CU_TRY(c, cudaEventRecord(d.ev[4], c->stream));
+  if (c->n_local && !decode_only) {
+    // records that start before excl_end_block are this rank's exclusive share of the stream (cmb_kept_tid_range)
+    uint32_t excl_n = 0xffffffffu;
+    if (in->ranged && in->excl_end_block < walk_end) {
+      if (in->excl_end_block <= first_block) excl_n = 0;
+      else {
+        uint64_t base = 0;
+        CU_TRY(c, cudaMemcpyAsync(&base, d.d_rec_base + in->excl_end_block, 8, cudaMemcpyDeviceToHost, c->stream));
+        CU_TRY(c, cudaStreamSynchronize(c->stream));
+        excl_n = (uint32_t)base;
       }
-      size_t table = 1u << 16;
-      while (table < 2 * (size_t)n_rec) table <<= 1;
-      if (d.pair_table_cap < table) {
-        cudaFree(d.d_pair_tag); cudaFree(d.d_pair_head);
-        d.d_pair_tag = nullptr; d.d_pair_head = nullptr; d.pair_table_cap = 0;
-        CU_TRY(c, cudaMalloc(&d.d_pair_tag, 8 * table));
-        CU_TRY(c, cudaMalloc(&d.d_pair_head, 4 * table));
-        d.pair_table_cap = table;
-      }
-      CU_TRY(c, cudaMemsetAsync(d.d_pair_tag, 0, 8 * table, c->stream));
-      CU_TRY(c, cudaMemsetAsync(d.d_pair_head, 0xff, 4 * table, c->stream));
-      PairArgs pa{};
-      pa.data = infl_base; pa.rec_off = d.d_rec_off; pa.n_records = (uint32_t)n_rec; pa.key = d.d_pair_key; pa.mate = d.d_pair_mate;
-      pa.next = d.d_pair_next; pa.slot_tag = d.d_pair_tag; pa.slot_head = d.d_pair_head; pa.table_mask = (uint32_t)(table - 1);
-      pa.flags = d.d_cnt + 1;
-      const uint32_t gr = (uint32_t)((n_rec + 255) / 256);
-      kd_pair_keys<<<gr, 256, 0, c->stream>>>(pa);
-      kd_pair_insert<<<gr, 256, 0, c->stream>>>(pa);
-      kd_pair_resolve<<<(uint32_t)((table + 255) / 256), 256, 0, c->stream>>>(pa);
-      CU_TRY(c, cudaGetLastError());
-      out->n_launches += 3;
-      CU_TRY(c, cudaMemcpyAsync(h_cnt, d.d_cnt, 64, cudaMemcpyDeviceToHost, c->stream));
-      CU_TRY(c, cudaStreamSynchronize(c->stream));
-      if (h_cnt[1]) return fail(c, CMB_E_DECLINED, "cmb_submit_bgzf: mate matching gave up (flags %u)", h_cnt[1]);
-      d.last_mate = d.d_pair_mate;
     }
-    CU_TRY(c, cudaEventRecord(d.ev[4], c->stream));
-    if (c->n_local && !decode_only) {
-      // records that start before excl_end_block are this rank's exclusive share of the stream (cmb_kept_tid_range)
-      uint32_t excl_n = 0xffffffffu;
-      if (in->ranged && in->excl_end_block < walk_end) {
-        if (in->excl_end_block <= first_block) excl_n = 0;
-        else {
-          uint64_t base = 0;
-          CU_TRY(c, cudaMemcpyAsync(&base, d.d_rec_base + in->excl_end_block, 8, cudaMemcpyDeviceToHost, c->stream));
-          CU_TRY(c, cudaStreamSynchronize(c->stream));
-          excl_n = (uint32_t)base;
-        }
-      }
-      d.last_excl_n = excl_n;
-      rc = launch_k1(c, tb, (uint32_t)n_rec, (uint32_t)n_cig, excl_n, d.last_mate);
-      if (rc) return rc;
-    }
-  } else {
-    CU_TRY(c, cudaEventRecord(d.ev[4], c->stream));
+    d.last_excl_n = excl_n;
+    if ((rc = launch_k1(c, tb, (uint32_t)n_rec, (uint32_t)n_cig, excl_n, d.last_mate))) return rc;
   }
   CU_TRY(c, cudaEventRecord(d.ev[5], c->stream));
+  return CMB_OK;
+}
+
+int submit_bgzf_impl(cmb_ctx* c, const cmb_bgzf_input* in, cmb_bgzf_result* out, bool decode_only) {
+  NvtxRange nvtx_fn("cmb_submit_bgzf");
+  if (!c || !in || !out || !in->data || !in->block_coffset || !in->block_clen || !in->block_isize)
+    return fail(c, CMB_E_ARG, "cmb_submit_bgzf: null argument");
+  if (!decode_only && !c->in_sample) return fail(c, CMB_E_ARG, "cmb_submit_bgzf: no sample in progress");
+  if (decode_only && (c->in_sample || !c->have_params)) return fail(c, CMB_E_ARG, "cmb_decode_bgzf: set the parameters first; not inside a sample");
+  if (c->n_acquired) return fail(c, CMB_E_ARG, "cmb_submit_bgzf: a staging batch is still acquired");
+  *out = cmb_bgzf_result{};
+  if (in->n_blocks == 0) return CMB_OK;
+  CU_TRY(c, cudaSetDevice(c->device));
+  BgzfCall j{c, c->dec, in, out, decode_only, in->n_blocks};
+  int rc;
+  if ((rc = j.prepare()) || j.nothing_to_decode) return rc;
+  if ((rc = j.copy_inflate()) || (rc = j.declined()) || (rc = j.chain()) || (rc = j.extract())) return rc;
+  auto& d = c->dec;
   CU_TRY(c, cudaEventSynchronize(d.ev[4]));
   cudaEventElapsedTime(&out->ms_copy_inflate, d.ev[0], d.ev[2]);
   cudaEventElapsedTime(&out->ms_chain, d.ev[2], d.ev[3]);
@@ -1949,4 +1722,99 @@ int submit_bgzf_impl(cmb_ctx* c, const cmb_bgzf_input* in, cmb_bgzf_result* out,
   cudaEventElapsedTime(&out->ms_total, d.ev[0], d.ev[4]);
   return CMB_OK;
 }
+
+int bgzf_entry(cmb_ctx* c, const cmb_bgzf_input* in, cmb_bgzf_result* out, bool decode_only) {
+  if (c) {
+    c->dec.last_valid = false;
+    c->dec.filter_planned = false;
+  }
+  const auto t_call0 = std::chrono::steady_clock::now();
+  const int rc = submit_bgzf_impl(c, in, out, decode_only);
+  if (out) out->ms_host_wall = (float)std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_call0).count();
+  if (rc == CMB_E_NOMEM) {
+    cudaGetLastError();
+    auto& d = c->dec;  // give the big buffers back so that the rest of the sample has room
+    d.d_comp.release();
+    d.d_inflated.release();
+    d.d_tuple_slab.release();
+    d.d_rec_off.release();
+    return fail(c, CMB_E_DECLINED, "cmb_submit_bgzf: not enough device memory for device-side decode");
+  }
+  return rc;
+}
 }  // namespace
+
+// Device memory for the decode buffers (compressed file + inflated stream + tuples) is requested before anything is
+// accumulated, so running out of it simply declines the sample: the host decoder needs only the staging batches.
+extern "C" int cmb_last_bgzf_batch(cmb_ctx* c, cmb_read_batch* dev_batch, uint32_t* n_records, uint32_t* n_intervals) {
+  if (!c || !dev_batch || !n_records || !n_intervals) return fail(c, CMB_E_ARG, "cmb_last_bgzf_batch: null argument");
+  if (!c->dec.last_valid || !c->dec.d_tuple_slab) return fail(c, CMB_E_ARG, "cmb_last_bgzf_batch: no device-decoded sample is resident");
+  carve_batch(c->dec.d_tuple_slab, c->dec.last_n_rec, c->dec.last_n_cig, dev_batch);
+  *n_records = c->dec.last_n_rec;
+  *n_intervals = c->dec.last_n_cig;
+  return CMB_OK;
+}
+
+extern "C" int cmb_submit_bgzf(cmb_ctx* c, const cmb_bgzf_input* in, cmb_bgzf_result* out) { return bgzf_entry(c, in, out, false); }
+extern "C" int cmb_decode_bgzf(cmb_ctx* c, const cmb_bgzf_input* in, cmb_bgzf_result* out) { return bgzf_entry(c, in, out, true); }
+
+extern "C" int cmb_filter_plan(cmb_ctx* c, int inverse, uint64_t* n_records, uint64_t* n_bytes) {
+  if (!c || !n_records || !n_bytes) return fail(c, CMB_E_ARG, "cmb_filter_plan: null argument");
+  auto& d = c->dec;
+  if (!d.last_valid || !d.d_tuple_slab || !c->have_params) return fail(c, CMB_E_ARG, "cmb_filter_plan: no device-decoded sample is resident (cmb_decode_bgzf first)");
+  CU_TRY(c, cudaSetDevice(c->device));
+  *n_records = 0;
+  *n_bytes = 0;
+  d.filter_planned = false;
+  const uint32_t n = d.last_n_rec;
+  if (n == 0) {
+    d.filter_bytes = 0;
+    d.filter_planned = true;
+    return CMB_OK;
+  }
+  const bool pair_path = !(c->mode.filter_single_reads && !c->mode.filter_pairs);
+  if (pair_path && !d.last_mate) return fail(c, CMB_E_ARG, "cmb_filter_plan: the sample was decoded without mate matching (set the parameters before cmb_decode_bgzf)");
+  int rc;
+  if ((rc = d.d_filter_anchor.ensure(c, (size_t)n + 1, with_slack(n))) || (rc = d.d_filter_role.ensure(c, (size_t)n + 1, with_slack(n))))
+    return rc;
+  cmb_read_batch tb;
+  carve_batch(d.d_tuple_slab, d.last_n_rec, d.last_n_cig, &tb);
+  FilterArgs a{};
+  a.data = d.last_infl_base; a.rec_off = d.d_rec_off; a.n = n; a.flag = tb.flag; a.mapq = tb.mapq; a.nm_state = tb.nm_state; a.nm = tb.nm;
+  a.l_seq = tb.l_seq; a.aligned = tb.aligned; a.del = tb.del; a.mate = pair_path ? d.last_mate : nullptr; a.p = c->params;
+  a.filter_single = c->mode.filter_single_reads; a.pair_path = pair_path; a.filter_out = inverse ? 0 : 1;
+  a.anchor_bytes = d.d_filter_anchor; a.role = d.d_filter_role; a.error_flags = d.d_cnt + 12; a.n_emit = (unsigned long long*)(d.d_cnt + 14);
+  CU_TRY(c, cudaMemsetAsync(d.d_cnt + 12, 0, 16, c->stream));
+  kf_decide<<<(n + 255) / 256, 256, 0, c->stream>>>(a);
+  kf_scan<<<1, 1024, 0, c->stream>>>(d.d_filter_anchor, n);
+  CU_TRY(c, cudaGetLastError());
+  uint32_t h[4];
+  unsigned long long total = 0;
+  CU_TRY(c, cudaMemcpyAsync(h, d.d_cnt + 12, 16, cudaMemcpyDeviceToHost, c->stream));
+  CU_TRY(c, cudaMemcpyAsync(&total, d.d_filter_anchor + n, 8, cudaMemcpyDeviceToHost, c->stream));
+  CU_TRY(c, cudaStreamSynchronize(c->stream));
+  if (h[0] & ERR_NM)
+    return fail(c, CMB_E_NM, "Mapping record encountered that does not have an 'NM' auxiliary tag in the SAM/BAM format. This is required to work out some coverage statistics");
+  unsigned long long n_emit;
+  memcpy(&n_emit, h + 2, 8);
+  if ((rc = d.d_filter_out.ensure(c, total, (size_t)total + (size_t)total / 8 + 4096))) return rc;
+  a.out = d.d_filter_out;
+  kf_gather<<<(n + 7) / 8, 256, 0, c->stream>>>(a);
+  CU_TRY(c, cudaGetLastError());
+  d.filter_bytes = total;
+  d.filter_planned = true;
+  *n_records = n_emit;
+  *n_bytes = total;
+  return CMB_OK;
+}
+
+extern "C" int cmb_filter_fetch(cmb_ctx* c, uint8_t* records, uint64_t n_bytes) {
+  if (!c || (!records && n_bytes)) return fail(c, CMB_E_ARG, "cmb_filter_fetch: null argument");
+  auto& d = c->dec;
+  if (!d.filter_planned || n_bytes != d.filter_bytes) return fail(c, CMB_E_ARG, "cmb_filter_fetch: call cmb_filter_plan first and pass the size it reported");
+  CU_TRY(c, cudaSetDevice(c->device));
+  if (n_bytes) CU_TRY(c, cudaMemcpyAsync(records, d.d_filter_out, n_bytes, cudaMemcpyDeviceToHost, c->stream));
+  CU_TRY(c, cudaStreamSynchronize(c->stream));
+  return CMB_OK;
+}
+

@@ -156,16 +156,16 @@ def test_host_decode_path_matches_oracle(synth, which, argv):
     assert any(l.startswith("#pipeline") for l in g.stderr.splitlines())
 
 
-INFLATE_MODES = [(k, m) for k in ("t1", "g8", "w1") for m in ("persistent", "serial")] + [("t1", "windows")]
+INFLATE_MODES = [(k, m) for k in ("t1", "g8", "w1") for m in ("persistent", "serial")]
 
 
 @pytest.mark.parametrize("kernel,mode", INFLATE_MODES, ids=[f"{k}-{m}" for k, m in INFLATE_MODES])
 def test_every_inflate_kernel_and_launch_mode_matches_zlib(synth, kernel, mode):
-    """The three inflate kernels (thread / eight lanes / warp per block) under the three launch disciplines: one persistent launch
-    whose lanes wait for their window's arrival flag (64 KB windows here, so that a small file spans many), one launch ordered
-    behind all the copies (what runs under ncu / compute-sanitizer and for single-window files), one launch per window."""
+    """The three inflate kernels (thread / eight lanes / warp per block) under both launch disciplines: one persistent launch
+    whose lanes wait for their window's arrival flag (64 KB windows here, so that a small file spans many), and one launch
+    ordered behind all the copies (what runs under ncu / compute-sanitizer and for single-window files)."""
     env = {"CMB_PIPELINE_STATS": "1", "CMB_DECODE_VERIFY": "1", "CMB_INFLATE": kernel, "CMB_DECODE_WINDOW_KB": "64",
-           "CMB_INFLATE_SERIAL": "1" if mode == "serial" else "0", "CMB_INFLATE_WINDOWS": "1" if mode == "windows" else "0"}
+           "CMB_INFLATE_SERIAL": "1" if mode == "serial" else "0"}
     for which in ("small", "mags"):
         g = _assert_same(["contig", "-m", "mean", "trimmed_mean", "count", "-b", synth[which]], env=env)
         st = _decode_stats(g)
@@ -326,6 +326,26 @@ def test_coverm_filter_on_the_device(synth, tmp_path, which, extra):
     assert outs[0][1] == outs[1][1]
     by_bytes = set(in_recs)
     assert all(r in by_bytes for r in outs[0][1][:2000])
+
+
+@pytest.mark.parametrize("extra", [[], ["--inverse"]], ids=["kept", "inverse"])
+def test_coverm_filter_over_several_inputs(synth, tmp_path, extra):
+    """`coverm filter -b tiny small deep -o ...` on the pair path: the inputs hold 60 k, 200 k and 600 k records, so the one
+    device context's mate-matching arrays grow twice between inputs while the filter's buffers of the previous input exist.
+    Every output holds exactly the records the oracle returns for its input alone."""
+    which = ["tiny", "small", "deep"]
+    outs = [str(tmp_path / f"{w}.bam") for w in which]
+    flt = ["--proper-pairs-only", "--min-read-aligned-length-pair", "250"] + extra
+    p = subprocess.run([coverm_b200.COVERM_BIN, "filter", "-b"] + [synth[w] for w in which] + ["-o"] + outs + ["-t", "8", "--timing"] + flt,
+                       capture_output=True, text=True, timeout=900)
+    assert p.returncode == 0, p.stderr[-800:]
+    for k, (w, out) in enumerate(zip(which, outs)):
+        assert any(l.startswith(f"#filter\tsample={k}\t") and l.endswith("device=1") for l in p.stderr.splitlines()), p.stderr[-800:]
+        names = subprocess.run([ORACLE_BIN, "filter-names", "-b", synth[w]] + flt, capture_output=True, text=True, timeout=900)
+        assert names.returncode == 0, names.stderr[-500:]
+        header, recs = _bam_records(out)
+        assert header == _bam_records(synth[w])[0]
+        assert [r[36:36 + r[12] - 1].decode() for r in recs] == names.stdout.split("\n")[:-1], w
 
 
 def test_histogram_buffer_overflow_grows_and_retries(synth):
