@@ -399,16 +399,37 @@ int launch_k1(cmb_ctx* c, const cmb_read_batch& b, uint32_t n_records, uint32_t 
   return CMB_OK;
 }
 
+// CTAs of k2_scan_reduce<HIST, CLEAN> that fit on one SM (K2 is persistent: it launches that many per SM)
 template <bool HIST, bool CLEAN>
-int launch_k2_variant(cmb_ctx* c, const K2Args& a) {
+int k2_blocks_per_sm(cmb_ctx* c, int* occ) {
   auto kern = k2_scan_reduce<HIST, CLEAN>;
   constexpr uint32_t smem_bytes = HIST ? K2_SMEM_BYTES_HIST : K2_SMEM_BYTES_NOHIST;
   CU_TRY(c, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
+  *occ = 0;
+  CU_TRY(c, cudaOccupancyMaxActiveBlocksPerMultiprocessor(occ, kern, (int)K2_THREADS, smem_bytes));
+  if (*occ < 1) return fail(c, CMB_E_CUDA, "k2_scan_reduce does not fit on an SM");
+  return CMB_OK;
+}
+
+// Histogram records K2 may reserve beyond those it writes: every warp of the largest histogram launch can leave up to one
+// run (K2_REC_RUN) unused.
+int k2_rec_slack(cmb_ctx* c, uint64_t* slack) {
+  int o1 = 0, o2 = 0;
+  if (int rc = k2_blocks_per_sm<true, true>(c, &o1)) return rc;
+  if (int rc = k2_blocks_per_sm<true, false>(c, &o2)) return rc;
+  *slack = (uint64_t)std::max(o1, o2) * c->sm_count * K2_WARPS * K2_REC_RUN;
+  return CMB_OK;
+}
+
+template <bool HIST, bool CLEAN>
+int launch_k2_variant(cmb_ctx* c, const K2Args& a) {
   int occ = 0;
-  CU_TRY(c, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, (int)K2_THREADS, smem_bytes));
-  if (occ < 1) return fail(c, CMB_E_CUDA, "k2_scan_reduce does not fit on an SM");
+  if (int rc = k2_blocks_per_sm<HIST, CLEAN>(c, &occ)) return rc;
   const uint32_t grid = std::min<uint32_t>(c->n_chunks, (uint32_t)(occ * c->sm_count));
-  kern<<<grid, K2_THREADS, smem_bytes, c->stream>>>(c->tmap, a);
+  if (getenv("CMB_PIPELINE_STATS"))
+    fprintf(stderr, "#k2_grid\tgrid=%u\tblocks_per_sm=%d\tsms=%d\thist=%d\tclean=%d\n", grid, occ, c->sm_count, (int)HIST, (int)CLEAN);
+  constexpr uint32_t smem_bytes = HIST ? K2_SMEM_BYTES_HIST : K2_SMEM_BYTES_NOHIST;
+  k2_scan_reduce<HIST, CLEAN><<<grid, K2_THREADS, smem_bytes, c->stream>>>(c->tmap, a);
   CU_TRY(c, cudaGetLastError());
   return CMB_OK;
 }
@@ -706,7 +727,10 @@ int cmb_set_reference(cmb_ctx* c, uint32_t n_contigs, const uint64_t* contig_len
   CU_TRY(c, cudaMemcpyAsync(r.d_chunk_first, chunk_first.data(), 4ull * (c->n_chunks + 1), cudaMemcpyHostToDevice, c->stream));
   CU_TRY(c, cudaStreamSynchronize(c->stream));
   // histogram record buffers: one 8 B record per 8 arena elements is far above anything a real sample produces
-  uint64_t rec_cap = std::min<uint64_t>(0xfffffff0ull, std::max<uint64_t>(1u << 20, c->arena_elems / 8));
+  // (plus the runs K2's warps may leave unused)
+  uint64_t rec_slack = 0;
+  if ((rc = k2_rec_slack(c, &rec_slack))) return rc;
+  uint64_t rec_cap = std::min<uint64_t>(0xfffffff0ull, std::max<uint64_t>(1u << 20, c->arena_elems / 8) + rec_slack);
   uint64_t ovf_cap = std::min<uint64_t>(1u << 26, std::max<uint64_t>(1u << 20, c->arena_elems / 64));
   if (getenv("CMB_TEST_SMALL_HIST")) {  // testing aid: buffers that overflow at once (cmb_grow_buffers path)
     rec_cap = 256;
@@ -909,7 +933,9 @@ int cmb_grow_buffers(cmb_ctx* c) {
   CU_TRY(c, cudaStreamSynchronize(c->stream));
   auto& r = c->ref;  // the next sample rebuilds what these hold
   int rc;
-  if ((rc = r.d_rec.ensure(c, std::min<uint64_t>(0xfffffff0ull, (uint64_t)r.d_rec.cap * 4))) ||
+  uint64_t rec_slack = 0;
+  if ((rc = k2_rec_slack(c, &rec_slack))) return rc;
+  if ((rc = r.d_rec.ensure(c, std::min<uint64_t>(0xfffffff0ull, (uint64_t)r.d_rec.cap * 4 + rec_slack))) ||
       (rc = r.d_ovf.ensure(c, std::min<uint64_t>(1ull << 30, (uint64_t)r.d_ovf.cap * 4))) ||
       (r.d_pairs && (rc = r.d_pairs.ensure(c, r.d_pairs.cap * 4))))
     return rc;

@@ -45,6 +45,11 @@ struct K2Args {
 #endif
 constexpr uint32_t K2_DENSE_SPANS = CMB_K2_DENSE_SPANS;
 static_assert(K2_STAGES >= 2, "the refill of a stage is issued one iteration after it was read");
+// Histogram records a warp reserves in `rec` at a time, instead of one global atomic per (chunk, contig slot) on a counter
+// that every warp of the grid shares.  A run holds any slot (at most HIST_BINS records); a warp leaves at most one run
+// unused at the end and fewer than HIST_BINS records per refill.
+constexpr uint32_t K2_REC_RUN = 512;
+static_assert(K2_REC_RUN >= HIST_BINS, "a run must hold the records of one slot");
 
 constexpr uint32_t K2_SMEM_STAGE_BYTES = K2_STAGES * CHUNK_BYTES;
 constexpr uint32_t K2_SMEM_MISC = 64 /*barriers*/ + 2 * K2_WARPS * 8 /*warp aggregates, double-buffered*/;
@@ -119,6 +124,10 @@ __global__ void __launch_bounds__(K2_THREADS, CMB_K2_MINBLOCKS) k2_scan_reduce(c
     return have;
   };
 
+  // Each warp writes its records into a private run of `rec` (K2_REC_RUN records) that it reserves with one global atomic
+  // when the run cannot take a slot's records; K3 reads the records only through warp_table, so the unused ends of the runs
+  // are never read.  run_base = ~0u: a reservation did not fit (ERR_CAPACITY is set, the host grows `rec` and retries).
+  uint32_t run_base = 0, run_left = 0;  // warp-uniform
   // flush one histogram buffer: a warp takes contig slots warp, warp + K2_WARPS, ... (128 bins, 4 per lane) -> (depth,count) records
   auto flush_hist = [&](uint32_t* hist, uint32_t chunk, uint32_t n_slots) {
     for (uint32_t sl = warp; sl < HIST_SLOTS && sl < n_slots; sl += K2_WARPS) {
@@ -131,9 +140,20 @@ __global__ void __launch_bounds__(K2_THREADS, CMB_K2_MINBLOCKS) k2_scan_reduce(c
       }
       uint32_t base = 0;
       if (total) {
-        if (lane == 0) base = atomicAdd(a.rec_count, total);
-        base = __shfl_sync(FULL, base, 0);
-        const bool fits = (uint64_t)base + total <= a.rec_capacity;
+        if (total > run_left && run_base != ~0u) {  // the run cannot take this slot: reserve the next one
+          uint32_t b = 0;
+          if (lane == 0) b = atomicAdd(a.rec_count, K2_REC_RUN);
+          b = __shfl_sync(FULL, b, 0);
+          const bool ok = (uint64_t)b + K2_REC_RUN <= a.rec_capacity;
+          run_base = ok ? b : ~0u;
+          run_left = ok ? K2_REC_RUN : 0u;
+        }
+        const bool fits = total <= run_left;
+        base = run_base;
+        if (fits) {
+          run_base += total;
+          run_left -= total;
+        }
         if (!fits && lane == 0) atomicOr(a.error_flags, ERR_CAPACITY);
         uint32_t before = 0;
 #pragma unroll
