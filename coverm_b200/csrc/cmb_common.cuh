@@ -17,20 +17,10 @@ constexpr uint32_t K2_WARPS = K2_THREADS / 32;  // 8 = span-bitmap words per chu
 // Span occupancy bitmap: one bit per span (K1 sets it for every event it adds), so one u32 word per warp of K2 spans.
 constexpr uint32_t BITMAP_SPANS_PER_WORD = 32;
 constexpr uint32_t BITMAP_ELEMS_PER_WORD = BITMAP_SPANS_PER_WORD * SPAN;  // 1024
-#ifndef CMB_HIST_SLOTS
-#define CMB_HIST_SLOTS 8
-#endif
 #ifndef CMB_K2_MINBLOCKS
 #define CMB_K2_MINBLOCKS 3
 #endif
-constexpr uint32_t HIST_SLOTS = CMB_HIST_SLOTS;             // contigs per chunk with a shared-memory histogram
-constexpr uint32_t HIST_BINS = 128;             // direct-mapped bins per slot: bin = depth % 128, word = tag|count
-constexpr uint32_t HIST_TOTAL = HIST_SLOTS * HIST_BINS;  // 2048
-constexpr uint32_t HIST_CNT_BITS = 14;          // a chunk holds 8192 = 2^13 positions, so a count fits 14 bits
-constexpr uint32_t HIST_MAX_DEPTH = ((1u << (32 - HIST_CNT_BITS)) - 2) * HIST_BINS;  // deeper runs use the overflow list
-constexpr uint32_t OVF_NIL = 0xffffffffu;
 constexpr uint32_t K1_THREADS = 256;
-constexpr uint32_t ROWFLAG_OVF = 1u;            // cmb_contig_stats.reserved: some records are in the overflow list
 
 // error_flags bits (device)
 constexpr uint32_t ERR_UNSORTED = 1u, ERR_NM = 2u, ERR_BOUNDS = 4u, ERR_CAPACITY = 8u, ERR_TID = 16u, ERR_INTERNAL = 32u;

@@ -12,20 +12,23 @@
 //   tail_sum     i32[n_chunks]      K1: sum of the deltas of the contig that continues past the chunk end
 //   carry_in     i32[n_chunks]      K1b: running depth at the first element of each chunk
 //   rows         cmb_contig_stats[n_contigs]
-//   rec / warp_table / ovf          K2 -> K3 histogram records
+//   bin_base     u64[n_local+1]     K1b: first bin of each contig in `bins` (read count + 1 bins for a contig with a window)
+//   bins         u32[pool]          K2 -> K3 window depth histogram, bins[bin_base[c] + depth]; zero between samples (K3
+//                                   re-zeroes what it reads); bin_hi u32[n_local] = highest depth K2 added per contig
 //
 // Kernels (all HBM-bound integer work, no tensor cores):
 //   K1  k1_filter_accumulate  one thread per record: FlagFilter + ReferenceSortedBamFilter predicates
 //                             (lib.rs:59-79, filter.rs:243-336), per-contig read counters (contig.rs:157-211),
 //                             +1/-1 delta REDs into the arena (contig.rs:166-202), chunk tail sums.
-//   K1b k1b_chunk_carry       segmented scan of the per-chunk tail sums -> carry_in (so K2 needs no look-back).
+//   K1b k1b_local/apply       segmented scan of the per-chunk tail sums -> carry_in (so K2 needs no look-back), and the
+//                             exclusive scan of the contigs' bin counts -> bin_base, in the same two launches.
 //   K2  k2_scan_reduce        persistent CTAs, ring of 32 KB chunks: whole-tile TMA (cp.async.bulk.tensor, 128B swizzle)
 //                             + mbarrier for chunks with many non-empty spans, cp.async of just the non-empty 128-B rows
 //                             for the others; blocked 32-element spans per thread, warp-shuffle segmented scan, then every
 //                             O(L) reduction of EST:366-502 in one pass: sum/covered over the end-trimmed window,
-//                             covered over the full contig, window depth histogram into a shared-memory table that
-//                             is flushed as (depth,count) records; optionally re-zeroes the arena as it goes.
-//   K3  k3_finalize           per contig: merge the records, trimmed-mean walk (EST:598-642) and the variance sums
+//                             covered over the full contig, window depth histogram as REDs into the contig's bins;
+//                             optionally re-zeroes the arena as it goes.
+//   K3  k3_finalize           per contig: walk its bins, trimmed-mean walk (EST:598-642) and the variance sums
 //                             (EST:790-805) in integers; optional CSR histogram output.
 //   KD* kd_inflate ...        device-side BAM decode behind cmb_submit_bgzf (cmb_decode.cuh): BGZF inflate, record chain,
 //                             tuple extraction -- the compressed file crosses PCIe instead of tuples.
@@ -181,16 +184,16 @@ struct cmb_ctx {
     Buf<int32_t> d_tail_sum, d_carry_in;
     Buf<int2> d_block_agg;
     Buf<cmb_contig_stats> d_rows;
-    Buf<uint2> d_rec;  // K2 -> K3 histogram records; cap is the capacity K2 is given
-    Buf<uint2> d_warp_table;
-    Buf<uint4> d_ovf;
-    Buf<uint32_t> d_ovf_head;
+    Buf<uint32_t> d_bins;  // K2 -> K3 histogram bin pool; cap is the capacity K2 is given.  Zero outside a sample
+    Buf<uint64_t> d_bin_base, d_bin_block_sum;
+    Buf<uint32_t> d_bin_hi;
     Buf<cmb_hist_pair> d_pairs;  // CSR histogram pairs (CMB_WANT_HIST_CSR)
     // gene mode (cmb_set_genes): segments are genes; records carry contig tids
     Buf<uint32_t> d_gene_first, d_gene_start, d_gene_end, d_gene_maxlen, d_contig_len32;
     Buf<uint8_t> d_contig_seen;
+    Buf<uint32_t> d_gene_bound;
   } ref;
-  Buf<uint32_t> d_counters;  // 16 words: [0] error flags, [2] rec_count, [3] ovf_count, [4..5] pair_count (u64),
+  Buf<uint32_t> d_counters;  // 16 words: [0] error flags, [4..5] pair_count (u64),
                              // [6..7] kept tid range of the exclusive records (K1Args::kept_range), [8..9] gene mode
                              // kept primaries (u64), [10..11] K2 spans loaded / chunks loaded whole
   uint32_t kept_range[2] = {0, 0};  // host copy after cmb_end_sample*
@@ -208,6 +211,7 @@ struct cmb_ctx {
   uint32_t n_ref_contigs = 0;  // contigs of the BAM header (== n_contigs outside gene mode)
   CUtensorMap tmap{};
   bool arena_dirty = true;
+  bool pool_dirty = false;  // a sample ended with an error: bins / bin_hi may hold counts (cmb_begin_sample zeroes them)
   bool clean_as_you_go = true;
   // params
   cmb_params params{};
@@ -370,6 +374,7 @@ int launch_k1(cmb_ctx* c, const cmb_read_batch& b, uint32_t n_records, uint32_t 
   if (c->gene_mode) {
     a.gene_first = r.d_gene_first; a.gene_start = r.d_gene_start; a.gene_end = r.d_gene_end; a.gene_maxlen = r.d_gene_maxlen;
     a.contig_len = r.d_contig_len32; a.contig_seen = r.d_contig_seen; a.kept_primary = (unsigned long long*)(c->d_counters + 8);
+    a.gene_bound = r.d_gene_bound;
   }
   a.arena = r.d_arena; a.span_bits = r.d_span_bits; a.tail_sum = r.d_tail_sum; a.rows = r.d_rows;
   a.block_minmax = c->d_block_minmax + c->block_minmax_used;
@@ -403,21 +408,10 @@ int launch_k1(cmb_ctx* c, const cmb_read_batch& b, uint32_t n_records, uint32_t 
 template <bool HIST, bool CLEAN>
 int k2_blocks_per_sm(cmb_ctx* c, int* occ) {
   auto kern = k2_scan_reduce<HIST, CLEAN>;
-  constexpr uint32_t smem_bytes = HIST ? K2_SMEM_BYTES_HIST : K2_SMEM_BYTES_NOHIST;
-  CU_TRY(c, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
+  CU_TRY(c, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)K2_SMEM_BYTES));
   *occ = 0;
-  CU_TRY(c, cudaOccupancyMaxActiveBlocksPerMultiprocessor(occ, kern, (int)K2_THREADS, smem_bytes));
+  CU_TRY(c, cudaOccupancyMaxActiveBlocksPerMultiprocessor(occ, kern, (int)K2_THREADS, K2_SMEM_BYTES));
   if (*occ < 1) return fail(c, CMB_E_CUDA, "k2_scan_reduce does not fit on an SM");
-  return CMB_OK;
-}
-
-// Histogram records K2 may reserve beyond those it writes: every warp of the largest histogram launch can leave up to one
-// run (K2_REC_RUN) unused.
-int k2_rec_slack(cmb_ctx* c, uint64_t* slack) {
-  int o1 = 0, o2 = 0;
-  if (int rc = k2_blocks_per_sm<true, true>(c, &o1)) return rc;
-  if (int rc = k2_blocks_per_sm<true, false>(c, &o2)) return rc;
-  *slack = (uint64_t)std::max(o1, o2) * c->sm_count * K2_WARPS * K2_REC_RUN;
   return CMB_OK;
 }
 
@@ -428,17 +422,27 @@ int launch_k2_variant(cmb_ctx* c, const K2Args& a) {
   const uint32_t grid = std::min<uint32_t>(c->n_chunks, (uint32_t)(occ * c->sm_count));
   if (getenv("CMB_PIPELINE_STATS"))
     fprintf(stderr, "#k2_grid\tgrid=%u\tblocks_per_sm=%d\tsms=%d\thist=%d\tclean=%d\n", grid, occ, c->sm_count, (int)HIST, (int)CLEAN);
-  constexpr uint32_t smem_bytes = HIST ? K2_SMEM_BYTES_HIST : K2_SMEM_BYTES_NOHIST;
-  k2_scan_reduce<HIST, CLEAN><<<grid, K2_THREADS, smem_bytes, c->stream>>>(c->tmap, a);
+  k2_scan_reduce<HIST, CLEAN><<<grid, K2_THREADS, K2_SMEM_BYTES, c->stream>>>(c->tmap, a);
   CU_TRY(c, cudaGetLastError());
   return CMB_OK;
 }
+
+// The bin pool holds at least `need` counts.  A new pool is zeroed: K2 only adds to it and K3 re-zeroes what it read.
+int ensure_pool(cmb_ctx* c, uint64_t need, uint64_t alloc) {
+  auto& r = c->ref;
+  if (r.d_bins.cap >= need) return CMB_OK;
+  if (int rc = r.d_bins.ensure(c, need, alloc)) return rc;
+  CU_TRY(c, cudaMemsetAsync(r.d_bins, 0, 4 * r.d_bins.cap, c->stream));
+  return CMB_OK;
+}
+
+bool small_hist() { return getenv("CMB_TEST_SMALL_HIST") != nullptr; }  // testing aid: no pre-sizing (cmb_grow_buffers path)
 
 int run_end_of_sample(cmb_ctx* c) {
   const bool hist = c->params.want & (CMB_WANT_HIST | CMB_WANT_HIST_CSR);
   const bool csr = c->params.want & CMB_WANT_HIST_CSR;
   const uint32_t excl = (uint32_t)std::min<uint64_t>(c->params.contig_end_exclusion, 0x7fffffffu);
-  const auto& r = c->ref;
+  auto& r = c->ref;
   CU_TRY(c, cudaEventRecord(c->ev[2], c->stream));
   if (c->block_minmax_used) {
     k1c_check_sorted<<<1, 1024, 0, c->stream>>>(c->d_block_minmax, c->block_minmax_used, c->d_counters + 0,
@@ -446,20 +450,32 @@ int run_end_of_sample(cmb_ctx* c) {
     CU_TRY(c, cudaGetLastError());
   }
   {
-    const uint32_t blocks = (c->n_chunks + K1B_BLOCK - 1) / K1B_BLOCK;
-    k1b_local<<<blocks, K1B_THREADS, 0, c->stream>>>(r.d_tail_sum, r.d_chunk_first, r.d_off_span, c->n_chunks, r.d_carry_in, r.d_block_agg);
+    K1bBins g{};
+    g.len = r.d_len; g.rows = r.d_rows + c->tid_begin; g.gene_bound = c->gene_mode ? r.d_gene_bound.p : nullptr;
+    g.n_seg = c->n_local; g.excl = excl; g.bin_base = r.d_bin_base; g.block_sum = r.d_bin_block_sum;
+    g.n_blocks = hist ? c->n_local / K1B_BLOCK + 1 : 0;  // n_local + 1 entries
+    const uint32_t blocks = (c->n_chunks + K1B_BLOCK - 1) / K1B_BLOCK + g.n_blocks;
+    k1b_local<<<blocks, K1B_THREADS, 0, c->stream>>>(r.d_tail_sum, r.d_chunk_first, r.d_off_span, c->n_chunks, r.d_carry_in, r.d_block_agg, g);
     CU_TRY(c, cudaGetLastError());
-    k1b_apply<<<blocks, K1B_THREADS, 0, c->stream>>>(r.d_tail_sum, r.d_block_agg, c->n_chunks, r.d_carry_in);
+    k1b_apply<<<blocks, K1B_THREADS, 0, c->stream>>>(r.d_tail_sum, r.d_block_agg, c->n_chunks, r.d_carry_in, g);
     CU_TRY(c, cudaGetLastError());
+  }
+  if (hist && !small_hist()) {
+    // Contig mode: a contig's bins are its read count + 1, and the records submitted bound the read counts together.  Gene
+    // mode: a read also covers the genes it starts before, so the pool size is read back (one round trip).
+    uint64_t need = c->n_records + c->n_local + 1;
+    if (c->gene_mode) {
+      CU_TRY(c, cudaMemcpyAsync(&need, r.d_bin_base + c->n_local, 8, cudaMemcpyDeviceToHost, c->stream));
+      CU_TRY(c, cudaStreamSynchronize(c->stream));
+    }
+    if (int rc = ensure_pool(c, need, with_slack(need))) return rc;
   }
   K2Args a{};
   a.off_span = r.d_off_span; a.len = r.d_len; a.chunk_first = r.d_chunk_first; a.carry_in = r.d_carry_in;
   a.rows = r.d_rows; a.tid_begin = c->tid_begin; a.n_local = c->n_local; a.n_chunks = c->n_chunks; a.excl = excl;
   a.arena = r.d_arena; a.span_bits = r.d_span_bits; a.load_stats = c->d_counters + 10;
-  a.rec = r.d_rec; a.rec_capacity = (uint32_t)r.d_rec.cap; a.rec_count = c->d_counters + 2;
-  a.warp_table = r.d_warp_table; a.ovf = r.d_ovf; a.ovf_head = r.d_ovf_head; a.ovf_capacity = (uint32_t)r.d_ovf.cap; a.ovf_count = c->d_counters + 3;
+  a.bin_base = r.d_bin_base; a.bins = r.d_bins; a.pool_cap = r.d_bins.cap; a.bin_hi = r.d_bin_hi;
   a.error_flags = c->d_counters + 0;
-  if (hist) CU_TRY(c, cudaMemsetAsync(r.d_ovf_head, 0xff, 4ull * c->n_chunks, c->stream));
   CU_TRY(c, cudaEventRecord(c->ev[3], c->stream));
   int rc;
   if (hist) rc = c->clean_as_you_go ? launch_k2_variant<true, true>(c, a) : launch_k2_variant<true, false>(c, a);
@@ -470,11 +486,10 @@ int run_end_of_sample(cmb_ctx* c) {
   CU_TRY(c, cudaEventRecord(c->ev[4], c->stream));
   if (hist) {
     K3Args k{};
-    k.off_span = r.d_off_span; k.len = r.d_len; k.chunk_first = r.d_chunk_first; k.rows = r.d_rows;
+    k.len = r.d_len; k.rows = r.d_rows;
     k.tid_begin = c->tid_begin; k.n_local = c->n_local; k.excl = excl;
     k.trim_min = c->params.trim_min; k.trim_max = c->params.trim_max;
-    k.rec = r.d_rec; k.warp_table = r.d_warp_table; k.ovf = r.d_ovf; k.ovf_head = r.d_ovf_head;
-    k.ovf_capacity = (uint32_t)r.d_ovf.cap;
+    k.bin_base = r.d_bin_base; k.bins = r.d_bins; k.pool_cap = r.d_bins.cap; k.bin_hi = r.d_bin_hi;
     k.pairs = r.d_pairs; k.pair_count = (unsigned long long*)(c->d_counters + 4); k.pair_capacity = r.d_pairs.cap;
     k.want_csr = csr; k.all_rows = c->gene_mode ? 1u : 0u; k.error_flags = c->d_counters + 0;
     const uint32_t grid = (c->n_local + K3_WARPS - 1) / K3_WARPS;  // one warp per contig
@@ -519,8 +534,10 @@ int collect_errors_and_timing(cmb_ctx* c, uint32_t* counters_out) {
   if (e & ERR_NM)
     return fail(c, CMB_E_NM, "Mapping record encountered that does not have an 'NM' auxiliary tag in the SAM/BAM format. This is required to work out some coverage statistics");
   if (e & (ERR_BOUNDS | ERR_TID)) return fail(c, CMB_E_BOUNDS, "index out of bounds: an aligned block starts beyond the end of its reference sequence");
-  if (e & ERR_CAPACITY) return fail(c, CMB_E_CAPACITY, "device histogram record buffer overflowed");
-  if (e & ERR_INTERNAL) return fail(c, CMB_E_CUDA, "internal error: negative running depth (inconsistent delta arena)");
+  if (e & ERR_CAPACITY) return fail(c, CMB_E_CAPACITY, "device histogram bin pool or pair buffer overflowed");
+  if (e & ERR_INTERNAL)
+    return fail(c, CMB_E_CUDA, "internal error: running depth below 0 or above the read count (inconsistent delta arena, or a "
+                "record whose aligned blocks overlap)");
   return CMB_OK;
 }
 
@@ -655,7 +672,8 @@ int cmb_set_genes(cmb_ctx* c, uint32_t n_contigs, const uint64_t* contig_len, ui
   auto& r = c->ref;
   const size_t n_ctg = std::max<uint32_t>(1, n_contigs);
   if ((rc = r.d_gene_first.ensure(c, (size_t)n_contigs + 1)) || (rc = r.d_gene_start.ensure(c, n_seg)) || (rc = r.d_gene_end.ensure(c, n_seg)) ||
-      (rc = r.d_gene_maxlen.ensure(c, n_ctg)) || (rc = r.d_contig_len32.ensure(c, n_ctg)) || (rc = r.d_contig_seen.ensure(c, n_ctg)))
+      (rc = r.d_gene_maxlen.ensure(c, n_ctg)) || (rc = r.d_contig_len32.ensure(c, n_ctg)) || (rc = r.d_contig_seen.ensure(c, n_ctg)) ||
+      (rc = r.d_gene_bound.ensure(c, n_seg)))
     return rc;
   CU_TRY(c, cudaMemcpyAsync(r.d_gene_first, first.data(), 4ull * (n_contigs + 1), cudaMemcpyHostToDevice, c->stream));
   CU_TRY(c, cudaMemcpyAsync(r.d_gene_start, gs.data(), 4ull * n_seg, cudaMemcpyHostToDevice, c->stream));
@@ -726,19 +744,14 @@ int cmb_set_reference(cmb_ctx* c, uint32_t n_contigs, const uint64_t* contig_len
   CU_TRY(c, cudaMemcpyAsync(r.d_len, len.data(), 4ull * c->n_local, cudaMemcpyHostToDevice, c->stream));
   CU_TRY(c, cudaMemcpyAsync(r.d_chunk_first, chunk_first.data(), 4ull * (c->n_chunks + 1), cudaMemcpyHostToDevice, c->stream));
   CU_TRY(c, cudaStreamSynchronize(c->stream));
-  // histogram record buffers: one 8 B record per 8 arena elements is far above anything a real sample produces
-  // (plus the runs K2's warps may leave unused)
-  uint64_t rec_slack = 0;
-  if ((rc = k2_rec_slack(c, &rec_slack))) return rc;
-  uint64_t rec_cap = std::min<uint64_t>(0xfffffff0ull, std::max<uint64_t>(1u << 20, c->arena_elems / 8) + rec_slack);
-  uint64_t ovf_cap = std::min<uint64_t>(1u << 26, std::max<uint64_t>(1u << 20, c->arena_elems / 64));
-  if (getenv("CMB_TEST_SMALL_HIST")) {  // testing aid: buffers that overflow at once (cmb_grow_buffers path)
-    rec_cap = 256;
-    ovf_cap = 64;
-  }
-  if ((rc = r.d_rec.ensure(c, rec_cap)) || (rc = r.d_warp_table.ensure(c, (size_t)c->n_chunks * HIST_SLOTS)) ||
-      (rc = r.d_ovf.ensure(c, ovf_cap)) || (rc = r.d_ovf_head.ensure(c, c->n_chunks)))
+  // histogram bin pool: sized before each K2 from the sample (run_end_of_sample); bin_hi starts at zero like the pool
+  if ((rc = r.d_bin_base.ensure(c, (size_t)c->n_local + 1)) || (rc = r.d_bin_block_sum.ensure(c, c->n_local / K1B_BLOCK + 1)) ||
+      (rc = r.d_bin_hi.ensure(c, c->n_local)))
     return rc;
+  CU_TRY(c, cudaMemsetAsync(r.d_bin_hi, 0, 4ull * c->n_local, c->stream));
+  CU_TRY(c, cudaMemsetAsync(r.d_bin_base, 0, 8ull * (c->n_local + 1), c->stream));
+  if (small_hist() && (rc = ensure_pool(c, 64, 64))) return rc;  // testing aid: a pool that overflows at once
+  c->pool_dirty = false;
   c->arena_dirty = true;
   // TMA descriptor: the arena as [rows][32] i32, box = one chunk (256 rows x 128 B), 128B swizzle
   PFN_encodeTiled encode = nullptr;
@@ -789,6 +802,12 @@ int cmb_begin_sample(cmb_ctx* c) {
       CU_TRY(c, cudaMemsetAsync(c->ref.d_span_bits, 0, c->arena_elems / BITMAP_ELEMS_PER_WORD * 4, c->stream));
     }
     CU_TRY(c, cudaMemsetAsync(c->ref.d_tail_sum, 0, 4ull * c->n_chunks, c->stream));
+    if (c->pool_dirty) {
+      if (c->ref.d_bins.cap) CU_TRY(c, cudaMemsetAsync(c->ref.d_bins, 0, 4 * c->ref.d_bins.cap, c->stream));
+      CU_TRY(c, cudaMemsetAsync(c->ref.d_bin_hi, 0, 4ull * c->n_local, c->stream));
+      c->pool_dirty = false;
+    }
+    if (c->gene_mode) CU_TRY(c, cudaMemsetAsync(c->ref.d_gene_bound, 0, 4ull * c->n_local, c->stream));
   }
   CU_TRY(c, cudaMemsetAsync(c->ref.d_rows, 0, sizeof(cmb_contig_stats) * (size_t)c->n_contigs, c->stream));
   CU_TRY(c, cudaMemsetAsync(c->d_counters, 0, 64, c->stream));
@@ -797,7 +816,7 @@ int cmb_begin_sample(cmb_ctx* c) {
   c->arena_dirty = true;  // until K2 has cleaned it
   if ((c->params.want & CMB_WANT_HIST_CSR) && c->n_local) {
     uint64_t want = std::max<uint64_t>(1u << 20, c->arena_elems / 16);
-    if (getenv("CMB_TEST_SMALL_HIST")) want = 64;  // testing aid: start with buffers that overflow at once (cmb_grow_buffers path)
+    if (small_hist()) want = 64;  // testing aid: start with a pair buffer that overflows at once (cmb_grow_buffers path)
     if (int rc = c->ref.d_pairs.ensure(c, want)) return rc;
   }
   c->in_sample = true;
@@ -876,6 +895,7 @@ int cmb_end_sample_device(cmb_ctx* c, const cmb_contig_stats** dev_stats) {
   if (c->n_acquired) return fail(c, CMB_E_ARG, "cmb_end_sample: an acquired batch was not submitted");
   CU_TRY(c, cudaSetDevice(c->device));
   c->in_sample = false;
+  c->pool_dirty = true;  // until the sample has ended without an error (K3 re-zeroed every bin K2 added)
   if (c->n_local) {
     int rc = run_end_of_sample(c);
     if (rc) return rc;
@@ -885,6 +905,7 @@ int cmb_end_sample_device(cmb_ctx* c, const cmb_contig_stats** dev_stats) {
   uint32_t counters[6];
   int rc = collect_errors_and_timing(c, counters);
   if (rc) return rc;
+  c->pool_dirty = false;
   c->ended = true;
   if (dev_stats) *dev_stats = c->ref.d_rows;
   return CMB_OK;
@@ -932,13 +953,12 @@ int cmb_grow_buffers(cmb_ctx* c) {
   CU_TRY(c, cudaSetDevice(c->device));
   CU_TRY(c, cudaStreamSynchronize(c->stream));
   auto& r = c->ref;  // the next sample rebuilds what these hold
+  // the bins the last sample needed: K1b's bin_base[n_local] (it stays in place until the next sample's K1b)
+  uint64_t need = 0;
+  CU_TRY(c, cudaMemcpyAsync(&need, r.d_bin_base + c->n_local, 8, cudaMemcpyDeviceToHost, c->stream));
+  CU_TRY(c, cudaStreamSynchronize(c->stream));
   int rc;
-  uint64_t rec_slack = 0;
-  if ((rc = k2_rec_slack(c, &rec_slack))) return rc;
-  if ((rc = r.d_rec.ensure(c, std::min<uint64_t>(0xfffffff0ull, (uint64_t)r.d_rec.cap * 4 + rec_slack))) ||
-      (rc = r.d_ovf.ensure(c, std::min<uint64_t>(1ull << 30, (uint64_t)r.d_ovf.cap * 4))) ||
-      (r.d_pairs && (rc = r.d_pairs.ensure(c, r.d_pairs.cap * 4))))
-    return rc;
+  if ((rc = ensure_pool(c, need, need)) || (r.d_pairs && (rc = r.d_pairs.ensure(c, r.d_pairs.cap * 4)))) return rc;
   c->arena_dirty = true;
   return CMB_OK;
 }

@@ -40,6 +40,7 @@ struct K1Args {
   const uint32_t* contig_len;   // [n_contigs]
   uint8_t* contig_seen;         // [n_contigs] a kept record mapped here (genes.rs:220-246)
   unsigned long long* kept_primary;  // primaries among the kept records (ReadsMapped.num_mapped_reads, genes.rs:249-252)
+  uint32_t* gene_bound;         // [n_genes] records that may add events to the gene: bounds its depth (K1b's bin pool layout)
   // pair path: partner of each record (cmb_pairs.cuh, records in file order) or NULL = the host layout (completed pairs
   // only, stored first mate at the even index, its partner right after)
   const int32_t* mate;
@@ -282,6 +283,7 @@ __global__ void __launch_bounds__(K1_THREADS, CMB_K1_MINBLOCKS) k1_filter_accumu
         for (uint32_t g = lo; g < g1; ++g) {
           const uint32_t gsx = a.gene_start[g], gex = a.gene_end[g];
           if ((uint64_t)gsx >= max(ref_end, (uint64_t)(uint32_t)pos + 1)) break;  // genes are sorted by start
+          atomicAdd(a.gene_bound + g, 1u);  // every gene the record may add events to: bounds the gene's depth
           if ((uint32_t)pos >= gsx && (uint32_t)pos < gex) {  // read_starts.partition_point range (genes.rs:518-523)
             cmb_contig_stats* row = a.rows + g;
             atomicAdd((unsigned long long*)&row->n_records, 1ull);

@@ -1,15 +1,32 @@
-// K1b: running depth at the first element of every chunk (carry_in), from the per-chunk tail sums K1 accumulated.
+// K1b: running depth at the first element of every chunk (carry_in), from the per-chunk tail sums K1 accumulated, and the
+// layout of the histogram bin pool (bin_base).
 //
 //   x_0 = 0;   x_{k+1} = mid_k ? ((same_k ? x_k : 0) + tail_sum[k]) : 0
 //   mid_k  = chunk k+1 starts in the middle of a contig,  same_k = that contig also owns the first span of chunk k.
 // A segmented scan over ~L/8192 elements, done in two tiny launches: k1b_local scans 1024-chunk blocks (thread = 4
 // consecutive chunks, warp shuffles, one shared-memory step) and leaves a "needs the block carry" flag in tail_sum;
 // k1b_apply folds in the block carries.  With the carries known up front K2 needs no inter-CTA look-back at all.
+//
+// The blocks after the chunk blocks (K1bBins) scan the segments instead: bin_base[c] = sum over c' < c of the bins of c',
+// (bound[c'] + 1) for a segment with an end-trimmed window (2E < L) and 0 otherwise, bin_base[n_seg] = the pool size.  bound
+// is the number of records that add an event to the segment (contig mode: rows[c].n_records; gene mode: gene_bound[c],
+// counted by K1).  A record's aligned blocks are disjoint, so it adds at most 1 to the depth at any position: every window
+// depth of c lies in [0, bound[c]] and K2 can add it straight into bin bin_base[c] + depth.
 #pragma once
 
 constexpr uint32_t K1B_THREADS = 256;
 constexpr uint32_t K1B_PER = 4;
-constexpr uint32_t K1B_BLOCK = K1B_THREADS * K1B_PER;  // chunks per block
+constexpr uint32_t K1B_BLOCK = K1B_THREADS * K1B_PER;  // chunks (or segments) per block
+
+struct K1bBins {
+  const uint32_t* len;            // [n_seg]
+  const cmb_contig_stats* rows;   // rows of the local segments (contig mode)
+  const uint32_t* gene_bound;     // [n_seg] gene mode, else NULL
+  uint32_t n_seg, excl;
+  uint64_t* bin_base;             // [n_seg + 1]
+  uint64_t* block_sum;            // [n_blocks]: bins of each block of K1B_BLOCK segments
+  uint32_t n_blocks;              // 0 = no histogram wanted
+};
 
 struct K1bElem {
   bool reset;
@@ -31,8 +48,66 @@ __device__ __forceinline__ K1bElem k1b_elem(uint32_t k, uint32_t n_chunks, const
   return e;
 }
 
+// Bin block `b` of k1b_local: local exclusive scan of the bins of its K1B_BLOCK segments (entry n_seg, with no bins, gets the
+// total) and the block's sum.
+__device__ __forceinline__ void k1b_bins_local(const K1bBins& g, uint32_t b) {
+  __shared__ unsigned long long s_w[K1B_THREADS / 32];
+  const uint32_t t = threadIdx.x, lane = t & 31, warp = t >> 5;
+  const uint32_t i0 = b * K1B_BLOCK + t * K1B_PER;
+  uint64_t nb[K1B_PER], sum = 0;
+#pragma unroll
+  for (uint32_t i = 0; i < K1B_PER; ++i) {
+    const uint32_t s = i0 + i;
+    nb[i] = 0;
+    if (s < g.n_seg && 2ull * g.excl < g.len[s]) nb[i] = (g.gene_bound ? (uint64_t)g.gene_bound[s] : (uint64_t)g.rows[s].n_records) + 1;
+    sum += nb[i];
+  }
+  uint64_t incl = sum;
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) {
+    const uint64_t o = __shfl_up_sync(FULL, incl, d);
+    if ((int)lane >= d) incl += o;
+  }
+  if (lane == 31) s_w[warp] = incl;
+  __syncthreads();
+  uint64_t x = incl - sum;
+  for (uint32_t w = 0; w < warp; ++w) x += s_w[w];
+  if (t == K1B_THREADS - 1) g.block_sum[b] = x + sum;
+#pragma unroll
+  for (uint32_t i = 0; i < K1B_PER; ++i) {
+    if (i0 + i <= g.n_seg) g.bin_base[i0 + i] = x;
+    x += nb[i];
+  }
+}
+
+// Bin block `b` of k1b_apply: adds the bins of the blocks before it.
+__device__ __forceinline__ void k1b_bins_apply(const K1bBins& g, uint32_t b) {
+  __shared__ unsigned long long s_w[K1B_THREADS / 32];
+  const uint32_t t = threadIdx.x;
+  uint64_t acc = 0;
+  for (uint32_t j = t; j < b; j += K1B_THREADS) acc += g.block_sum[j];
+  acc = warp_sum_u64(acc);
+  if ((t & 31) == 0) s_w[t >> 5] = acc;
+  __syncthreads();
+  uint64_t before = 0;
+#pragma unroll
+  for (uint32_t w = 0; w < K1B_THREADS / 32; ++w) before += s_w[w];
+  if (before == 0) return;
+#pragma unroll
+  for (uint32_t i = 0; i < K1B_PER; ++i) {
+    const uint32_t s = b * K1B_BLOCK + t * K1B_PER + i;
+    if (s <= g.n_seg) g.bin_base[s] += before;
+  }
+}
+
+// Blocks [0, ceil(n_chunks / K1B_BLOCK)) scan the chunks, the g.n_blocks after them the segments.
 __global__ void __launch_bounds__(K1B_THREADS) k1b_local(int32_t* tail_sum, const uint32_t* chunk_first, const uint32_t* off_span,
-                                                        uint32_t n_chunks, int32_t* carry_in, int2* block_agg) {
+                                                        uint32_t n_chunks, int32_t* carry_in, int2* block_agg, const K1bBins g) {
+  const uint32_t chunk_blocks = gridDim.x - g.n_blocks;
+  if (blockIdx.x >= chunk_blocks) {
+    k1b_bins_local(g, blockIdx.x - chunk_blocks);
+    return;
+  }
   __shared__ int2 s_w[K1B_THREADS / 32];
   const uint32_t t = threadIdx.x, lane = t & 31, warp = t >> 5;
   const uint32_t k0 = blockIdx.x * K1B_BLOCK + t * K1B_PER;
@@ -100,7 +175,13 @@ __global__ void __launch_bounds__(K1B_THREADS) k1b_local(int32_t* tail_sum, cons
   }
 }
 
-__global__ void __launch_bounds__(K1B_THREADS) k1b_apply(const int32_t* needs, const int2* block_agg, uint32_t n_chunks, int32_t* carry_in) {
+__global__ void __launch_bounds__(K1B_THREADS) k1b_apply(const int32_t* needs, const int2* block_agg, uint32_t n_chunks, int32_t* carry_in,
+                                                        const K1bBins g) {
+  const uint32_t chunk_blocks = gridDim.x - g.n_blocks;
+  if (blockIdx.x >= chunk_blocks) {
+    k1b_bins_apply(g, blockIdx.x - chunk_blocks);
+    return;
+  }
   __shared__ int s_carry;
   if (threadIdx.x == 0) {
     int acc = 0;

@@ -10,9 +10,11 @@
 // of the span totals.  Depth is piecewise constant and deltas are sparse (~1-2 % of positions), so a thread only keeps the
 // span total and a 32-bit mask of its non-zero positions; covered bases, sum of depth and the depth histogram of the
 // end-trimmed window are then accumulated per RUN in a short loop over the set bits (the deltas are re-read from the
-// shared-memory tile, which stays resident until the next iteration's barrier).  The histogram lives in shared memory
-// per (contig slot, depth % 128) with the high depth bits as a tag, and is flushed as (depth,count) records while the
-// next chunk is being scanned (double-buffered: one __syncthreads per chunk).
+// shared-memory tile, which stays resident until the next iteration's barrier).  The window depth histogram is a dense
+// array of u32 counts per contig in global memory, bins[bin_base[c] + depth] (K1b laid it out: every window depth of c is at
+// most its read count), so a run's count is one fire-and-forget RED; K3 reads the bins in depth order and re-zeroes them.
+// Depth 0 is not added: K3 derives its count from the window length and covered_window.  At config 2's coverage about half
+// of the runs are at depth 0, all of them on one address per contig.
 #pragma once
 
 struct K2Args {
@@ -25,14 +27,10 @@ struct K2Args {
   int32_t* arena;
   uint32_t* span_bits;   // [n_chunks * K2_WARPS] span occupancy bitmap (K1); word w of a chunk = the spans of its warp w
   uint32_t* load_stats;  // [0] += spans loaded, [1] += chunks loaded whole (CMB_PIPELINE_STATS)
-  uint2* rec;
-  uint32_t rec_capacity;
-  uint32_t* rec_count;
-  uint2* warp_table;  // [n_chunks * HIST_SLOTS] {offset, count}: records of contig slot w of the chunk
-  uint4* ovf;         // {contig_local, depth, count, next} — per-chunk linked lists
-  uint32_t* ovf_head; // [n_chunks] list heads (OVF_NIL = empty)
-  uint32_t ovf_capacity;
-  uint32_t* ovf_count;
+  const uint64_t* bin_base;  // [n_local + 1] first bin of each contig (K1b); bin_base[n_local] = bins needed
+  uint32_t* bins;            // the bin pool: pool_cap u32 counts, zero outside a sample
+  uint64_t pool_cap;
+  uint32_t* bin_hi;          // [n_local] highest depth added per contig (atomicMax)
   uint32_t* error_flags;
 };
 
@@ -45,25 +43,22 @@ struct K2Args {
 #endif
 constexpr uint32_t K2_DENSE_SPANS = CMB_K2_DENSE_SPANS;
 static_assert(K2_STAGES >= 2, "the refill of a stage is issued one iteration after it was read");
-// Histogram records a warp reserves in `rec` at a time, instead of one global atomic per (chunk, contig slot) on a counter
-// that every warp of the grid shares.  A run holds any slot (at most HIST_BINS records); a warp leaves at most one run
-// unused at the end and fewer than HIST_BINS records per refill.
-constexpr uint32_t K2_REC_RUN = 512;
-static_assert(K2_REC_RUN >= HIST_BINS, "a run must hold the records of one slot");
 
 constexpr uint32_t K2_SMEM_STAGE_BYTES = K2_STAGES * CHUNK_BYTES;
 constexpr uint32_t K2_SMEM_MISC = 64 /*barriers*/ + 2 * K2_WARPS * 8 /*warp aggregates, double-buffered*/;
-constexpr uint32_t K2_SMEM_BYTES_HIST = K2_SMEM_STAGE_BYTES + K2_SMEM_MISC + 2 * HIST_TOTAL * 4;
-constexpr uint32_t K2_SMEM_BYTES_NOHIST = K2_SMEM_STAGE_BYTES + K2_SMEM_MISC;
+constexpr uint32_t K2_SMEM_BYTES = K2_SMEM_STAGE_BYTES + K2_SMEM_MISC;
 
 template <bool HIST, bool CLEAN>
 __global__ void __launch_bounds__(K2_THREADS, CMB_K2_MINBLOCKS) k2_scan_reduce(const __grid_constant__ CUtensorMap tmap, const K2Args a) {
   extern __shared__ __align__(1024) uint8_t smem[];  // stage tiles need the 1024 B swizzle-atom alignment
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + K2_SMEM_STAGE_BYTES);
   int2* wagg2 = reinterpret_cast<int2*>(smem + K2_SMEM_STAGE_BYTES + 64);
-  uint32_t* hist2 = reinterpret_cast<uint32_t*>(wagg2 + 2 * K2_WARPS);
 
   const uint32_t t = threadIdx.x, lane = t & 31, warp = t >> 5;
+  // The pool is sized before the launch from a bound of bin_base[n_local]; when it is still too small (cmb_grow_buffers
+  // then grows it to exactly that) no bin is added and K3 reads none.
+  const bool hist = HIST && __ldg(a.bin_base + a.n_local) <= a.pool_cap;
+  if (HIST && !hist && blockIdx.x == 0 && t == 0) atomicOr(a.error_flags, ERR_CAPACITY);
 
   // Static schedule: iteration i of CTA b works on chunk b + i * gridDim.x.  Every thread knows its next chunk, so the chunk's
   // metadata (first / last contig, carry-in, bitmap words) is requested ahead and the dependent lookups (contig of the span,
@@ -124,59 +119,10 @@ __global__ void __launch_bounds__(K2_THREADS, CMB_K2_MINBLOCKS) k2_scan_reduce(c
     return have;
   };
 
-  // Each warp writes its records into a private run of `rec` (K2_REC_RUN records) that it reserves with one global atomic
-  // when the run cannot take a slot's records; K3 reads the records only through warp_table, so the unused ends of the runs
-  // are never read.  run_base = ~0u: a reservation did not fit (ERR_CAPACITY is set, the host grows `rec` and retries).
-  uint32_t run_base = 0, run_left = 0;  // warp-uniform
-  // flush one histogram buffer: a warp takes contig slots warp, warp + K2_WARPS, ... (128 bins, 4 per lane) -> (depth,count) records
-  auto flush_hist = [&](uint32_t* hist, uint32_t chunk, uint32_t n_slots) {
-    for (uint32_t sl = warp; sl < HIST_SLOTS && sl < n_slots; sl += K2_WARPS) {
-      uint32_t word[4], msk[4], total = 0;
-#pragma unroll
-      for (uint32_t k = 0; k < 4; ++k) {
-        word[k] = hist[sl * HIST_BINS + lane + 32 * k];
-        msk[k] = __ballot_sync(FULL, word[k] != 0);
-        total += __popc(msk[k]);
-      }
-      uint32_t base = 0;
-      if (total) {
-        if (total > run_left && run_base != ~0u) {  // the run cannot take this slot: reserve the next one
-          uint32_t b = 0;
-          if (lane == 0) b = atomicAdd(a.rec_count, K2_REC_RUN);
-          b = __shfl_sync(FULL, b, 0);
-          const bool ok = (uint64_t)b + K2_REC_RUN <= a.rec_capacity;
-          run_base = ok ? b : ~0u;
-          run_left = ok ? K2_REC_RUN : 0u;
-        }
-        const bool fits = total <= run_left;
-        base = run_base;
-        if (fits) {
-          run_base += total;
-          run_left -= total;
-        }
-        if (!fits && lane == 0) atomicOr(a.error_flags, ERR_CAPACITY);
-        uint32_t before = 0;
-#pragma unroll
-        for (uint32_t k = 0; k < 4; ++k) {
-          if (word[k]) {
-            const uint32_t depth = ((word[k] >> HIST_CNT_BITS) - 1) * HIST_BINS + lane + 32 * k;
-            if (fits) a.rec[base + before + __popc(msk[k] & ((1u << lane) - 1))] = make_uint2(depth, word[k] & ((1u << HIST_CNT_BITS) - 1));
-            hist[sl * HIST_BINS + lane + 32 * k] = 0;
-          }
-          before += __popc(msk[k]);
-        }
-        if (!fits) total = 0;
-      }
-      if (lane == 0) a.warp_table[(uint64_t)chunk * HIST_SLOTS + sl] = make_uint2(base, total);
-    }
-  };
-
   if (t == 0) {
     for (uint32_t s = 0; s < K2_STAGES; ++s) mbar_init(smem_u32(full + s), 1);
     fence_barrier_init();
   }
-  if (HIST)
-    for (uint32_t b = t; b < 2 * HIST_TOTAL; b += K2_THREADS) hist2[b] = 0;
   __syncthreads();
   // have[k] / own[k]: the spans of this warp that stage k holds / the bitmap word of this warp for the chunk in stage k
   uint32_t have[K2_STAGES], own[K2_STAGES];
@@ -194,7 +140,6 @@ __global__ void __launch_bounds__(K2_THREADS, CMB_K2_MINBLOCKS) k2_scan_reduce(c
   // byte offset inside a stage tile of element e of this thread's span
   auto elem_off = [&](uint32_t e) -> uint32_t { return row * 128 + (((e >> 2) ^ (row & 7)) << 4) + ((e & 3) << 2); };
   const uint32_t E = a.excl;
-  uint32_t prev_chunk = 0, prev_slots = 0;
   uint32_t n_cf = 0, n_cl = 0;  // metadata of the NEXT iteration's chunk, requested an iteration ahead
   int n_cin = 0;
   if (chunk_of(0) < a.n_chunks) {
@@ -232,6 +177,11 @@ __global__ void __launch_bounds__(K2_THREADS, CMB_K2_MINBLOCKS) k2_scan_reduce(c
     }
     const uint32_t cstart = __ldg(a.off_span + c);
     const uint32_t L = __ldg(a.len + c);
+    uint64_t bin0 = 0, bin1 = 0;  // this contig's bins
+    if (hist) {
+      bin0 = __ldg(a.bin_base + c);
+      bin1 = __ldg(a.bin_base + c + 1);
+    }
     uint32_t s_have = 0, s_own = 0;
 #pragma unroll
     for (uint32_t k = 0; k < K2_STAGES; ++k)
@@ -244,7 +194,6 @@ __global__ void __launch_bounds__(K2_THREADS, CMB_K2_MINBLOCKS) k2_scan_reduce(c
     __syncwarp();                    // ... and those of the other lanes of its warp
     if (CLEAN && lane == 0 && s_own) a.span_bits[chunk * K2_WARPS + warp] = 0;
     int2* wagg = wagg2 + (it & 1) * K2_WARPS;
-    uint32_t* hist = hist2 + (it & 1) * HIST_TOTAL;
 
     // ---- SPAN consecutive deltas per thread: LDS.128s through the 128B swizzle (conflict-free).
     //      Only their sum and the mask of non-zero positions stay in registers.  A span the stage does not hold is all zero.
@@ -292,7 +241,7 @@ __global__ void __launch_bounds__(K2_THREADS, CMB_K2_MINBLOCKS) k2_scan_reduce(c
       pflg = 0;
     }
     if (lane == 31) wagg[warp] = make_int2(val, flg);
-    __syncthreads();  // warp aggregates visible; the previous iteration's tile and histogram adds are complete
+    __syncthreads();  // warp aggregates visible; the previous iteration's tile reads are complete
     if (it > 0) {
       // refill the stage of the previous iteration (read until this barrier)
       const uint32_t rs = (it - 1) % K2_STAGES, rk = chunk_of(it - 1 + K2_STAGES);
@@ -305,7 +254,6 @@ __global__ void __launch_bounds__(K2_THREADS, CMB_K2_MINBLOCKS) k2_scan_reduce(c
           own[k] = r_own;
         }
       n_bits = load_bits(chunk_of(it + K2_STAGES));
-      if (HIST) flush_hist(hist2 + ((it & 1) ^ 1) * HIST_TOTAL, prev_chunk, prev_slots);
     }
 
     int wv, wf;
@@ -339,35 +287,16 @@ __global__ void __launch_bounds__(K2_THREADS, CMB_K2_MINBLOCKS) k2_scan_reduce(c
     // ---- reductions over this span (EST:393-404, 447-465, 494-501), run by run
     uint32_t cov_full = 0, cov_win = 0;
     uint64_t sum_win = 0;
-    const uint32_t slot = c - cf;
+    uint32_t bin_top = 0;  // highest depth this thread added to contig c's bins
     auto hist_add = [&](int depth, uint32_t cnt) {
-      // direct-mapped bin (depth % 128) holding (depth / 128 + 1) << 14 | count: conflict-free while the depths of one
-      // contig inside one chunk span < 128 values, wherever that range sits
-      if (depth < 0) {  // impossible for a consistent arena (every -1 follows its +1 within the contig)
+      // 0 <= depth <= bound = bin1 - bin0 - 1 for a consistent arena (every -1 follows its +1 within the contig, and a
+      // record adds at most 1 at any position)
+      if (depth < 0 || (uint64_t)depth >= bin1 - bin0) {
         atomicOr(a.error_flags, ERR_INTERNAL);
         return;
       }
-      bool done = false;
-      if (slot < HIST_SLOTS && (uint32_t)depth < HIST_MAX_DEPTH) {
-        uint32_t* w = hist + slot * HIST_BINS + ((uint32_t)depth & (HIST_BINS - 1));
-        const uint32_t tag = ((uint32_t)depth / HIST_BINS) + 1;
-        uint32_t cur = *(volatile uint32_t*)w;
-        if (cur == 0) cur = atomicCAS(w, 0u, (tag << HIST_CNT_BITS) | cnt);
-        if (cur == 0) done = true;  // we installed tag and count
-        else if ((cur >> HIST_CNT_BITS) == tag) {
-          atomicAdd(w, cnt);
-          done = true;
-        }
-      }
-      if (!done) {  // > 16 contigs in the chunk, or two depths 128 apart in one chunk: per-chunk overflow list
-        const uint32_t o = atomicAdd(a.ovf_count, 1u);
-        if (o < a.ovf_capacity) {
-          const uint32_t next = atomicExch(a.ovf_head + chunk, o);
-          a.ovf[o] = make_uint4(c, (uint32_t)depth, cnt, next);
-        } else {
-          atomicOr(a.error_flags, ERR_CAPACITY);
-        }
-      }
+      atomicAdd(a.bins + bin0 + (uint32_t)depth, cnt);
+      bin_top = max(bin_top, (uint32_t)depth);
     };
     // a run [from, to) of the span at one depth, clipped to the contig and to its end-trimmed window
     auto close_run = [&](int depth, uint32_t from, uint32_t to) {
@@ -379,7 +308,7 @@ __global__ void __launch_bounds__(K2_THREADS, CMB_K2_MINBLOCKS) k2_scan_reduce(c
       }
       if (nw) {
         sum_win += (uint64_t)(int64_t)depth * nw;
-        if (HIST) hist_add(depth, nw);
+        if (hist && depth != 0) hist_add(depth, nw);
       }
     };
     if (ev) {
@@ -402,51 +331,46 @@ __global__ void __launch_bounds__(K2_THREADS, CMB_K2_MINBLOCKS) k2_scan_reduce(c
       }
       sum_win += (uint64_t)(int64_t)carry * nw;
     }
-    if (HIST) {
-      // event-free spans: aggregate the lanes that agree with the first such lane into one shared-memory atomic
+    if (hist) {
+      // event-free spans: one RED per distinct (contig, depth) of the warp, added by the group's first lane (usually 1-3 groups)
       const uint32_t nw = w1 - w0;
-      const bool cand = ev == 0 && nw > 0;
-      const uint32_t cm = __ballot_sync(FULL, cand);
-      if (cm) {
+      uint32_t cm = __ballot_sync(FULL, ev == 0 && nw > 0 && carry != 0);
+      while (cm) {
         const int leader = __ffs(cm) - 1;
         const int d0 = __shfl_sync(FULL, carry, leader);
         const uint32_t c0 = __shfl_sync(FULL, c, leader);
-        const bool same = cand && carry == d0 && c == c0;
+        const bool same = ((cm >> lane) & 1u) && carry == d0 && c == c0;
         const uint32_t m = __ballot_sync(FULL, same);
         if (same) {
           const uint32_t tot = __reduce_add_sync(m, nw);
           if ((int)lane == leader) hist_add(carry, tot);
-        } else if (cand) {
-          hist_add(carry, nw);
         }
+        cm &= ~m;
       }
     }
 
-    // ---- per-contig accumulation: one RED triple per (warp, contig)
+    // ---- per-contig accumulation: one RED triple (and the bin_hi max) per (warp, contig)
     {
       const uint32_t c0 = __shfl_sync(FULL, c, 0);
       if (__all_sync(FULL, c == c0)) {
         const uint32_t sf = __reduce_add_sync(FULL, cov_full), sw = __reduce_add_sync(FULL, cov_win);
         const uint64_t sd = warp_sum_u64(sum_win);
+        const uint32_t top = hist ? __reduce_max_sync(FULL, bin_top) : 0u;
         if (lane == 0) {
           cmb_contig_stats* rowp2 = a.rows + a.tid_begin + c0;
           if (sf) atomicAdd((unsigned long long*)&rowp2->covered_full, (unsigned long long)sf);
           if (sw) atomicAdd((unsigned long long*)&rowp2->covered_window, (unsigned long long)sw);
           if (sd) atomicAdd((unsigned long long*)&rowp2->sum_depth_window, (unsigned long long)sd);
+          if (top) atomicMax(a.bin_hi + c0, top);
         }
       } else {
         cmb_contig_stats* rowp2 = a.rows + a.tid_begin + c;
         if (cov_full) atomicAdd((unsigned long long*)&rowp2->covered_full, (unsigned long long)cov_full);
         if (cov_win) atomicAdd((unsigned long long*)&rowp2->covered_window, (unsigned long long)cov_win);
         if (sum_win) atomicAdd((unsigned long long*)&rowp2->sum_depth_window, (unsigned long long)sum_win);
+        if (bin_top) atomicMax(a.bin_hi + c, bin_top);
       }
     }
-    prev_chunk = chunk;
-    prev_slots = cl - cf + 1;
-  }
-  if (HIST && it > 0) {
-    __syncthreads();  // the last chunk's histogram adds
-    flush_hist(hist2 + ((it & 1) ^ 1) * HIST_TOTAL, prev_chunk, prev_slots);
   }
   if (t == 0 && n_loaded) {
     atomicAdd(a.load_stats + 0, n_loaded);

@@ -1,29 +1,26 @@
 // K3: per-contig histogram finalisation, one WARP per contig.
 //
-// K2 left, per (chunk, contig slot), a short list of (depth,count) records (plus, rarely, records on the chunk's
-// overflow list).  A contig gathers the lists of the chunks it overlaps into a per-warp shared-memory window of depth
-// bins [dmin, dmin+512) (repeated for deeper windows if ever needed), then walks the bins in order with warp scans:
+// K2 left the window depth histogram of contig c in bins[bin_base[c] .. bin_base[c] + bin_hi[c]] (one u32 count per depth),
+// except depth 0, which it never adds: that count is the window length minus covered_window (the window positions of depth
+// > 0, which K2 counts anyway).  The warp walks the bins in depth order, 32 per step, with warp scans:
 //   * trimmed-mean `total` exactly as the reference's ascending walk (EST:598-642),
 //   * S0 = sum n, S1 = sum x n, S2 = sum x^2 n (wrapping u64) and k = lowest depth -> variance sums (EST:790-805),
-//   * optionally the merged (depth,count) pairs (CSR) for the host-side per-genome merge / coverage_histogram.
+//   * optionally the (depth,count) pairs (CSR) for the host-side per-genome merge / coverage_histogram,
+// and re-zeroes every bin it read and bin_hi[c], so that the pool is zero again for the next sample.
 #pragma once
 
 constexpr uint32_t K3_WARPS = 8;
 constexpr uint32_t K3_THREADS = K3_WARPS * 32;
-constexpr uint32_t K3_WINDOW = 512;  // depth bins per warp window
 
 struct K3Args {
-  const uint32_t* off_span;
   const uint32_t* len;
-  const uint32_t* chunk_first;
   cmb_contig_stats* rows;
   uint32_t tid_begin, n_local, excl;
   float trim_min, trim_max;
-  const uint2* rec;
-  const uint2* warp_table;
-  const uint4* ovf;
-  const uint32_t* ovf_head;
-  uint32_t ovf_capacity;
+  const uint64_t* bin_base;
+  uint32_t* bins;
+  uint64_t pool_cap;
+  uint32_t* bin_hi;
   cmb_hist_pair* pairs;
   unsigned long long* pair_count;
   uint64_t pair_capacity;
@@ -33,120 +30,84 @@ struct K3Args {
 };
 
 __global__ void __launch_bounds__(K3_THREADS) k3_finalize(const K3Args a) {
-  __shared__ uint32_t whist_all[K3_WARPS][K3_WINDOW];
   const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  uint32_t* whist = whist_all[warp];
   const uint32_t lc = blockIdx.x * K3_WARPS + warp;
   if (lc >= a.n_local) return;
+  // K3 is latency-bound (a warp per contig, little work each): every per-contig value is requested at once, before any branch
   cmb_contig_stats* row = a.rows + a.tid_begin + lc;
-  if (row->n_records == 0 && !a.all_rows) return;  // unseen contig: the host never consults its histogram
-  const uint32_t L = a.len[lc];
-  const uint64_t E = a.excl;
-  if (!(2 * E < L)) return;  // no window (EST:436-445)
-  const uint64_t T = (uint64_t)L - 2 * E;
+  const uint64_t pool_need = __ldg(a.bin_base + a.n_local), b_first = __ldg(a.bin_base + lc), b_end = __ldg(a.bin_base + lc + 1);
+  const uint32_t hi = a.bin_hi[lc];  // K3 re-zeroes it below: not a read-only load
+  const uint32_t L = __ldg(a.len + lc);
+  const uint64_t n_records = row->n_records, covered_window = row->covered_window;
+  if (pool_need > a.pool_cap) return;  // K2 added no bin (ERR_CAPACITY)
+  if (b_end == b_first) return;        // no window (EST:436-445), no bins
+  // unseen contig: the host never consults its histogram, and with no read every depth is 0, so K2 added no bin
+  if (n_records == 0 && !a.all_rows) return;
+  uint32_t* bins = a.bins + b_first;
+  const uint64_t T = (uint64_t)L - 2ull * a.excl;
+  const uint32_t n_zero = (uint32_t)(T - covered_window);  // window positions at depth 0
   const float Tf = __ull2float_rn(T);  // EST:591-592: f32 products, `as usize` saturating casts
   const uint64_t min_index = (uint64_t)floorf(__fmul_rn(a.trim_min, Tf));
   const uint64_t max_index = (uint64_t)ceilf(__fmul_rn(a.trim_max, Tf));
-  const uint32_t k0 = a.off_span[lc] / CHUNK_SPANS, k1 = (a.off_span[lc + 1] - 1) / CHUNK_SPANS;
-  const uint32_t n_chunk = k1 - k0 + 1;
-
-  // Visits every record of this contig: the (chunk, slot) lists one after the other with the records lane-parallel,
-  // then the chunks' overflow lists (one lane per chunk).
-  auto for_each_record = [&](auto&& fn) {
-    for (uint32_t i = 0; i < n_chunk; ++i) {
-      const uint32_t k = k0 + i;
-      const uint32_t slot = lc - a.chunk_first[k];
-      if (slot >= HIST_SLOTS) continue;
-      const uint2 ent = a.warp_table[(uint64_t)k * HIST_SLOTS + slot];
-      for (uint32_t r = lane; r < ent.y; r += 32) {
-        const uint2 rc = a.rec[ent.x + r];
-        fn(rc.x, rc.y);
-      }
-    }
-    for (uint32_t i = lane; i < n_chunk; i += 32) {
-      for (uint32_t o = a.ovf_head[k0 + i]; o != OVF_NIL && o < a.ovf_capacity;) {
-        const uint4 rc = a.ovf[o];
-        if (rc.x == lc) fn(rc.y, rc.z);
-        o = rc.w;
-      }
-    }
-  };
-
-  // ---- depth range of this contig's records
-  uint32_t dmin = 0xffffffffu, dmax = 0;
-  for_each_record([&](uint32_t depth, uint32_t) {
-    dmin = min(dmin, depth);
-    dmax = max(dmax, depth);
-  });
-  dmin = __reduce_min_sync(FULL, dmin);
-  dmax = __reduce_max_sync(FULL, dmax);
-  if (dmin > dmax) return;  // no records (cannot happen for a contig with a window)
 
   unsigned long long ltot = 0, l0 = 0, l1 = 0, l2 = 0;  // per-lane partial sums
-  uint32_t n_pairs = 0;
+  uint32_t n_pairs = 0, k = 0xffffffffu;                // k: lowest depth with a non-zero count
   unsigned long long pair_base = 0;
   const int n_rounds = a.want_csr ? 2 : 1;  // round 0: statistics (+ count the pairs); round 1: write the pairs
   for (int round = 0; round < n_rounds; ++round) {
-    unsigned long long cum = 0;  // counts below the current window
+    const bool last = round == n_rounds - 1;
+    unsigned long long cum = 0;  // counts below the current step
     uint32_t written = 0;
-    for (uint32_t wbase = dmin;; wbase += K3_WINDOW) {
-      const uint32_t nb = min(K3_WINDOW, dmax - wbase + 1);
-      for (uint32_t b = lane; b < nb; b += 32) whist[b] = 0;
-      __syncwarp();
-      for_each_record([&](uint32_t depth, uint32_t cnt) {
-        const uint32_t b = depth - wbase;
-        if (depth >= wbase && b < nb) atomicAdd(&whist[b], cnt);
-      });
-      __syncwarp();
-      for (uint32_t b0 = 0; b0 < nb; b0 += 32) {
-        const uint32_t b = b0 + lane;
-        const uint32_t n = b < nb ? whist[b] : 0u;
-        uint32_t incl = n;  // inclusive scan of the 32 bins (a contig holds < 2^31 bases: fits u32)
+    for (uint32_t b0 = 0; b0 <= hi; b0 += 32) {
+      const uint32_t b = b0 + lane;
+      const uint32_t got = b <= hi ? bins[b] : 0u;
+      if (last && got) bins[b] = 0;
+      const uint32_t n = b == 0 ? n_zero : got;
+      uint32_t incl = n;  // inclusive scan of the 32 bins (a contig holds < 2^31 bases: fits u32)
 #pragma unroll
-        for (int d = 1; d < 32; d <<= 1) {
-          const uint32_t o = __shfl_up_sync(FULL, incl, d);
-          if ((int)lane >= d) incl += o;
-        }
-        const uint32_t nzmask = __ballot_sync(FULL, n != 0);
-        if (round == 0) {
-          if (n) {
-            const unsigned long long depth = (unsigned long long)wbase + b;
-            const unsigned long long cprev = cum + (incl - n), ccur = cum + incl;
-            unsigned long long w;
-            if (ccur < min_index) w = 0;
-            else if (cprev < min_index) w = ccur > max_index ? max_index - min_index + 1 : ccur - min_index + 1;
-            else w = cprev > max_index ? 0 : (ccur > max_index ? max_index - cprev + 1 : (unsigned long long)n);
-            ltot += w * depth;
-            l0 += n;
-            l1 += depth * n;
-            l2 += depth * depth * n;
-          }
-          n_pairs += __popc(nzmask);
-        } else if (n) {
-          const unsigned long long idx = pair_base + written + __popc(nzmask & ((1u << lane) - 1));
-          if (idx < a.pair_capacity) {
-            cmb_hist_pair pr;
-            pr.depth = wbase + b;
-            pr.count = n;
-            a.pairs[idx] = pr;
-          }
-        }
-        written += __popc(nzmask);
-        cum += __shfl_sync(FULL, incl, 31);
+      for (int d = 1; d < 32; d <<= 1) {
+        const uint32_t o = __shfl_up_sync(FULL, incl, d);
+        if ((int)lane >= d) incl += o;
       }
-      if (dmax - wbase < K3_WINDOW) break;
-      __syncwarp();
+      const uint32_t nzmask = __ballot_sync(FULL, n != 0);
+      if (round == 0) {
+        if (nzmask && k == 0xffffffffu) k = b0 + __ffs(nzmask) - 1;
+        if (n) {
+          const unsigned long long depth = b;
+          const unsigned long long cprev = cum + (incl - n), ccur = cum + incl;
+          unsigned long long w;
+          if (ccur < min_index) w = 0;
+          else if (cprev < min_index) w = ccur > max_index ? max_index - min_index + 1 : ccur - min_index + 1;
+          else w = cprev > max_index ? 0 : (ccur > max_index ? max_index - cprev + 1 : (unsigned long long)n);
+          ltot += w * depth;
+          l0 += n;
+          l1 += depth * n;
+          l2 += depth * depth * n;
+        }
+        n_pairs += __popc(nzmask);
+      } else if (n) {
+        const unsigned long long idx = pair_base + written + __popc(nzmask & ((1u << lane) - 1));
+        if (idx < a.pair_capacity) {
+          cmb_hist_pair pr;
+          pr.depth = b;
+          pr.count = n;
+          a.pairs[idx] = pr;
+        }
+      }
+      written += __popc(nzmask);
+      cum += __shfl_sync(FULL, incl, 31);
     }
     if (round == 0) {
+      if (k == 0xffffffffu) break;  // no count at all (cannot happen for a contig with a window)
       const unsigned long long total = warp_sum_u64(ltot), S0 = warp_sum_u64(l0), S1 = warp_sum_u64(l1), S2 = warp_sum_u64(l2);
       if (lane == 0) {
-        const unsigned long long k = dmin;  // lowest depth with a non-zero count
+        const unsigned long long kk = k;
         row->trimmed_total = total;
         row->trim_min_index = min_index;
         row->trim_max_index = max_index;
-        row->var_k = k;
-        row->var_ex = S1 - k * S0;                    // sum (x-k) n    (mod 2^64, as the reference's usize)
-        row->var_ex2 = S2 - 2 * k * S1 + k * k * S0;  // sum (x-k)^2 n
+        row->var_k = kk;
+        row->var_ex = S1 - kk * S0;                     // sum (x-k) n    (mod 2^64, as the reference's usize)
+        row->var_ex2 = S2 - 2 * kk * S1 + kk * kk * S0;  // sum (x-k)^2 n
         row->hist_count = n_pairs;
         if (a.want_csr) {
           pair_base = atomicAdd(a.pair_count, (unsigned long long)n_pairs);
@@ -157,4 +118,5 @@ __global__ void __launch_bounds__(K3_THREADS) k3_finalize(const K3Args a) {
       pair_base = __shfl_sync(FULL, pair_base, 0);
     }
   }
+  if (lane == 0) a.bin_hi[lc] = 0;
 }

@@ -50,7 +50,7 @@ extern "C" {
 #define CMB_E_UNSORTED (-4)  /* records not sorted by reference   (contig.rs:129-132 panic) */
 #define CMB_E_NM (-5)        /* NM aux missing / wrong type where the reference calls nm()  (lib.rs:138-158 panic) */
 #define CMB_E_BOUNDS (-6)    /* an aligned block starts at/after the contig end (contig.rs:178 index panic) */
-#define CMB_E_CAPACITY (-7)  /* a device-side buffer (histogram records) overflowed         */
+#define CMB_E_CAPACITY (-7)  /* a device-side buffer (histogram bin pool or pairs) overflowed */
 #define CMB_E_DECLINED (-8)  /* cmb_submit_bgzf: the device decoder cannot vouch for this stream; nothing was
                                 accumulated -- decode on the host instead                    */
 
@@ -284,9 +284,11 @@ int cmb_filter_fetch(cmb_ctx* ctx, uint8_t* records, uint64_t n_bytes);
  * Lets a caller re-run the filter/scan/reduce kernels over an already decoded sample (device-only timing, parameter sweeps). */
 int cmb_last_bgzf_batch(cmb_ctx* ctx, cmb_read_batch* dev_batch, uint32_t* n_records, uint32_t* n_intervals);
 
-/* After cmb_end_sample* failed with CMB_E_CAPACITY (a device-side histogram buffer overflowed: very deep coverage over many
- * small contigs): enlarges those buffers (x4).  A caller whose tuples are still in device memory (cmb_last_bgzf_batch) can then
- * run the sample again -- cmb_begin_sample, cmb_submit_device_batch, cmb_end_sample. */
+/* After cmb_end_sample* failed with CMB_E_CAPACITY (a device-side histogram buffer overflowed): grows the histogram bin pool to
+ * exactly the size the failed sample needed (one bin per window depth up to each contig's read count; the library sizes it
+ * before every sample, so this takes a caller that bypassed that sizing) and the CSR pair buffer x4.  A caller whose tuples
+ * are still in device memory (cmb_last_bgzf_batch) can then run the sample again -- cmb_begin_sample,
+ * cmb_submit_device_batch, cmb_end_sample. */
 int cmb_grow_buffers(cmb_ctx* ctx);
 
 /* Page-locked host memory for result buffers (cmb_end_sample copies straight into it at PCIe speed).  Plain malloc
