@@ -6,6 +6,9 @@
 // (contig.rs:124,166-168; filter.rs:251-277) and the NM aux lookup (lib.rs:138-158).  Written from the SAM/BAM
 // specification (SAMv1 §4.1 BGZF, §4.2 BAM, §1.4 SAM); BGZF blocks are inflated with zlib on a thread pool
 // (the reference's set_threads, bam_generator.rs:125-129) and tuples are extracted in parallel.
+//
+// Every BAM-format rule of the host lives here, once: opening an input (SAM converted to BAM), the BGZF block index,
+// the header, the record decoder, the walk of an in-memory record stream and the host's mate matching.
 #pragma once
 #include <fcntl.h>
 #include <sys/mman.h>
@@ -15,9 +18,11 @@
 
 #include "fast_inflate.hpp"
 
+#include <climits>
 #include <cstring>
 #include <map>
 #include <memory>
+#include <optional>
 #include <stdexcept>
 #include <string>
 #include <unordered_map>
@@ -91,6 +96,17 @@ struct Tuple {
   uint32_t n_iv;
 };
 
+inline uint32_t rd_u32(const uint8_t* p) {
+  uint32_t v;
+  memcpy(&v, p, 4);
+  return v;
+}
+inline uint16_t rd_u16(const uint8_t* p) {
+  uint16_t v;
+  memcpy(&v, p, 2);
+  return v;
+}
+
 class ByteSource {  // whole input mapped (file) or borrowed (memory)
  public:
   explicit ByteSource(const InputSpec& in) {
@@ -127,118 +143,286 @@ class ByteSource {  // whole input mapped (file) or borrowed (memory)
   bool mapped_ = false;
 };
 
-// Streams the uncompressed bytes of a BGZF (or plain gzip, or uncompressed) file in windows.
+// Converts SAM text to BAM record bytes so that one decoder serves both (htslib reads SAM through the same
+// bam::Reader; tests/data/mapq_test.sam).  Integer aux tags get htslib's smallest-fitting type.
+class SamToBam {
+ public:
+  static bool looks_like_sam(const uint8_t* p, size_t n) { return n == 0 || p[0] == '@' || (n > 4 && memcmp(p, "BAM\1", 4) != 0); }
+  static void convert(const uint8_t* p, size_t n, Header& header, std::vector<uint8_t>& out) {
+    std::unordered_map<std::string, int32_t> name_to_tid;
+    size_t o = 0;
+    auto next_line = [&](std::string& line) {
+      if (o >= n) return false;
+      size_t e = o;
+      while (e < n && p[e] != '\n') ++e;
+      line.assign((const char*)p + o, e - o);
+      o = e < n ? e + 1 : e;
+      if (!line.empty() && line.back() == '\r') line.pop_back();
+      return true;
+    };
+    auto split = [](const std::string& s) {
+      std::vector<std::string> v;
+      size_t a = 0;
+      for (;;) {
+        size_t b = s.find('\t', a);
+        if (b == std::string::npos) { v.push_back(s.substr(a)); break; }
+        v.push_back(s.substr(a, b - a));
+        a = b + 1;
+      }
+      return v;
+    };
+    out.assign({'B', 'A', 'M', 1});
+    std::string line;
+    std::vector<uint8_t> body;
+    auto put32 = [](std::vector<uint8_t>& v, uint32_t x) { for (int k = 0; k < 4; ++k) v.push_back((x >> (8 * k)) & 0xff); };
+    auto put16 = [](std::vector<uint8_t>& v, uint32_t x) { v.push_back(x & 0xff); v.push_back((x >> 8) & 0xff); };
+    bool header_done = false;
+    std::vector<uint8_t> recs;
+    while (next_line(line)) {
+      if (line.empty()) continue;
+      if (line[0] == '@' && !header_done) {
+        if (line.compare(0, 3, "@SQ") == 0) {
+          std::string sn;
+          uint64_t ln = 0;
+          for (auto& f : split(line)) {
+            if (f.compare(0, 3, "SN:") == 0) sn = f.substr(3);
+            if (f.compare(0, 3, "LN:") == 0) ln = strtoull(f.c_str() + 3, nullptr, 10);
+          }
+          name_to_tid[sn] = (int32_t)header.names.size();
+          header.names.push_back(sn);
+          header.lens.push_back(ln);
+        }
+        continue;
+      }
+      header_done = true;
+      auto f = split(line);
+      if (f.size() < 11) throw Panic("Error reading BAM record: malformed SAM line");
+      auto tid_of = [&](const std::string& s) -> int32_t {
+        if (s == "*") return -1;
+        auto it = name_to_tid.find(s);
+        if (it == name_to_tid.end()) throw Panic("Error reading BAM record: unknown reference " + s);
+        return it->second;
+      };
+      const int32_t tid = tid_of(f[2]);
+      std::vector<uint32_t> cigar;
+      if (f[5] != "*") {
+        const char* c = f[5].c_str();
+        while (*c) {
+          char* e;
+          const uint32_t len = (uint32_t)strtoul(c, &e, 10);
+          static const char* ops = "MIDNSHP=X";
+          const char* w = *e ? strchr(ops, *e) : nullptr;
+          if (!w) throw Panic("Error reading BAM record: bad CIGAR");
+          cigar.push_back((len << 4) | (uint32_t)(w - ops));
+          c = e + 1;
+        }
+      }
+      const uint32_t l_seq = f[9] == "*" ? 0 : (uint32_t)f[9].size();
+      body.clear();
+      put32(body, (uint32_t)tid);
+      put32(body, (uint32_t)((int32_t)strtol(f[3].c_str(), nullptr, 10) - 1));
+      body.push_back((uint8_t)std::min<size_t>(255, f[0].size() + 1));
+      body.push_back((uint8_t)strtoul(f[4].c_str(), nullptr, 10));
+      put16(body, 0);
+      put16(body, (uint32_t)cigar.size());
+      put16(body, (uint32_t)strtoul(f[1].c_str(), nullptr, 10));
+      put32(body, l_seq);
+      put32(body, (uint32_t)(f[6] == "=" ? tid : tid_of(f[6])));
+      put32(body, (uint32_t)((int32_t)strtol(f[7].c_str(), nullptr, 10) - 1));
+      put32(body, (uint32_t)strtol(f[8].c_str(), nullptr, 10));
+      body.insert(body.end(), f[0].begin(), f[0].begin() + std::min<size_t>(254, f[0].size()));
+      body.push_back(0);
+      for (uint32_t cg : cigar) put32(body, cg);
+      body.insert(body.end(), (l_seq + 1) / 2 + l_seq, 0);
+      for (size_t i = 11; i < f.size(); ++i) {
+        if (f[i].size() < 5 || f[i][2] != ':' || f[i][4] != ':') continue;
+        if (f[i][0] != 'N' || f[i][1] != 'M') continue;  // only NM matters on this path
+        body.push_back('N');
+        body.push_back('M');
+        if (f[i][3] == 'i') {
+          const long long v = strtoll(f[i].c_str() + 5, nullptr, 10);
+          if (v < 0) { body.push_back('i'); put32(body, (uint32_t)(int32_t)v); }
+          else if (v <= 0xff) { body.push_back('C'); body.push_back((uint8_t)v); }
+          else if (v <= 0xffff) { body.push_back('S'); put16(body, (uint32_t)v); }
+          else { body.push_back('I'); put32(body, (uint32_t)v); }
+        } else {
+          body.push_back('A');
+          body.push_back('?');
+        }
+      }
+      put32(recs, (uint32_t)body.size());
+      recs.insert(recs.end(), body.begin(), body.end());
+    }
+    put32(out, 0);  // l_text
+    put32(out, (uint32_t)header.names.size());
+    for (size_t i = 0; i < header.names.size(); ++i) {
+      put32(out, (uint32_t)header.names[i].size() + 1);
+      out.insert(out.end(), header.names[i].begin(), header.names[i].end());
+      out.push_back(0);
+      put32(out, (uint32_t)header.lens[i]);
+    }
+    out.insert(out.end(), recs.begin(), recs.end());
+    header = Header{};  // re-parsed from the BAM bytes by the caller
+  }
+};
+
+// The BAM bytes of an input: the file mapped (or the caller's buffer), or its SAM text converted to BAM.
+class BamInput {
+ public:
+  explicit BamInput(const InputSpec& in) : src_(in), p_(src_.data()), n_(src_.size()) {
+    if (!(n_ >= 2 && p_[0] == 0x1f && p_[1] == 0x8b) && SamToBam::looks_like_sam(p_, n_)) {
+      Header sam_header;
+      SamToBam::convert(p_, n_, sam_header, sam_as_bam_);
+      p_ = sam_as_bam_.data();
+      n_ = sam_as_bam_.size();
+    }
+  }
+  const uint8_t* data() const { return p_; }
+  size_t size() const { return n_; }
+
+ private:
+  ByteSource src_;
+  const uint8_t* p_;
+  size_t n_;
+  std::vector<uint8_t> sam_as_bam_;
+};
+
+struct BlockRef {
+  size_t cdata, clen;  // compressed payload (BGZF) or raw slice [cdata, cdata+clen)
+  uint32_t isize;      // uncompressed size
+};
+
+// The blocks of an input with their uncompressed offsets: its BGZF blocks (SAMv1 §4.1) when it starts with one, otherwise
+// 64 KB slices of the bytes as they are.  The only BGZF block-header parser of the host: InflateStream grows the table
+// block by block as it reads, the decoders take it whole (finish()).
+class BlockIndex {
+ public:
+  std::vector<BlockRef> blocks;
+  std::vector<uint64_t> ustart{0};  // blocks.size()+1 cumulative uncompressed offsets
+  bool bgzf = false;
+  const uint8_t* p = nullptr;
+  size_t n = 0;
+
+  void build(const uint8_t* data, size_t size) {
+    start(data, size);
+    finish();
+  }
+  // An empty table over a BGZF input, or every slice of any other (or of one that must not be taken for BGZF).
+  void start(const uint8_t* data, size_t size, bool may_be_bgzf = true) {
+    p = data;
+    n = size;
+    next_header_ = 0;
+    blocks.clear();
+    ustart.assign(1, 0);
+    BlockRef b;
+    size_t end;
+    bgzf = may_be_bgzf && !parse(0, b, end);
+    if (!bgzf)
+      for (size_t o = 0; o < size; o += 65536) add({o, std::min<size_t>(65536, size - o), (uint32_t)std::min<size_t>(65536, size - o)});
+  }
+  // BGZF: appends the block whose header comes next.  false at the end of the input.
+  bool next() {
+    if (!bgzf || next_header_ >= n) return false;
+    BlockRef b;
+    if (const char* bad = parse(next_header_, b, next_header_)) throw Panic(std::string("Error reading BAM record: ") + bad);
+    add(b);
+    return true;
+  }
+  const BlockIndex& finish() {
+    while (next()) {
+    }
+    return *this;
+  }
+
+  // Inflate blocks [b0, b1) into dst (which has room for ustart[b1]-ustart[b0] bytes).
+  void inflate(size_t b0, size_t b1, uint8_t* dst, BgzfInflater& inf) const {
+    for (size_t b = b0; b < b1; ++b) {
+      const BlockRef& r = blocks[b];
+      uint8_t* out = dst + (ustart[b] - ustart[b0]);
+      if (!bgzf) {
+        memcpy(out, p + r.cdata, r.clen);
+        continue;
+      }
+      if (!inf.block(p + r.cdata, r.clen, out, r.isize)) throw Panic("Error reading BAM record: BGZF inflate failed");
+    }
+  }
+
+ private:
+  size_t next_header_ = 0;  // BGZF: file offset of the first block header not in the table yet
+
+  void add(const BlockRef& b) {
+    blocks.push_back(b);
+    ustart.push_back(ustart.back() + b.isize);
+  }
+  // The block whose header is at `o`, and the offset after it; nullptr, or what is wrong with the header.
+  const char* parse(size_t o, BlockRef& b, size_t& end) const {
+    if (o + 18 > n || p[o] != 0x1f || p[o + 1] != 0x8b || p[o + 2] != 8 || !(p[o + 3] & 4)) return "corrupt BGZF block header";
+    const size_t xlen = p[o + 10] | (p[o + 11] << 8);
+    size_t x = o + 12;
+    const size_t xend = x + xlen;
+    if (xend > n) return "truncated BGZF block";
+    int bsize = -1;
+    while (x + 4 <= xend) {
+      const size_t slen = p[x + 2] | (p[x + 3] << 8);
+      if (p[x] == 'B' && p[x + 1] == 'C' && slen == 2) bsize = p[x + 4] | (p[x + 5] << 8);
+      x += 4 + slen;
+    }
+    if (bsize < 0) return "gzip member without a BGZF block size";
+    const size_t e = o + (size_t)bsize + 1;
+    if (e > n || e < xend + 8) return "truncated BGZF block";
+    b.cdata = xend;
+    b.clen = e - 8 - xend;
+    b.isize = rd_u32(p + e - 4);
+    end = e;
+    return nullptr;
+  }
+};
+
+// Streams the uncompressed bytes of a BGZF (or plain gzip, or uncompressed) input in windows, building its block index on
+// the way.
 class InflateStream {
  public:
-  InflateStream(const uint8_t* p, size_t n, ThreadPool& pool, size_t window_bytes)
-      : p_(p), n_(n), pool_(pool), window_(window_bytes) {
-    if (n_ >= 2 && p_[0] == 0x1f && p_[1] == 0x8b) {
-      kind_ = probe_bgzf(0) ? BGZF : GZIP;
-      if (kind_ == GZIP) {  // not block-indexable: inflate everything once (small inputs only)
-        inflate_whole();
-        kind_ = RAW;
-      }
-    } else {
-      kind_ = RAW;
-      raw_p_ = p_;
-      raw_n_ = n_;
+  InflateStream(const uint8_t* p, size_t n, ThreadPool& pool, size_t window_bytes) : pool_(pool), window_(window_bytes) {
+    index_.start(p, n);
+    if (!index_.bgzf && n >= 2 && p[0] == 0x1f && p[1] == 0x8b) {  // plain gzip, not block-indexable: inflate it whole
+      inflate_whole(p, n);                                           // (small inputs only)
+      index_.start(whole_.data(), whole_.size(), false);
     }
   }
   // Appends up to ~window bytes of uncompressed data to buf (after buf.size()). Returns false at EOF (nothing appended).
   bool fill(std::vector<uint8_t>& buf) {
-    if (kind_ == RAW) {
-      if (raw_off_ >= raw_n_) return false;
-      size_t take = std::min(window_, raw_n_ - raw_off_);
-      size_t o = buf.size();
-      buf.resize(o + take);
-      memcpy(buf.data() + o, raw_p_ + raw_off_, take);
-      raw_off_ += take;
-      return true;
-    }
-    blocks_.clear();
-    size_t total = 0;
-    while (off_ < n_ && total < window_) {
-      Block b;
-      if (!parse_block(off_, b)) throw Panic("Error reading BAM record: corrupt BGZF block header");
-      b.out_off = total;
-      total += b.isize;
-      blocks_.push_back(b);
-      off_ = b.next;
-    }
-    if (blocks_.empty()) return false;
-    size_t o = buf.size();
-    buf.resize(o + total);
+    const size_t b0 = next_;
+    while (index_.ustart[next_] - index_.ustart[b0] < window_ && (next_ < index_.blocks.size() || index_.next())) ++next_;
+    if (next_ == b0) return false;
+    const size_t o = buf.size();
+    buf.resize(o + (index_.ustart[next_] - index_.ustart[b0]));
     uint8_t* out = buf.data() + o;
-    std::atomic<bool> bad{false};
-    // group blocks so that each task is ~256 KB of output
-    const size_t per = 4;
-    const size_t n_tasks = (blocks_.size() + per - 1) / per;
-    pool_.parallel_for(n_tasks, [&](size_t task, int) {
+    const size_t per = 4;  // blocks per task: ~256 KB of output
+    pool_.parallel_for((next_ - b0 + per - 1) / per, [&](size_t task, int) {
       BgzfInflater inf;
-      for (size_t i = task * per; i < std::min(blocks_.size(), (task + 1) * per); ++i) {
-        const Block& b = blocks_[i];
-        if (!inf.block(p_ + b.cdata, b.clen, out + b.out_off, b.isize)) bad = true;
-      }
+      const size_t t0 = b0 + task * per;
+      index_.inflate(t0, std::min(next_, t0 + per), out + (index_.ustart[t0] - index_.ustart[b0]), inf);
     });
-    if (bad) throw Panic("Error reading BAM record: BGZF inflate failed");
     return true;
   }
   void set_window(size_t window_bytes) { window_ = window_bytes; }
-  bool is_bgzf() const { return kind_ == BGZF; }
-  size_t compressed_consumed() const { return off_; }  // BGZF: file bytes behind everything fill() has returned so far
-  uint64_t compressed_bytes() const { return n_; }
-  // uncompressed / fully inflated inputs: the raw byte range (BlockIndex cuts it into slices)
-  bool is_raw() const { return kind_ == RAW; }
-  const uint8_t* raw_data() const { return raw_p_; }
-  size_t raw_size() const { return raw_n_; }
+  bool is_bgzf() const { return index_.bgzf; }
+  // The whole block table (of the inflated bytes for plain gzip); a Panic at the first bad block header.
+  const BlockIndex& index() { return index_.finish(); }
 
  private:
-  struct Block {
-    size_t cdata, clen, next, out_off;
-    uint32_t isize;
-  };
-  enum Kind { BGZF, GZIP, RAW } kind_;
-  const uint8_t* p_;
-  size_t n_;
   ThreadPool& pool_;
   size_t window_;
-  size_t off_ = 0;
-  std::vector<Block> blocks_;
+  BlockIndex index_;
+  size_t next_ = 0;  // first block fill() has not returned yet
   std::vector<uint8_t> whole_;
-  const uint8_t* raw_p_ = nullptr;
-  size_t raw_n_ = 0, raw_off_ = 0;
 
-  bool probe_bgzf(size_t o) {
-    Block b;
-    return parse_block(o, b);
-  }
-  bool parse_block(size_t o, Block& b) {
-    if (o + 18 > n_ || p_[o] != 0x1f || p_[o + 1] != 0x8b || p_[o + 2] != 8 || !(p_[o + 3] & 4)) return false;
-    if (p_[o + 3] & ~4) return false;
-    size_t xlen = p_[o + 10] | (p_[o + 11] << 8);
-    size_t x = o + 12, xend = x + xlen;
-    if (xend > n_) return false;
-    int bsize = -1;
-    while (x + 4 <= xend) {
-      size_t slen = p_[x + 2] | (p_[x + 3] << 8);
-      if (p_[x] == 'B' && p_[x + 1] == 'C' && slen == 2) bsize = p_[x + 4] | (p_[x + 5] << 8);
-      x += 4 + slen;
-    }
-    if (bsize < 0) return false;
-    size_t end = o + (size_t)bsize + 1;
-    if (end > n_ || end < xend + 8) return false;
-    b.cdata = xend;
-    b.clen = end - 8 - xend;
-    b.isize = p_[end - 4] | (p_[end - 3] << 8) | (p_[end - 2] << 16) | ((uint32_t)p_[end - 1] << 24);
-    b.next = end;
-    return true;
-  }
-  void inflate_whole() {
+  void inflate_whole(const uint8_t* p, size_t n) {
     z_stream zs;
     memset(&zs, 0, sizeof zs);
     if (inflateInit2(&zs, 15 + 32) != Z_OK) throw Panic("zlib init failed");
-    zs.next_in = const_cast<Bytef*>(p_);
-    zs.avail_in = (uInt)n_;
+    zs.next_in = const_cast<Bytef*>(p);
+    zs.avail_in = (uInt)n;
     std::vector<uint8_t> chunk(1 << 20);
     for (;;) {
       zs.next_out = chunk.data();
@@ -254,22 +438,144 @@ class InflateStream {
       }
     }
     inflateEnd(&zs);
-    raw_p_ = whole_.data();
-    raw_n_ = whole_.size();
   }
 };
 
-inline uint32_t rd_u32(const uint8_t* p) {
-  uint32_t v;
-  memcpy(&v, p, 4);
-  return v;
-}
-inline uint16_t rd_u16(const uint8_t* p) {
-  uint16_t v;
-  memcpy(&v, p, 2);
-  return v;
+// The BAM header (SAMv1 §4.2) read from the start of a stream.
+struct BamHeader {
+  std::shared_ptr<Header> header;  // nullptr: the reference list is byte for byte the caller's `known_refs`
+  size_t refs_at = 0;              // offset of n_ref; the @-text in front of it (e.g. @PG) may differ between samples
+  uint64_t records_at = 0;         // offset of the first record: [refs_at, records_at) is the raw reference list
+};
+// Reads the header into the empty `buf`, which then holds at least the header's bytes.
+inline BamHeader read_bam_header(InflateStream& stream, std::vector<uint8_t>& buf, const std::string& path,
+                                 const std::vector<uint8_t>& known_refs = {}) {
+  auto need = [&](size_t bytes) {  // buf[0, bytes) available; false at EOF
+    while (buf.size() < bytes)
+      if (!stream.fill(buf)) return false;
+    return true;
+  };
+  BamHeader h;
+  if (!need(12) || memcmp(buf.data(), "BAM\1", 4) != 0) throw Panic("Error reading BAM header: not a BAM/SAM file: " + path);
+  const uint32_t l_text = rd_u32(buf.data() + 4);
+  if (!need(12 + (size_t)l_text)) throw Panic("Error reading BAM header: truncated");
+  h.refs_at = 8 + (size_t)l_text;
+  if (known_refs.size() >= 4 && need(h.refs_at + known_refs.size()) &&
+      memcmp(buf.data() + h.refs_at, known_refs.data(), known_refs.size()) == 0) {
+    h.records_at = h.refs_at + known_refs.size();
+    return h;
+  }
+  h.header = std::make_shared<Header>();
+  const uint32_t n_ref = rd_u32(buf.data() + h.refs_at);
+  size_t o = h.refs_at + 4;
+  h.header->names.reserve(n_ref);
+  h.header->lens.reserve(n_ref);
+  for (uint32_t i = 0; i < n_ref; ++i) {
+    if (!need(o + 4)) throw Panic("Error reading BAM header: truncated");
+    const uint32_t l_name = rd_u32(buf.data() + o);
+    if (!need(o + 8 + l_name)) throw Panic("Error reading BAM header: truncated");
+    h.header->names.emplace_back((const char*)buf.data() + o + 4, l_name ? l_name - 1 : 0);
+    h.header->lens.push_back(rd_u32(buf.data() + o + 4 + l_name));
+    o += 8 + l_name;
+  }
+  h.records_at = o;
+  return h;
 }
 
+// cmb_bgzf_input over the blocks of a BGZF index (the device inflates and decodes them itself), with the per-block arrays it
+// points at.
+class BgzfInput {
+ public:
+  cmb_bgzf_input in{};
+  BgzfInput(const BlockIndex& bx, uint32_t n_ref, uint64_t records_at, int threads)
+      : coff_(bx.blocks.size()), clen_(bx.blocks.size()), isz_(bx.blocks.size()) {
+    for (size_t b = 0; b < bx.blocks.size(); ++b) {
+      coff_[b] = bx.blocks[b].cdata;
+      clen_[b] = (uint32_t)bx.blocks[b].clen;
+      isz_[b] = bx.blocks[b].isize;
+    }
+    in.data = bx.p;
+    in.size = bx.n;
+    in.n_blocks = (uint32_t)bx.blocks.size();
+    in.n_ref = n_ref;
+    in.block_coffset = coff_.data();
+    in.block_clen = clen_.data();
+    in.block_isize = isz_.data();
+    in.records_at = records_at;
+    in.copy_threads = (uint32_t)std::min(threads, 8);
+  }
+  BgzfInput(const BgzfInput&) = delete;
+
+ private:
+  std::vector<uint64_t> coff_;
+  std::vector<uint32_t> clen_, isz_;
+};
+
+// A BAM record header that could be real: sane block_size, reference ids, name length and NUL, field sizes.  Shared by
+// the speculative record alignment of the host decoder (decode_runner.hpp) and the block-range probe (shard_range.hpp).
+inline bool record_plausible(const uint8_t* buf, size_t s, size_t usize, uint32_t n_ref) {
+  if (s + 36 > usize) return false;
+  const uint32_t bs = rd_u32(buf + s);
+  if (bs < 32 || bs > (64u << 20)) return false;
+  const int32_t tid = (int32_t)rd_u32(buf + s + 4), pos = (int32_t)rd_u32(buf + s + 8), mtid = (int32_t)rd_u32(buf + s + 24);
+  if (tid < -1 || tid >= (int32_t)n_ref || mtid < -1 || mtid >= (int32_t)n_ref || pos < -1) return false;
+  const uint32_t l_name = buf[s + 12], n_cig = rd_u16(buf + s + 16), l_seq = rd_u32(buf + s + 20);
+  if (l_name == 0 || l_seq > (1u << 28)) return false;
+  const uint64_t fixed = 32ull + l_name + 4ull * n_cig + (l_seq + 1) / 2 + l_seq;
+  if (fixed > bs) return false;
+  if (s + 36 + l_name <= usize && buf[s + 36 + l_name - 1] != 0) return false;
+  return true;
+}
+
+// Walks the block_size chain of the records in buf[from, size): f(offset) for every complete record, until f returns false.
+// Returns where the walk stopped.  `at_eof`: the stream ends at `size`, and bytes left over there are a record cut short --
+// htslib's bam_read1 fails on it and the reference panics on the Err (contig.rs:113-115).
+template <class F>
+inline size_t walk_records(const uint8_t* buf, size_t from, size_t size, bool at_eof, F f) {
+  size_t q = from;
+  while (q + 4 <= size) {
+    const uint32_t bs = rd_u32(buf + q);
+    if (bs < 32) throw Panic("Error reading BAM record: corrupt block_size");
+    if (q + 4 + (size_t)bs > size) break;
+    const size_t rec = q;
+    q += 4 + (size_t)bs;
+    if (!f(rec)) break;
+  }
+  if (at_eof && q != size) throw Panic("Error reading BAM record: truncated");
+  return q;
+}
+
+// Walks the aux fields in [a, end) (SAMv1 §4.2.4): f(tag0, tag1, type, value, size) for each, until f returns true.  A 'B'
+// array cut short by `end` comes with the bytes that are left (size < 5).  Returns false at an unknown type.
+template <class F>
+inline bool walk_aux(const uint8_t* a, const uint8_t* end, F f) {
+  while (a + 3 <= end) {
+    const uint8_t t0 = a[0], t1 = a[1], ty = a[2];
+    a += 3;
+    size_t sz;
+    switch (ty) {
+      case 'A': case 'c': case 'C': sz = 1; break;
+      case 's': case 'S': sz = 2; break;
+      case 'i': case 'I': case 'f': sz = 4; break;
+      case 'Z': case 'H': {
+        const uint8_t* e = (const uint8_t*)memchr(a, 0, (size_t)(end - a));
+        sz = e ? (size_t)(e - a) + 1 : (size_t)(end - a);
+        break;
+      }
+      case 'B': {
+        if (a + 5 > end) { sz = (size_t)(end - a); break; }
+        const uint8_t sub = a[0];
+        const size_t es = (sub == 'c' || sub == 'C') ? 1 : (sub == 's' || sub == 'S') ? 2 : 4;
+        sz = 5 + es * (size_t)rd_u32(a + 1);
+        break;
+      }
+      default: return false;
+    }
+    if (f(t0, t1, ty, a, sz)) return true;
+    a += sz;
+  }
+  return true;
+}
 
 // ---- record layout checks shared by every host decoder -------------------------------------------------------------
 // htslib's bam_read1 rejects a record whose fixed-size fields do not fit its block_size (the reference then panics with
@@ -295,40 +601,20 @@ inline CigarView effective_cigar(const uint8_t* rec) {
   const uint32_t op0 = rd_u32(v.ops);
   if ((op0 & 0xf) != 4 || (op0 >> 4) != l_seq) return v;  // not the placeholder: the common case ends here
   if ((int32_t)rd_u32(o) < 0 || (int32_t)rd_u32(o + 4) < 0) return v;
-  const uint8_t* a = o + fixed;
   const uint8_t* end = o + block_size;
-  while (a + 3 <= end) {  // bam_aux_get(b, "CG")
-    const uint8_t t0 = a[0], t1 = a[1], ty = a[2];
-    a += 3;
-    size_t sz;
-    switch (ty) {
-      case 'A': case 'c': case 'C': sz = 1; break;
-      case 's': case 'S': sz = 2; break;
-      case 'i': case 'I': case 'f': sz = 4; break;
-      case 'Z': case 'H': {
-        const uint8_t* e = (const uint8_t*)memchr(a, 0, (size_t)(end - a));
-        sz = e ? (size_t)(e - a) + 1 : (size_t)(end - a);
-        break;
-      }
-      case 'B': {
-        if (a + 5 > end) return v;
-        const uint8_t sub = a[0];
-        const uint32_t cnt = rd_u32(a + 1);
-        const size_t es = (sub == 'c' || sub == 'C') ? 1 : (sub == 's' || sub == 'S') ? 2 : 4;
-        sz = 5 + es * (size_t)cnt;
-        if (t0 == 'C' && t1 == 'G') {
-          if ((sub == 'I' || sub == 'i') && cnt >= n_cigar && cnt < (1u << 29) && a + sz <= end) {
-            v.ops = a + 5;
-            v.n = cnt;
-          }
-          return v;
-        }
-        break;
-      }
-      default: return v;  // the NM walk raises the unknown-aux-type error
+  // bam_aux_get(b, "CG"); an unknown aux type ends the search (the NM walk raises the error)
+  walk_aux(o + fixed, end, [&](uint8_t t0, uint8_t t1, uint8_t ty, const uint8_t* a, size_t sz) {
+    if (ty != 'B') return false;
+    if (sz < 5) return true;
+    if (t0 != 'C' || t1 != 'G') return false;
+    const uint8_t sub = a[0];
+    const uint32_t cnt = rd_u32(a + 1);
+    if ((sub == 'I' || sub == 'i') && cnt >= n_cigar && cnt < (1u << 29) && sz <= (size_t)(end - a)) {
+      v.ops = a + 5;
+      v.n = cnt;
     }
-    a += sz;
-  }
+    return true;
+  });
   return v;
 }
 [[noreturn]] inline void throw_bad_record_layout() {
@@ -340,12 +626,12 @@ inline int64_t record_cigar_ops(const uint8_t* rec) {
   return v.valid ? (int64_t)v.n : -1;
 }
 
-// Decode the fixed fields, CIGAR summary and NM aux of one BAM record (`rec` points at block_size).
-// Intervals (M/=/X blocks, contig.rs:171-186) are appended to iv_start/iv_len.
-inline void decode_bam_record(const uint8_t* rec, Tuple& t, std::vector<int32_t>& iv_start, std::vector<int32_t>& iv_len) {
+// Decode the fixed fields, CIGAR summary and NM aux of one BAM record (`rec` points at block_size); M/=/X blocks
+// (contig.rs:171-186) are written to ivs/ivl (room for record_cigar_ops entries).  A block starting before the contig is
+// clamped to -1 as on the device (cmb_decode.cuh), which K1 rejects as out of bounds.  Returns the number of intervals.
+inline uint32_t decode_bam_record(const uint8_t* rec, Tuple& t, int32_t* ivs, int32_t* ivl) {
   const uint32_t block_size = rd_u32(rec);
   const uint8_t* o = rec + 4;
-  const uint8_t* end = o + block_size;
   t.tid = (int32_t)rd_u32(o);
   t.pos = (int32_t)rd_u32(o + 4);
   const uint32_t l_read_name = o[8];
@@ -356,7 +642,6 @@ inline void decode_bam_record(const uint8_t* rec, Tuple& t, std::vector<int32_t>
   t.mtid = (int32_t)rd_u32(o + 20);
   const CigarView cv = effective_cigar(rec);
   if (!cv.valid) throw_bad_record_layout();
-  const uint8_t* cig = o + 32 + l_read_name;
   uint32_t aligned = 0, del = 0, ins = 0, n_iv = 0;
   int64_t cursor = t.pos;
   for (uint32_t i = 0; i < cv.n; ++i) {
@@ -364,8 +649,8 @@ inline void decode_bam_record(const uint8_t* rec, Tuple& t, std::vector<int32_t>
     const uint32_t op = v & 0xf, len = v >> 4;
     switch (op) {
       case 0: case 7: case 8:  // M = X
-        iv_start.push_back((int32_t)std::min<int64_t>(cursor, INT32_MAX));
-        iv_len.push_back((int32_t)len);
+        ivs[n_iv] = cursor < 0 ? -1 : (int32_t)std::min<int64_t>(cursor, INT32_MAX);
+        ivl[n_iv] = (int32_t)len;
         ++n_iv;
         cursor += len;
         aligned += len;
@@ -381,45 +666,79 @@ inline void decode_bam_record(const uint8_t* rec, Tuple& t, std::vector<int32_t>
   t.ins = ins;
   t.n_iv = n_iv;
   // aux: NM (lib.rs:139-156: U8/U16/U32 accepted, anything else is a type panic, absent is a panic)
-  const uint8_t* a = cig + 4 * (size_t)n_cigar + (t.l_seq + 1) / 2 + t.l_seq;
   t.nm_state = 0;
   t.nm = 0;
-  while (a + 3 <= end) {
-    const uint8_t t0 = a[0], t1 = a[1], ty = a[2];
-    a += 3;
-    size_t sz;
-    switch (ty) {
-      case 'A': case 'c': case 'C': sz = 1; break;
-      case 's': case 'S': sz = 2; break;
-      case 'i': case 'I': case 'f': sz = 4; break;
-      case 'Z': case 'H': {
-        const uint8_t* e = (const uint8_t*)memchr(a, 0, (size_t)(end - a));
-        sz = e ? (size_t)(e - a) + 1 : (size_t)(end - a);
-        break;
-      }
-      case 'B': {
-        if (a + 5 > end) { sz = (size_t)(end - a); break; }
-        const uint8_t sub = a[0];
-        const uint32_t cnt = rd_u32(a + 1);
-        const size_t es = (sub == 'c' || sub == 'C') ? 1 : (sub == 's' || sub == 'S') ? 2 : 4;
-        sz = 5 + es * (size_t)cnt;
-        break;
-      }
-      default: throw Panic("Error reading BAM record: unknown aux type");
-    }
+  const uint8_t* aux = o + 32 + l_read_name + 4 * (size_t)n_cigar + (t.l_seq + 1) / 2 + t.l_seq;
+  const bool known = walk_aux(aux, o + block_size, [&](uint8_t t0, uint8_t t1, uint8_t ty, const uint8_t* a, size_t) {
     if (t0 == 'N' && t1 == 'M' && t.nm_state == 0) {
       if (ty == 'C') { t.nm_state = 1; t.nm = a[0]; }
       else if (ty == 'S') { t.nm_state = 1; t.nm = rd_u16(a); }
       else if (ty == 'I') { t.nm_state = 1; t.nm = rd_u32(a); }
       else t.nm_state = 2;
     }
-    a += sz;
-  }
+    return false;  // the whole list is walked: an unknown type further on is still an error
+  });
+  if (!known) throw Panic("Error reading BAM record: unknown aux type");
+  return n_iv;
+}
+// The same, appending the intervals to ivs/ivl.
+inline void decode_bam_record(const uint8_t* rec, Tuple& t, std::vector<int32_t>& ivs, std::vector<int32_t>& ivl) {
+  const int64_t ops = record_cigar_ops(rec);
+  if (ops < 0) throw_bad_record_layout();
+  const size_t at = ivs.size();
+  ivs.resize(at + (size_t)ops);
+  ivl.resize(at + (size_t)ops);
+  const uint32_t n_iv = decode_bam_record(rec, t, ivs.data() + at, ivl.data() + at);
+  ivs.resize(at + n_iv);
+  ivl.resize(at + n_iv);
+}
+
+// Row r of a tuple table in SoA form (a cmb_read_batch, or cmbh_tuples) whose intervals start at `iv`; ivs/ivl are copied
+// there, or are there already when nullptr.
+template <class Soa>
+inline void put_tuple(const Soa& b, size_t r, uint32_t iv, const Tuple& t, const int32_t* ivs, const int32_t* ivl) {
+  b.tid[r] = t.tid; b.pos[r] = t.pos; b.flag[r] = t.flag; b.mapq[r] = t.mapq; b.nm_state[r] = t.nm_state;
+  b.nm[r] = t.nm; b.l_seq[r] = t.l_seq; b.aligned[r] = t.aligned; b.del[r] = t.del; b.ins[r] = t.ins;
+  b.iv_begin[r] = iv;
+  if (ivs)
+    for (uint32_t k = 0; k < t.n_iv; ++k) {
+      b.iv_start[iv + k] = ivs[k];
+      b.iv_len[iv + k] = ivl[k];
+    }
 }
 
 inline std::string bam_qname(const uint8_t* rec) {
   const uint32_t l = rec[4 + 8];
   return std::string((const char*)rec + 4 + 32, l ? l - 1 : 0);
 }
+
+// The host's mate matching, ReferenceSortedBamFilter's (filter.rs:149-224), over the proper-pair records of a stream in
+// stream order: the names kept are forgotten when the reference changes, a first mate is kept only when its mate maps to
+// the current reference, and the second record of a name hands the kept first mate back.  Which records take part is the
+// caller's business.
+template <class Stored>
+class HostMates {
+ public:
+  // The kept first mate of `t`, if any; otherwise make()'s copy of `t` is kept when its mate maps to the current reference.
+  template <class Make>
+  std::optional<Stored> match(const Tuple& t, std::string qname, Make make) {
+    if (t.tid != current_reference_) {
+      current_reference_ = t.tid;
+      first_set_.clear();
+    }
+    auto it = first_set_.find(qname);
+    if (it == first_set_.end()) {
+      if (t.mtid == current_reference_) first_set_.emplace(std::move(qname), make());
+      return std::nullopt;
+    }
+    std::optional<Stored> first(std::move(it->second));
+    first_set_.erase(it);
+    return first;
+  }
+
+ private:
+  std::map<std::string, Stored> first_set_;  // filter.rs:16-18
+  int32_t current_reference_ = -1;
+};
 
 }  // namespace cmbh

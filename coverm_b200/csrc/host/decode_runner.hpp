@@ -1,4 +1,4 @@
-// The task scheduler of the region-parallel BAM decode (see decode_pipeline.hpp for the pieces it runs).
+// The task scheduler of the region-parallel BAM decode (the block index and the record decoder it runs are in bam_source.hpp).
 //
 // Work items are ~1 MB of uncompressed data (whole BGZF blocks).  Three kinds of work, none of which ever blocks on
 // another thread:
@@ -13,10 +13,15 @@
 // The calling thread is the coordinator: it alone talks to the (not thread-safe) device ABI — it keeps one staging
 // batch acquired ahead of the chain and submits each batch once every item assigned to it has been extracted.
 #pragma once
+#include <atomic>
 #include <chrono>
 #include <deque>
+#include <exception>
+#include <memory>
+#include <mutex>
+#include <thread>
 
-#include "decode_pipeline.hpp"
+#include "bam_source.hpp"
 
 namespace cmbh {
 
@@ -185,16 +190,13 @@ PipelineCounts run_decode_pipeline(const BlockIndex& bx, uint64_t records_at, ui
       carry.assign(buf + it.guess_tail, buf + usize);
     } else {
       w.offs.clear();
-      while (pos + 4 <= usize) {
-        const uint32_t bs = rd_u32(buf + pos);
-        if (bs < 32) throw Panic("Error reading BAM record: corrupt block_size");
-        if (pos + 4 + (size_t)bs > usize) break;
-        w.offs.push_back((uint32_t)pos);
-        const int64_t ops = record_cigar_ops(buf + pos);
+      pos = walk_records(buf, pos, usize, false, [&](size_t rec) {
+        const int64_t ops = record_cigar_ops(buf + rec);
         if (ops < 0) throw_bad_record_layout();
+        w.offs.push_back((uint32_t)rec);
         ub_iv += (uint64_t)ops;
-        pos += 4 + (size_t)bs;
-      }
+        return true;
+      });
       carry.assign(buf + pos, buf + usize);
     }
     const uint32_t n_rec = (uint32_t)w.offs.size() + (it.have_stitched ? 1u : 0u);
@@ -309,10 +311,8 @@ PipelineCounts run_decode_pipeline(const BlockIndex& bx, uint64_t records_at, ui
     uint32_t r = it.r0, iv = it.i0;
     Tuple t;
     auto put = [&](const uint8_t* rec) {
-      const uint32_t n_iv = decode_bam_record_into(rec, t, b.iv_start + iv, b.iv_len + iv);
-      b.tid[r] = t.tid; b.pos[r] = t.pos; b.flag[r] = t.flag; b.mapq[r] = t.mapq; b.nm_state[r] = t.nm_state;
-      b.nm[r] = t.nm; b.l_seq[r] = t.l_seq; b.aligned[r] = t.aligned; b.del[r] = t.del; b.ins[r] = t.ins;
-      b.iv_begin[r] = iv;
+      const uint32_t n_iv = decode_bam_record(rec, t, b.iv_start + iv, b.iv_len + iv);
+      put_tuple(b, r, iv, t, nullptr, nullptr);
       iv += n_iv;
       ++r;
       if (!(t.flag & 0x900)) ++my_primaries;

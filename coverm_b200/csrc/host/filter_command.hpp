@@ -8,7 +8,6 @@
 // (filter.rs:342-844) state their expectations.
 #pragma once
 #include <fstream>
-#include <map>
 
 #include "sample_processor.hpp"
 
@@ -43,18 +42,15 @@ inline void filter_on_host(const uint8_t* recs, size_t n_bytes, const HostFilter
     Tuple t;
     size_t off, size;
   };
-  std::map<std::string, Stored> first_set;
-  int32_t current_reference = -1;
+  HostMates<Stored> mates;
   std::vector<int32_t> ivs, ivl;
   auto emit = [&](size_t off, size_t size) {
     out.insert(out.end(), recs + off, recs + off + size);
     ++n_out;
   };
   const bool singles = f.filter_single && !f.filter_pairs;
-  for (size_t o = 0; o + 4 <= n_bytes;) {
-    const uint32_t bs = rd_u32(recs + o);
-    if (bs < 32 || o + 4 + (size_t)bs > n_bytes) throw Panic("Error reading BAM record: truncated");
-    const size_t size = 4 + (size_t)bs;
+  walk_records(recs, 0, n_bytes, true, [&](size_t o) {
+    const size_t size = 4 + (size_t)rd_u32(recs + o);
     Tuple t;
     ivs.clear();
     ivl.clear();
@@ -71,29 +67,17 @@ inline void filter_on_host(const uint8_t* recs, size_t n_bytes, const HostFilter
       else if (secondary || supplementary) {
       } else if (!proper) {
         if (!f.filter_out) emit(o, size);
-      } else {
-        if (t.tid != current_reference) {
-          current_reference = t.tid;
-          first_set.clear();
-        }
-        std::string qname = bam_qname(recs + o);
-        auto it = first_set.find(qname);
-        if (it == first_set.end()) {
-          if (t.mtid == current_reference) first_set.emplace(std::move(qname), Stored{t, o, size});
-        } else {
-          const Stored s = it->second;
-          first_set.erase(it);
-          const bool passes = (!f.filter_single || (host_single_read_passes(s.t, f.p) && host_single_read_passes(t, f.p))) &&
-                              host_read_pair_passes(t, s.t, f.p);
-          if (passes == f.filter_out) {
-            emit(s.off, s.size);
-            emit(o, size);
-          }
+      } else if (const std::optional<Stored> s = mates.match(t, bam_qname(recs + o), [&] { return Stored{t, o, size}; })) {
+        const bool passes = (!f.filter_single || (host_single_read_passes(s->t, f.p) && host_single_read_passes(t, f.p))) &&
+                            host_read_pair_passes(t, s->t, f.p);
+        if (passes == f.filter_out) {
+          emit(s->off, s->size);
+          emit(o, size);
         }
       }
     }
-    o += size;
-  }
+    return true;
+  });
 }
 
 // BGZF writer: `data` cut into blocks of at most 0xff00 bytes, deflated on all threads, followed by the EOF marker.
@@ -162,66 +146,20 @@ struct FilterRun {
 // One input through the filter.  `params`: thresholds + flag includes with filtering = 1; inverse = --inverse.
 inline FilterRun filter_one_input(DeviceSession& session, const InputSpec& in, const cmb_params& params, bool inverse) {
   FilterRun run;
-  ByteSource bytes(in);
-  std::vector<uint8_t> sam_as_bam;
-  const uint8_t* p = bytes.data();
-  size_t n = bytes.size();
-  Header sam_header;
-  if (!(n >= 2 && p[0] == 0x1f && p[1] == 0x8b) && SamToBam::looks_like_sam(p, n)) {
-    SamToBam::convert(p, n, sam_header, sam_as_bam);
-    p = sam_as_bam.data();
-    n = sam_as_bam.size();
-  }
+  const BamInput input(in);
   cmb_ctx* ctx = session.ctx();
   cmb_filter_mode mode{};
   int rc = cmb_set_params(ctx, &params, &mode);
   if (rc) throw_device_error(ctx, rc);
-  // header: inflate from the start until the reference list is complete
-  InflateStream stream(p, n, session.pool(), 1u << 20);
+  InflateStream stream(input.data(), input.size(), session.pool(), 1u << 20);
   std::vector<uint8_t> buf;
-  auto need = [&](size_t want) {
-    while (buf.size() < want)
-      if (!stream.fill(buf)) return false;
-    return true;
-  };
-  if (!need(12) || memcmp(buf.data(), "BAM\1", 4) != 0) throw Panic("Error reading BAM header: not a BAM/SAM file: " + in.path);
-  const uint32_t l_text = rd_u32(buf.data() + 4);
-  if (!need(12 + (size_t)l_text)) throw Panic("Error reading BAM header: truncated");
-  const uint32_t n_ref = rd_u32(buf.data() + 8 + l_text);
-  size_t o = 12 + (size_t)l_text;
-  for (uint32_t i = 0; i < n_ref; ++i) {
-    if (!need(o + 4)) throw Panic("Error reading BAM header: truncated");
-    const uint32_t l_name = rd_u32(buf.data() + o);
-    if (!need(o + 8 + l_name)) throw Panic("Error reading BAM header: truncated");
-    o += 8 + l_name;
-  }
-  const uint64_t records_at = o;
-  run.header_bytes.assign(buf.begin(), buf.begin() + (ptrdiff_t)o);
-
-  BlockIndex bx;
-  if (stream.is_raw()) bx.build(stream.raw_data(), stream.raw_size());
-  else bx.build(p, n);
-  if (bx.bgzf && !stream.is_raw() && !getenv("CMB_HOST_DECODE")) {
-    const size_t nb = bx.blocks.size();
-    std::vector<uint64_t> coff(nb);
-    std::vector<uint32_t> clen(nb), isz(nb);
-    for (size_t b = 0; b < nb; ++b) {
-      coff[b] = bx.blocks[b].cdata;
-      clen[b] = (uint32_t)bx.blocks[b].clen;
-      isz[b] = bx.blocks[b].isize;
-    }
-    cmb_bgzf_input bi{};
-    bi.data = p;
-    bi.size = n;
-    bi.n_blocks = (uint32_t)nb;
-    bi.n_ref = n_ref;
-    bi.block_coffset = coff.data();
-    bi.block_clen = clen.data();
-    bi.block_isize = isz.data();
-    bi.records_at = records_at;
-    bi.copy_threads = (uint32_t)std::min(session.pool().size(), 8);
+  const BamHeader h = read_bam_header(stream, buf, in.path);
+  run.header_bytes.assign(buf.begin(), buf.begin() + (ptrdiff_t)h.records_at);
+  const BlockIndex& bx = stream.index();
+  if (bx.bgzf && !getenv("CMB_HOST_DECODE")) {
+    const BgzfInput bi(bx, (uint32_t)h.header->names.size(), h.records_at, session.pool().size());
     cmb_bgzf_result br{};
-    rc = cmb_decode_bgzf(ctx, &bi, &br);
+    rc = cmb_decode_bgzf(ctx, &bi.in, &br);
     if (rc == CMB_OK) {
       uint64_t n_rec = 0, n_bytes = 0;
       rc = cmb_filter_plan(ctx, inverse ? 1 : 0, &n_rec, &n_bytes);
@@ -243,7 +181,7 @@ inline FilterRun filter_one_input(DeviceSession& session, const InputSpec& in, c
   f.filter_single = mode.filter_single_reads;
   f.filter_pairs = mode.filter_pairs;
   f.filter_out = !inverse;
-  filter_on_host(buf.data() + records_at, buf.size() - records_at, f, run.records, run.n_records);
+  filter_on_host(buf.data() + h.records_at, buf.size() - h.records_at, f, run.records, run.n_records);
   return run;
 }
 

@@ -225,36 +225,19 @@ int cmbh_extract_tuples(const char* path, const uint8_t* data, size_t size, int 
     in.data = data;
     in.size = size;
     ThreadPool pool(threads);
-    ByteSource bytes(in);
-    std::vector<uint8_t> sam_as_bam;
-    const uint8_t* p = bytes.data();
-    size_t n = bytes.size();
-    Header header;
-    if (!(n >= 2 && p[0] == 0x1f && p[1] == 0x8b) && SamToBam::looks_like_sam(p, n)) {
-      SamToBam::convert(p, n, header, sam_as_bam);
-      p = sam_as_bam.data();
-      n = sam_as_bam.size();
-    }
-    InflateStream stream(p, n, pool, 256u << 20);
+    const BamInput input(in);
+    InflateStream stream(input.data(), input.size(), pool, 256u << 20);
     std::vector<uint8_t> buf;
+    const BamHeader h = read_bam_header(stream, buf, in.path);
     while (stream.fill(buf)) {
     }
-    if (buf.size() < 12 || memcmp(buf.data(), "BAM\1", 4) != 0) throw Panic("not a BAM/SAM file");
-    size_t o = 12 + (size_t)rd_u32(buf.data() + 4);
-    const uint32_t n_ref = rd_u32(buf.data() + o - 4);
-    std::vector<uint64_t> lens;
-    for (uint32_t i = 0; i < n_ref; ++i) {
-      const uint32_t l_name = rd_u32(buf.data() + o);
-      lens.push_back(rd_u32(buf.data() + o + 4 + l_name));
-      o += 8 + l_name;
-    }
     std::vector<size_t> rec_off;
-    while (o + 4 <= buf.size()) {
-      const uint32_t bs = rd_u32(buf.data() + o);
-      if (o + 4 + (size_t)bs > buf.size()) break;
+    walk_records(buf.data(), h.records_at, buf.size(), true, [&](size_t o) {
       rec_off.push_back(o);
-      o += 4 + (size_t)bs;
-    }
+      return true;
+    });
+    const std::vector<uint64_t>& lens = h.header->lens;
+    const uint32_t n_ref = (uint32_t)lens.size();
     const size_t nrec = rec_off.size();
     constexpr size_t ITEM = 8192;
     const size_t n_items = (nrec + ITEM - 1) / ITEM;
@@ -272,11 +255,9 @@ int cmbh_extract_tuples(const char* path, const uint8_t* data, size_t size, int 
     pool.parallel_for(n_items, [&](size_t it, int) {
       Tuple t;
       for (size_t r = it * ITEM; r < std::min(nrec, (it + 1) * ITEM); ++r) {
-        const uint32_t before = (uint32_t)items[it].s.size();
+        const uint32_t before = (uint32_t)items[it].s.size();  // made global below, once every item's count is known
         decode_bam_record(buf.data() + rec_off[r], t, items[it].s, items[it].l);
-        out->tid[r] = t.tid; out->pos[r] = t.pos; out->flag[r] = t.flag; out->mapq[r] = t.mapq; out->nm_state[r] = t.nm_state;
-        out->nm[r] = t.nm; out->l_seq[r] = t.l_seq; out->aligned[r] = t.aligned; out->del[r] = t.del; out->ins[r] = t.ins;
-        out->iv_begin[r] = before;
+        put_tuple(*out, r, before, t, nullptr, nullptr);
       }
     });
     std::vector<uint64_t> base(n_items + 1, 0);

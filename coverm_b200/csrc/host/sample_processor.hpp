@@ -73,129 +73,6 @@ struct SampleResult {
   throw ExitError(1, "device error " + std::to_string(rc) + ": " + msg);
 }
 
-// Converts SAM text to BAM record bytes so that one decoder serves both (htslib reads SAM through the same
-// bam::Reader; tests/data/mapq_test.sam).  Integer aux tags get htslib's smallest-fitting type.
-class SamToBam {
- public:
-  static bool looks_like_sam(const uint8_t* p, size_t n) { return n == 0 || p[0] == '@' || (n > 4 && memcmp(p, "BAM\1", 4) != 0); }
-  static void convert(const uint8_t* p, size_t n, Header& header, std::vector<uint8_t>& out) {
-    std::unordered_map<std::string, int32_t> name_to_tid;
-    size_t o = 0;
-    auto next_line = [&](std::string& line) {
-      if (o >= n) return false;
-      size_t e = o;
-      while (e < n && p[e] != '\n') ++e;
-      line.assign((const char*)p + o, e - o);
-      o = e < n ? e + 1 : e;
-      if (!line.empty() && line.back() == '\r') line.pop_back();
-      return true;
-    };
-    auto split = [](const std::string& s) {
-      std::vector<std::string> v;
-      size_t a = 0;
-      for (;;) {
-        size_t b = s.find('\t', a);
-        if (b == std::string::npos) { v.push_back(s.substr(a)); break; }
-        v.push_back(s.substr(a, b - a));
-        a = b + 1;
-      }
-      return v;
-    };
-    out.assign({'B', 'A', 'M', 1});
-    std::string line;
-    std::vector<uint8_t> body;
-    auto put32 = [](std::vector<uint8_t>& v, uint32_t x) { for (int k = 0; k < 4; ++k) v.push_back((x >> (8 * k)) & 0xff); };
-    auto put16 = [](std::vector<uint8_t>& v, uint32_t x) { v.push_back(x & 0xff); v.push_back((x >> 8) & 0xff); };
-    bool header_done = false;
-    std::vector<uint8_t> recs;
-    while (next_line(line)) {
-      if (line.empty()) continue;
-      if (line[0] == '@' && !header_done) {
-        if (line.compare(0, 3, "@SQ") == 0) {
-          std::string sn;
-          uint64_t ln = 0;
-          for (auto& f : split(line)) {
-            if (f.compare(0, 3, "SN:") == 0) sn = f.substr(3);
-            if (f.compare(0, 3, "LN:") == 0) ln = strtoull(f.c_str() + 3, nullptr, 10);
-          }
-          name_to_tid[sn] = (int32_t)header.names.size();
-          header.names.push_back(sn);
-          header.lens.push_back(ln);
-        }
-        continue;
-      }
-      header_done = true;
-      auto f = split(line);
-      if (f.size() < 11) throw Panic("Error reading BAM record: malformed SAM line");
-      auto tid_of = [&](const std::string& s) -> int32_t {
-        if (s == "*") return -1;
-        auto it = name_to_tid.find(s);
-        if (it == name_to_tid.end()) throw Panic("Error reading BAM record: unknown reference " + s);
-        return it->second;
-      };
-      const int32_t tid = tid_of(f[2]);
-      std::vector<uint32_t> cigar;
-      if (f[5] != "*") {
-        const char* c = f[5].c_str();
-        while (*c) {
-          char* e;
-          const uint32_t len = (uint32_t)strtoul(c, &e, 10);
-          static const char* ops = "MIDNSHP=X";
-          const char* w = *e ? strchr(ops, *e) : nullptr;
-          if (!w) throw Panic("Error reading BAM record: bad CIGAR");
-          cigar.push_back((len << 4) | (uint32_t)(w - ops));
-          c = e + 1;
-        }
-      }
-      const uint32_t l_seq = f[9] == "*" ? 0 : (uint32_t)f[9].size();
-      body.clear();
-      put32(body, (uint32_t)tid);
-      put32(body, (uint32_t)((int32_t)strtol(f[3].c_str(), nullptr, 10) - 1));
-      body.push_back((uint8_t)std::min<size_t>(255, f[0].size() + 1));
-      body.push_back((uint8_t)strtoul(f[4].c_str(), nullptr, 10));
-      put16(body, 0);
-      put16(body, (uint32_t)cigar.size());
-      put16(body, (uint32_t)strtoul(f[1].c_str(), nullptr, 10));
-      put32(body, l_seq);
-      put32(body, (uint32_t)(f[6] == "=" ? tid : tid_of(f[6])));
-      put32(body, (uint32_t)((int32_t)strtol(f[7].c_str(), nullptr, 10) - 1));
-      put32(body, (uint32_t)strtol(f[8].c_str(), nullptr, 10));
-      body.insert(body.end(), f[0].begin(), f[0].begin() + std::min<size_t>(254, f[0].size()));
-      body.push_back(0);
-      for (uint32_t cg : cigar) put32(body, cg);
-      body.insert(body.end(), (l_seq + 1) / 2 + l_seq, 0);
-      for (size_t i = 11; i < f.size(); ++i) {
-        if (f[i].size() < 5 || f[i][2] != ':' || f[i][4] != ':') continue;
-        if (f[i][0] != 'N' || f[i][1] != 'M') continue;  // only NM matters on this path
-        body.push_back('N');
-        body.push_back('M');
-        if (f[i][3] == 'i') {
-          const long long v = strtoll(f[i].c_str() + 5, nullptr, 10);
-          if (v < 0) { body.push_back('i'); put32(body, (uint32_t)(int32_t)v); }
-          else if (v <= 0xff) { body.push_back('C'); body.push_back((uint8_t)v); }
-          else if (v <= 0xffff) { body.push_back('S'); put16(body, (uint32_t)v); }
-          else { body.push_back('I'); put32(body, (uint32_t)v); }
-        } else {
-          body.push_back('A');
-          body.push_back('?');
-        }
-      }
-      put32(recs, (uint32_t)body.size());
-      recs.insert(recs.end(), body.begin(), body.end());
-    }
-    put32(out, 0);  // l_text
-    put32(out, (uint32_t)header.names.size());
-    for (size_t i = 0; i < header.names.size(); ++i) {
-      put32(out, (uint32_t)header.names[i].size() + 1);
-      out.insert(out.end(), header.names[i].begin(), header.names[i].end());
-      out.push_back(0);
-      put32(out, (uint32_t)header.lens[i]);
-    }
-    out.insert(out.end(), recs.begin(), recs.end());
-    header = Header{};  // re-parsed from the BAM bytes by the caller
-  }
-};
-
 class DeviceSession {
  public:
   DeviceSession(int device, int threads, uint32_t batch_records = 1u << 20) : pool_(threads) {
@@ -307,17 +184,7 @@ class DeviceSession {
       if (s.kind == 1) throw Panic(s.message);
       if (s.kind == 2) throw ExitError(s.code, s.message);
     }
-    // cross-rank half of the sortedness check (contig.rs:129-132): each rank has verified its own (overlapping) stretch of
-    // the stream; the kept tids of the ranks' exclusive shares must not decrease from rank to rank either
-    {
-      int64_t seen_max = INT64_MIN;
-      for (const RankSummary& s : all) {
-        if (s.counts_global || s.min_tid > s.max_tid) continue;
-        if ((int64_t)s.min_tid < seen_max)
-          throw Panic("BAM file appears to be unsorted. Input BAM files must be sorted by reference (i.e. by samtools sort)");
-        seen_max = std::max<int64_t>(seen_max, s.max_tid);
-      }
-    }
+    check_rank_order(all);
     // ---- the gather of the path: every rank ends up with the complete per-contig table (+ histogram pairs)
     const uint32_t n_ref = (uint32_t)res.hdr->names.size();
     std::vector<uint64_t> pair_base((size_t)group_n_ + 1, 0);
@@ -333,23 +200,7 @@ class DeviceSession {
       gather_rows_through_host(sh, res, all, pair_base, csr);
     }
     res.rows = rows_buf_;
-    // whole-file counters: summed over the ranks' owned records -- or taken from a rank that had to read the whole file
-    uint64_t n_rec = 0, n_pri = 0;
-    bool have_global = false;
-    for (const RankSummary& s : all) {
-      if (s.counts_global) {
-        if (!have_global) {
-          n_rec = s.n_records;
-          n_pri = s.n_primary;
-          have_global = true;
-        }
-      } else if (!have_global) {
-        n_rec += s.n_records;
-        n_pri += s.n_primary;
-      }
-    }
-    res.n_records = n_rec;
-    res.num_detected_primary_alignments = n_pri;
+    fold_counters(all, res);
     res.timing.gather_s = now_s() - t_g0;
     res.timing.total_s += res.timing.gather_s;
     res.timing.group_ranks = (uint32_t)group_n_;
@@ -370,6 +221,31 @@ class DeviceSession {
     uint32_t counts_global, reserved;
     char message[208];
   };
+
+  // The cross-rank half of the sortedness check (contig.rs:129-132): each rank has verified its own (overlapping) stretch of
+  // the stream; the kept tids of the ranks' exclusive shares must not decrease from rank to rank either.
+  static void check_rank_order(const std::vector<RankSummary>& all) {
+    int64_t seen_max = INT64_MIN;
+    for (const RankSummary& s : all) {
+      if (s.counts_global || s.min_tid > s.max_tid) continue;
+      if ((int64_t)s.min_tid < seen_max)
+        throw Panic("BAM file appears to be unsorted. Input BAM files must be sorted by reference (i.e. by samtools sort)");
+      seen_max = std::max<int64_t>(seen_max, s.max_tid);
+    }
+  }
+  // The whole-file counters: taken from the first rank that had to read the whole file, else summed over the ranks' owned records.
+  static void fold_counters(const std::vector<RankSummary>& all, SampleResult& res) {
+    res.n_records = res.num_detected_primary_alignments = 0;
+    for (const RankSummary& s : all) {
+      if (s.counts_global) {
+        res.n_records = s.n_records;
+        res.num_detected_primary_alignments = s.n_primary;
+        return;
+      }
+      res.n_records += s.n_records;
+      res.num_detected_primary_alignments += s.n_primary;
+    }
+  }
 
   void group_allgather(const void* send, void* recv, size_t bytes) {
     if (group_nccl_) {
@@ -421,430 +297,388 @@ class DeviceSession {
     }
   }
 
-  SampleResult process_local(const InputSpec& in, const cmb_params& params, ShardState* shard) {
-    SampleResult res;
-    HostRange nvtx_sample("host: sample");
-    HostRange nvtx_header("host: open + BAM header");
-    const double t0 = now_s();
-    res.stoit_name = file_stem(in.path);
-    ByteSource bytes(in);
-    std::vector<uint8_t> sam_as_bam;
-    const uint8_t* p = bytes.data();
-    size_t n = bytes.size();
-    if (!(n >= 2 && p[0] == 0x1f && p[1] == 0x8b) && SamToBam::looks_like_sam(p, n)) {
-      SamToBam::convert(p, n, *res.hdr, sam_as_bam);
-      p = sam_as_bam.data();
-      n = sam_as_bam.size();
-    }
-    int rc;
+  // cmb_set_params; whether the parameters filter read pairs
+  bool set_params(const cmb_params& params) {
     cmb_filter_mode mode{};
-    rc = cmb_set_params(ctx_, &params, &mode);
+    const int rc = cmb_set_params(ctx_, &params, &mode);
     if (rc) throw_device_error(ctx_, rc);
-    const bool pair_mode = mode.filter_pairs;
-    // only the header is read through this stream, unless the host's mate-matching fallback below needs the records too
-    InflateStream stream(p, n, pool_, 1u << 20);
-    std::vector<uint8_t> buf;
-    size_t begin = 0;  // first unconsumed byte of buf
-    auto need = [&](size_t bytes_needed) {  // make buf[begin, begin+bytes_needed) available; false at EOF
-      while (buf.size() - begin < bytes_needed) {
-        if (begin) {
-          buf.erase(buf.begin(), buf.begin() + (ptrdiff_t)begin);
-          begin = 0;
-        }
-        if (!stream.fill(buf)) return false;
-      }
-      return true;
-    };
-    // ---- header (SAMv1 §4.2).  Samples mapped to the same reference carry byte-identical headers up to the first record:
-    //      the parsed copy of the previous sample is reused then (500 000 names are not rebuilt per sample).
-    uint64_t records_at = 0;
-    uint32_t n_ref = 0;
-    // Fastest case: the file starts with the very same COMPRESSED bytes as the previous sample's header did (the same file
-    // again, or samples written by one pipeline): nothing is inflated on the host at all.
-    bool hdr_fast = false;
-    if (hdr_cache_ && stream.is_bgzf() && !hdr_comp_.empty() && n >= hdr_comp_.size() && memcmp(p, hdr_comp_.data(), hdr_comp_.size()) == 0) {
-      hdr_fast = true;
-      res.hdr = hdr_cache_;
-      n_ref = (uint32_t)res.hdr->names.size();
-      records_at = hdr_records_at_;
-    } else {
-    if (!need(12) || memcmp(buf.data() + begin, "BAM\1", 4) != 0) throw Panic("Error reading BAM header: not a BAM/SAM file: " + in.path);
-    const uint32_t l_text = rd_u32(buf.data() + begin + 4);
-    if (!need(12 + (size_t)l_text)) throw Panic("Error reading BAM header: truncated");
-    const size_t refs_at = 8 + (size_t)l_text;  // the n_ref field; the @-lines before it (e.g. @PG) may differ between samples
-    if (hdr_cache_ && hdr_raw_.size() >= 4 && need(refs_at + hdr_raw_.size()) &&
-        memcmp(buf.data() + begin + refs_at, hdr_raw_.data(), hdr_raw_.size()) == 0) {
-      res.hdr = hdr_cache_;
-      n_ref = (uint32_t)res.hdr->names.size();
-      records_at = refs_at + hdr_raw_.size();
-    } else {
-      n_ref = rd_u32(buf.data() + begin + refs_at);
-      size_t o = refs_at + 4;
-      res.hdr->names.reserve(n_ref);
-      res.hdr->lens.reserve(n_ref);
-      for (uint32_t i = 0; i < n_ref; ++i) {
-        if (!need(o + 4)) throw Panic("Error reading BAM header: truncated");
-        const uint32_t l_name = rd_u32(buf.data() + begin + o);
-        if (!need(o + 8 + l_name)) throw Panic("Error reading BAM header: truncated");
-        res.hdr->names.emplace_back((const char*)buf.data() + begin + o + 4, l_name ? l_name - 1 : 0);
-        res.hdr->lens.push_back(rd_u32(buf.data() + begin + o + 4 + l_name));
-        o += 8 + l_name;
-      }
-      records_at = o;  // uncompressed offset of the first record (nothing has been discarded yet)
-      hdr_raw_.assign(buf.data() + begin + refs_at, buf.data() + begin + o);
-      hdr_cache_ = res.hdr;
-    }
-    hdr_comp_.clear();  // refreshed below, once the block index is known
-    begin += records_at;
-    }
-    res.timing.header_s = now_s() - t0;
-    nvtx_header.end();
+    return mode.filter_pairs;
+  }
 
-    // ---- device reference + params
-    uint32_t sb = std::min<uint32_t>(shard_begin_, n_ref), se = std::min<uint32_t>(shard_end_, n_ref);
-    if (shard) {
-      shard->cuts = tid_cuts_by_length(res.hdr->lens, group_n_);
-      sb = shard->cuts[(size_t)group_rank_];
-      se = shard->cuts[(size_t)group_rank_ + 1];
-    }
-    res.timing.tid_begin = sb;
-    res.timing.tid_end = se;
-    uint32_t n_rows = n_ref;
-    if (gene_defs_) {
-      if (shard) throw ExitError(1, "--gff is not available together with --gpus (per-gene coverage runs on one GPU)");
-      if (!gene_cache_ || res.hdr->lens != ref_lens_ || res.hdr->names != gene_cache_names_) {
-        gene_cache_ = std::make_shared<ResolvedGenes>(resolve_genes_against_header(*gene_defs_, *res.hdr, gene_namer_));
-        gene_cache_names_ = res.hdr->names;
-        std::vector<cmb_gene> genes(gene_cache_->entries.size());
-        for (size_t g = 0; g < genes.size(); ++g) genes[g] = cmb_gene{gene_cache_->entries[g].tid, gene_cache_->entries[g].start, gene_cache_->entries[g].end};
-        rc = cmb_set_genes(ctx_, n_ref, res.hdr->lens.data(), (uint32_t)genes.size(), genes.data());
-        if (rc) throw_device_error(ctx_, rc);
-        ref_lens_ = res.hdr->lens;
-      }
-      res.genes = gene_cache_;
-      n_rows = std::max<uint32_t>(1, (uint32_t)gene_cache_->entries.size());
-    } else if (res.hdr->lens != ref_lens_ || sb != ref_sb_ || se != ref_se_) {
-      ref_sb_ = sb;
-      ref_se_ = se;
-      rc = cmb_set_reference(ctx_, n_ref, res.hdr->lens.data(), sb, se);
-      if (rc) throw_device_error(ctx_, rc);
-      ref_lens_ = res.hdr->lens;
-    }
-    rc = cmb_begin_sample(ctx_);
-    if (rc) throw_device_error(ctx_, rc);
-
-    // ---- records
-    cmb_read_batch batch{};
-    bool have_batch = false;
-    uint32_t used_r = 0, used_i = 0;
-    double wait_s = 0;
-    auto acquire = [&]() {
-      const double a = now_s();
-      int r2 = cmb_acquire_batch(ctx_, &batch);
-      wait_s += now_s() - a;
-      if (r2) throw_device_error(ctx_, r2);
-      have_batch = true;
-      used_r = used_i = 0;
-    };
-    auto submit = [&]() {
-      if (!have_batch) return;
-      batch.iv_begin[used_r] = used_i;
-      const double a = now_s();
-      int r2 = cmb_submit_batch(ctx_, used_r, used_i);
-      wait_s += now_s() - a;
-      if (r2) throw_device_error(ctx_, r2);
-      have_batch = false;
-    };
-    std::vector<size_t> rec_off;
-    constexpr size_t ITEM = 4096;  // records per parallel work item
-    struct ItemOut {
-      std::vector<int32_t> iv_start, iv_len;
-      uint64_t primaries = 0;
-    };
-    std::vector<ItemOut> items;
-    std::vector<Tuple> tuples;  // pair mode only
-    // mate matching state (filter.rs:16-18)
-    struct Stored {
-      Tuple t;
-      std::vector<int32_t> iv_start, iv_len;
-    };
-    std::map<std::string, Stored> first_set;
-    int32_t current_reference = -1;
-
-    auto put_record = [&](const Tuple& t, const int32_t* ivs, const int32_t* ivl) {
-      const uint32_t i = used_r++;
-      batch.tid[i] = t.tid; batch.pos[i] = t.pos; batch.flag[i] = t.flag; batch.mapq[i] = t.mapq;
-      batch.nm_state[i] = t.nm_state; batch.nm[i] = t.nm; batch.l_seq[i] = t.l_seq; batch.aligned[i] = t.aligned;
-      batch.del[i] = t.del; batch.ins[i] = t.ins; batch.iv_begin[i] = used_i;
-      for (uint32_t k = 0; k < t.n_iv; ++k) {
-        batch.iv_start[used_i] = ivs[k];
-        batch.iv_len[used_i] = ivl[k];
-        ++used_i;
-      }
-    };
-
-    bool decoded_on_device = false;
+  SampleResult process_local(const InputSpec& in, const cmb_params& params, ShardState* shard) {
+    HostRange nvtx_sample("host: sample");
+    SampleCall c(*this, in, params, shard);
+    c.header();
+    c.reference();
     {
-      // region-parallel pipeline (decode_runner.hpp): this thread only acquires / submits staging batches
       HostRange nvtx_index("host: BGZF block index (+ range probes in a group)");
       const double t_index0 = now_s();
-      BlockIndex bx;
-      if (stream.is_raw()) bx.build(stream.raw_data(), stream.raw_size());
-      else bx.build(p, n);
+      const BlockIndex& bx = c.index(t_index0);
+      // Device-side decode first (compressed blocks cross PCIe, the GPU inflates and parses them); the host pipeline runs
+      // when the input is not BGZF, when CMB_HOST_DECODE is set, or when the device declines the stream.  Pair filtering
+      // included: the device matches mates itself (cmb_pairs.cuh); the host's map-based matching is the fallback.
+      if (bx.bgzf && !getenv("CMB_HOST_DECODE")) c.device_decode(bx, nvtx_index, t_index0);
+      if (!c.decoded_on_device && !c.pair_mode) c.host_pipeline(bx);
+    }
+    if (!c.decoded_on_device && c.pair_mode) c.pair_fallback();
+    return c.end_sample();
+  }
+
+  // One process_local call, handed from stage to stage.
+  struct SampleCall {
+    DeviceSession& s;
+    const InputSpec& in;
+    const cmb_params& params;
+    ShardState* shard;
+    HostRange nvtx_header{"host: open + BAM header"};
+    const double t0 = now_s();
+    SampleResult res;
+    BamInput input;
+    const bool pair_mode;
+    InflateStream stream;  // only the header is read through it, unless the host's mate matching needs the records too
+    std::vector<uint8_t> buf;
+    size_t begin = 0;      // first unconsumed byte of buf
+    bool hdr_fast = false, decoded_on_device = false;
+    uint64_t records_at = 0;
+    uint32_t n_ref = 0, n_rows = 0, sb = 0, se = 0;
+    double wait_s = 0;     // in cmb_acquire_batch / cmb_submit_batch
+
+    SampleCall(DeviceSession& session, const InputSpec& input_spec, const cmb_params& p, ShardState* sh)
+        : s(session), in(input_spec), params(p), shard(sh), input(in), pair_mode(s.set_params(params)),
+          stream(input.data(), input.size(), s.pool_, 1u << 20) {
+      res.stoit_name = file_stem(in.path);
+    }
+
+    void acquire(cmb_read_batch* b) {
+      const double a = now_s();
+      const int rc = cmb_acquire_batch(s.ctx_, b);
+      wait_s += now_s() - a;
+      if (rc) throw_device_error(s.ctx_, rc);
+    }
+    void submit(uint32_t n_records, uint32_t n_intervals) {
+      const double a = now_s();
+      const int rc = cmb_submit_batch(s.ctx_, n_records, n_intervals);
+      wait_s += now_s() - a;
+      if (rc) throw_device_error(s.ctx_, rc);
+    }
+
+    // Header (SAMv1 §4.2).  Samples mapped to the same reference carry byte-identical headers up to the first record: the
+    // parsed copy of the previous sample is reused then (500 000 names are not rebuilt per sample).
+    void header() {
+      // Fastest case: the file starts with the very same COMPRESSED bytes as the previous sample's header did (the same
+      // file again, or samples written by one pipeline): nothing is inflated on the host at all.
+      if (s.hdr_cache_ && stream.is_bgzf() && !s.hdr_comp_.empty() && input.size() >= s.hdr_comp_.size() &&
+          memcmp(input.data(), s.hdr_comp_.data(), s.hdr_comp_.size()) == 0) {
+        hdr_fast = true;
+        res.hdr = s.hdr_cache_;
+        records_at = s.hdr_records_at_;
+      } else {  // otherwise the raw reference list may still be the previous sample's, behind a different @-text
+        const BamHeader h = read_bam_header(stream, buf, in.path, s.hdr_raw_);
+        if (h.header) {
+          res.hdr = s.hdr_cache_ = h.header;
+          s.hdr_raw_.assign(buf.data() + h.refs_at, buf.data() + h.records_at);
+        } else {
+          res.hdr = s.hdr_cache_;
+        }
+        records_at = h.records_at;
+        begin = (size_t)records_at;
+        s.hdr_comp_.clear();  // refreshed by index(), once the block table is known
+      }
+      n_ref = (uint32_t)res.hdr->names.size();
+      res.timing.header_s = now_s() - t0;
+      nvtx_header.end();
+    }
+
+    // The device's reference (or genes) and the sample begun.
+    void reference() {
+      sb = std::min<uint32_t>(s.shard_begin_, n_ref);
+      se = std::min<uint32_t>(s.shard_end_, n_ref);
+      if (shard) {
+        shard->cuts = tid_cuts_by_length(res.hdr->lens, s.group_n_);
+        sb = shard->cuts[(size_t)s.group_rank_];
+        se = shard->cuts[(size_t)s.group_rank_ + 1];
+      }
+      res.timing.tid_begin = sb;
+      res.timing.tid_end = se;
+      n_rows = n_ref;
+      int rc;
+      if (s.gene_defs_) {
+        if (shard) throw ExitError(1, "--gff is not available together with --gpus (per-gene coverage runs on one GPU)");
+        if (!s.gene_cache_ || res.hdr->lens != s.ref_lens_ || res.hdr->names != s.gene_cache_names_) {
+          s.gene_cache_ = std::make_shared<ResolvedGenes>(resolve_genes_against_header(*s.gene_defs_, *res.hdr, s.gene_namer_));
+          s.gene_cache_names_ = res.hdr->names;
+          const auto& entries = s.gene_cache_->entries;
+          std::vector<cmb_gene> genes(entries.size());
+          for (size_t g = 0; g < genes.size(); ++g) genes[g] = cmb_gene{entries[g].tid, entries[g].start, entries[g].end};
+          rc = cmb_set_genes(s.ctx_, n_ref, res.hdr->lens.data(), (uint32_t)genes.size(), genes.data());
+          if (rc) throw_device_error(s.ctx_, rc);
+          s.ref_lens_ = res.hdr->lens;
+        }
+        res.genes = s.gene_cache_;
+        n_rows = std::max<uint32_t>(1, (uint32_t)s.gene_cache_->entries.size());
+      } else if (res.hdr->lens != s.ref_lens_ || sb != s.ref_sb_ || se != s.ref_se_) {
+        s.ref_sb_ = sb;
+        s.ref_se_ = se;
+        rc = cmb_set_reference(s.ctx_, n_ref, res.hdr->lens.data(), sb, se);
+        if (rc) throw_device_error(s.ctx_, rc);
+        s.ref_lens_ = res.hdr->lens;
+      }
+      rc = cmb_begin_sample(s.ctx_);
+      if (rc) throw_device_error(s.ctx_, rc);
+    }
+
+    // The whole block table.  htslib flushes the BGZF block after the header (bam_hdr_write), so the records usually start
+    // a block: then the compressed bytes in front of that block ARE the header, and the next sample that begins with the
+    // same bytes needs no header inflate at all.
+    const BlockIndex& index(double t_index0) {
+      const BlockIndex& bx = stream.index();
       res.timing.index_s = now_s() - t_index0;
-      if (!hdr_fast && bx.bgzf && !stream.is_raw()) {
-        // htslib flushes the BGZF block after the header (bam_hdr_write), so the records usually start a block: then the
-        // compressed bytes in front of that block ARE the header, and the next sample that begins with the same bytes needs no
-        // header inflate at all.
+      if (!hdr_fast && bx.bgzf) {
         const size_t b = (size_t)(std::lower_bound(bx.ustart.begin(), bx.ustart.end(), records_at) - bx.ustart.begin());
         if (b > 0 && b < bx.blocks.size() && bx.ustart[b] == records_at && bx.blocks[b].cdata >= 18) {
           const size_t start = bx.blocks[b].cdata - 18;
-          if (start <= (256u << 20) && p[start] == 0x1f && p[start + 1] == 0x8b) {
-            hdr_comp_.assign(p, p + start);
-            hdr_records_at_ = records_at;
+          if (start <= (256u << 20) && bx.p[start] == 0x1f && bx.p[start + 1] == 0x8b) {
+            s.hdr_comp_.assign(bx.p, bx.p + start);
+            s.hdr_records_at_ = records_at;
           }
         }
       }
-      // Device-side decode first (compressed blocks cross PCIe, the GPU inflates and parses them); the host pipeline
-      // below runs when the input is not BGZF, when CMB_HOST_DECODE is set, or when the device declines the stream.  Pair
-      // filtering included: the device matches mates itself (cmb_pairs.cuh); the host's BTreeMap-style matching further
-      // down is the fallback.
-      if (bx.bgzf && !stream.is_raw() && !getenv("CMB_HOST_DECODE")) {
-        const size_t nb = bx.blocks.size();
-        std::vector<uint64_t> coff(nb);
-        std::vector<uint32_t> clen(nb), isz(nb);
-        for (size_t b = 0; b < nb; ++b) {
-          coff[b] = bx.blocks[b].cdata;
-          clen[b] = (uint32_t)bx.blocks[b].clen;
-          isz[b] = bx.blocks[b].isize;
-        }
-        cmb_bgzf_input bi{};
-        bi.data = p;
-        bi.size = n;
-        bi.n_blocks = (uint32_t)nb;
-        bi.n_ref = n_ref;
-        bi.block_coffset = coff.data();
-        bi.block_clen = clen.data();
-        bi.block_isize = isz.data();
-        bi.records_at = records_at;
-        bi.copy_threads = (uint32_t)std::min(pool_.size(), 8);
-        bool range_ok = true;
-        if (shard) {  // this rank's block range (shard_range.hpp); a stream whose alignment cannot be confirmed is read whole
-          try {
-            BlockRangeFinder finder(bx, n_ref, records_at);
-            const bool last = group_rank_ == group_n_ - 1;
-            // reads cover the reference roughly evenly, so a tid's records start near its share of the summed contig length
-            double frac_lo = -1.0, frac_hi = -1.0;
-            {
-              long double before_lo = 0, before_hi = 0, total = 0;
-              const auto& lens = res.hdr->lens;
-              for (size_t t = 0; t < lens.size(); ++t) {
-                if (t == sb) before_lo = total;
-                if (t == se) before_hi = total;
-                total += (long double)lens[t];
-              }
-              if (se >= lens.size()) before_hi = total;
-              if (total > 0) {
-                frac_lo = (double)(before_lo / total);
-                frac_hi = (double)(before_hi / total);
-              }
-            }
-            const BlockRange br = finder.find(sb, se, group_rank_ == 0, last, frac_lo, frac_hi);
-            bi.ranged = 1;
-            bi.walk_begin_block = br.walk_begin;
-            bi.walk_end_block = br.walk_end;
-            bi.records_at = br.records_at;
-            bi.excl_end_block = br.excl_end;
-            bi.own_tid_begin = (int32_t)sb;
-            bi.own_tid_end = (int32_t)se;
-            bi.own_unplaced = last ? 1u : 0u;
-            res.timing.shard_blocks = br.walk_end - br.walk_begin;
-            res.timing.total_blocks = (uint32_t)nb;
-            res.timing.range_probes = br.probes;
-          } catch (const Panic&) {
-            range_ok = false;
-          }
-        }
-        cmb_bgzf_result br{};
-        nvtx_index.end();
-        const double a = now_s();
-        res.timing.index_s = now_s() - t_index0;  // incl. the block table and, in a group, the range probes
-        const int r2 = range_ok ? cmb_submit_bgzf(ctx_, &bi, &br) : CMB_E_DECLINED;
-        res.timing.device_call_s = now_s() - a;
-        if (r2 == CMB_OK) {
-          decoded_on_device = true;
-          res.timing.device_decode = true;
-          res.timing.bgzf = br;
-          res.timing.h2d_bytes = br.h2d_bytes;
-          res.timing.decode_launches = br.n_launches;
-          res.n_records = br.n_records;
-          res.num_detected_primary_alignments = br.n_primary;
-          if (getenv("CMB_PIPELINE_STATS"))
-            fprintf(stderr, "#device_decode\tblocks=%zu\thost_blocks=%u\trepairs=%u\tcopy_inflate_ms=%.2f\tchain_ms=%.2f\textract_ms=%.2f\ttotal_ms=%.2f\tcall_s=%.4f\n",
-                    nb, br.n_blocks_host, br.chain_repairs, br.ms_copy_inflate, br.ms_chain, br.ms_extract, br.ms_total, now_s() - a);
-        } else if (r2 != CMB_E_DECLINED) {
-          throw_device_error(ctx_, r2);
-        } else if (getenv("CMB_PIPELINE_STATS")) {
-          fprintf(stderr, "#device_decode\tdeclined: %s\n", cmb_last_error(ctx_));
-        }
+      return bx;
+    }
+
+    // cmb_submit_bgzf over the sample's blocks (in a group, over this rank's block range).
+    void device_decode(const BlockIndex& bx, HostRange& nvtx_index, double t_index0) {
+      BgzfInput bi(bx, n_ref, records_at, s.pool_.size());
+      const bool range_ok = !shard || rank_block_range(bx, bi.in);
+      cmb_bgzf_result br{};
+      nvtx_index.end();
+      const double a = now_s();
+      res.timing.index_s = a - t_index0;  // incl. the block table and, in a group, the range probes
+      const int rc = range_ok ? cmb_submit_bgzf(s.ctx_, &bi.in, &br) : CMB_E_DECLINED;
+      res.timing.device_call_s = now_s() - a;
+      if (rc == CMB_OK) {
+        decoded_on_device = true;
+        res.timing.device_decode = true;
+        res.timing.bgzf = br;
+        res.timing.h2d_bytes = br.h2d_bytes;
+        res.timing.decode_launches = br.n_launches;
+        res.n_records = br.n_records;
+        res.num_detected_primary_alignments = br.n_primary;
+        if (getenv("CMB_PIPELINE_STATS"))
+          fprintf(stderr, "#device_decode\tblocks=%zu\thost_blocks=%u\trepairs=%u\tcopy_inflate_ms=%.2f\tchain_ms=%.2f\textract_ms=%.2f\ttotal_ms=%.2f\tcall_s=%.4f\n",
+                  bx.blocks.size(), br.n_blocks_host, br.chain_repairs, br.ms_copy_inflate, br.ms_chain, br.ms_extract, br.ms_total, now_s() - a);
+      } else if (rc != CMB_E_DECLINED) {
+        throw_device_error(s.ctx_, rc);
+      } else if (getenv("CMB_PIPELINE_STATS")) {
+        fprintf(stderr, "#device_decode\tdeclined: %s\n", cmb_last_error(s.ctx_));
       }
-      if (!decoded_on_device && !pair_mode) {
+    }
+
+    // This rank's block range (shard_range.hpp), into `bi`; false when the stream's alignment cannot be confirmed (the
+    // rank then reads the stream whole).
+    bool rank_block_range(const BlockIndex& bx, cmb_bgzf_input& bi) {
+      try {
+        BlockRangeFinder finder(bx, n_ref, records_at);
+        const bool last = s.group_rank_ == s.group_n_ - 1;
+        // reads cover the reference roughly evenly, so a tid's records start near its share of the summed contig length
+        double frac_lo = -1.0, frac_hi = -1.0;
+        long double before_lo = 0, before_hi = 0, total = 0;
+        const auto& lens = res.hdr->lens;
+        for (size_t t = 0; t < lens.size(); ++t) {
+          if (t == sb) before_lo = total;
+          if (t == se) before_hi = total;
+          total += (long double)lens[t];
+        }
+        if (se >= lens.size()) before_hi = total;
+        if (total > 0) {
+          frac_lo = (double)(before_lo / total);
+          frac_hi = (double)(before_hi / total);
+        }
+        const BlockRange br = finder.find(sb, se, s.group_rank_ == 0, last, frac_lo, frac_hi);
+        bi.ranged = 1;
+        bi.walk_begin_block = br.walk_begin;
+        bi.walk_end_block = br.walk_end;
+        bi.records_at = br.records_at;
+        bi.excl_end_block = br.excl_end;
+        bi.own_tid_begin = (int32_t)sb;
+        bi.own_tid_end = (int32_t)se;
+        bi.own_unplaced = last ? 1u : 0u;
+        res.timing.shard_blocks = br.walk_end - br.walk_begin;
+        res.timing.total_blocks = (uint32_t)bx.blocks.size();
+        res.timing.range_probes = br.probes;
+        return true;
+      } catch (const Panic&) {
+        return false;
+      }
+    }
+
+    // The region-parallel host decode (decode_runner.hpp): this thread only acquires / submits staging batches.
+    void host_pipeline(const BlockIndex& bx) {
       if (shard) shard->counts_global = true;  // every rank's host decoder reads the whole file; K1 keeps the rank's own tids
       const PipelineCounts pc = run_decode_pipeline(
-          bx, records_at, n_ref, pool_.size(), batch_records_, batch_intervals_, n_staging_, scratch_,
-          [&](cmb_read_batch* b) {
-            const double a = now_s();
-            int r2 = cmb_acquire_batch(ctx_, b);
-            wait_s += now_s() - a;
-            if (r2) throw_device_error(ctx_, r2);
-          },
-          [&](uint32_t nr, uint32_t ni) {
-            const double a = now_s();
-            int r2 = cmb_submit_batch(ctx_, nr, ni);
-            wait_s += now_s() - a;
-            if (r2) throw_device_error(ctx_, r2);
-          });
+          bx, records_at, n_ref, s.pool_.size(), s.batch_records_, s.batch_intervals_, s.n_staging_, s.scratch_,
+          [&](cmb_read_batch* b) { acquire(b); }, [&](uint32_t nr, uint32_t ni) { submit(nr, ni); });
       res.n_records = pc.n_records;
       res.num_detected_primary_alignments = pc.primaries;
       if (getenv("CMB_PIPELINE_STATS"))
         fprintf(stderr, "#pipeline\titems=%u\tworkers=%u\tinflate_s=%.3f\tchain_s=%.3f\textract_s=%.3f\tidle_s=%.3f (summed over workers)\n",
                 pc.n_items, pc.n_workers, pc.inflate_s, pc.scan_s, pc.extract_s, pc.idle_s);
-      }
     }
-    if (pair_mode && !decoded_on_device && hdr_fast) {  // the header was recognised without inflating it: skip over it now
-      if (!need((size_t)records_at)) throw Panic("Error reading BAM header: truncated");
-      begin = (size_t)records_at;
-    }
-    if (pair_mode && !decoded_on_device) stream.set_window(48u << 20);  // mate matching is sequential: decode window by window
-    if (pair_mode && !decoded_on_device) for (;;) {
-      if (shard) shard->counts_global = true;  // mate matching reads the whole file on every rank
-      // complete records currently in buf
-      rec_off.clear();
-      size_t q = begin;
-      size_t max_iv = 0;
-      while (q + 4 <= buf.size()) {
-        const uint32_t bs = rd_u32(buf.data() + q);
-        if (bs < 32) throw Panic("Error reading BAM record: corrupt block_size");
-        if (q + 4 + (size_t)bs > buf.size()) break;
-        rec_off.push_back(q);
-        const int64_t ops = record_cigar_ops(buf.data() + q);
-        if (ops < 0) throw_bad_record_layout();
-        max_iv += (size_t)ops;
-        q += 4 + (size_t)bs;
-        if (rec_off.size() == batch_records_ / 2) break;  // keep one window within a batch
-      }
-      if (rec_off.empty()) {
-        if (!need((buf.size() - begin) + 1)) break;  // EOF
-        continue;
-      }
-      const size_t nrec = rec_off.size();
-      res.n_records += nrec;
-      const size_t n_items = (nrec + ITEM - 1) / ITEM;
-      if (items.size() < n_items) items.resize(n_items);
-      if (max_iv > batch_intervals_) throw ExitError(1, "a window of records has more aligned blocks than a device batch holds");
 
-      {
-        // filter.rs:117-233: decode in parallel, then match mates in stream order; only completed pairs reach the GPU
+    // Pair filtering when the device did not decode the stream (filter.rs:117-233): windows of records are decoded in
+    // parallel, then mates are matched in stream order; only completed pairs reach the GPU, the first mate at the even index.
+    void pair_fallback() {
+      if (shard) shard->counts_global = true;  // mate matching reads the whole file on every rank
+      if (hdr_fast) {  // the header was recognised without inflating it: skip over it now
+        while (buf.size() < records_at)
+          if (!stream.fill(buf)) throw Panic("Error reading BAM header: truncated");
+        begin = (size_t)records_at;
+      }
+      stream.set_window(48u << 20);  // mate matching is sequential: decode window by window
+      struct Stored {
+        Tuple t;
+        std::vector<int32_t> iv_start, iv_len;
+      };
+      HostMates<Stored> mates;
+      constexpr size_t ITEM = 4096;  // records per parallel work item
+      struct ItemOut {
+        std::vector<int32_t> iv_start, iv_len;
+      };
+      std::vector<ItemOut> items;
+      std::vector<size_t> rec_off;
+      std::vector<Tuple> tuples;
+      std::vector<uint32_t> iv_at;
+      cmb_read_batch batch{};
+      bool have_batch = false;
+      uint32_t used_r = 0, used_i = 0;
+      auto put = [&](const Tuple& t, const int32_t* ivs, const int32_t* ivl) {
+        put_tuple(batch, used_r++, used_i, t, ivs, ivl);
+        used_i += t.n_iv;
+      };
+      auto flush = [&]() {
+        if (!have_batch) return;
+        batch.iv_begin[used_r] = used_i;
+        submit(used_r, used_i);
+        have_batch = false;
+      };
+      for (;;) {
+        // the complete records currently in buf (one window within a batch)
+        rec_off.clear();
+        size_t max_iv = 0;
+        const size_t q = walk_records(buf.data(), begin, buf.size(), false, [&](size_t o) {
+          const int64_t ops = record_cigar_ops(buf.data() + o);
+          if (ops < 0) throw_bad_record_layout();
+          rec_off.push_back(o);
+          max_iv += (size_t)ops;
+          return rec_off.size() < s.batch_records_ / 2;
+        });
+        if (rec_off.empty()) {
+          buf.erase(buf.begin(), buf.begin() + (ptrdiff_t)begin);
+          begin = 0;
+          if (stream.fill(buf)) continue;
+          if (!buf.empty()) throw Panic("Error reading BAM record: truncated");  // as walk_records' at_eof
+          break;
+        }
+        const size_t nrec = rec_off.size();
+        res.n_records += nrec;
+        const size_t n_items = (nrec + ITEM - 1) / ITEM;
+        if (items.size() < n_items) items.resize(n_items);
+        if (max_iv > s.batch_intervals_) throw ExitError(1, "a window of records has more aligned blocks than a device batch holds");
         tuples.resize(nrec);
-        std::vector<uint32_t> iv_at(nrec);
+        iv_at.resize(nrec);
         const uint8_t* base = buf.data();
-        pool_.parallel_for(n_items, [&](size_t it, int) {
+        s.pool_.parallel_for(n_items, [&](size_t it, int) {
           ItemOut& io = items[it];
           io.iv_start.clear();
           io.iv_len.clear();
-          const size_t r0 = it * ITEM, r1 = std::min(nrec, r0 + ITEM);
-          for (size_t r = r0; r < r1; ++r) {
+          for (size_t r = it * ITEM; r < std::min(nrec, (it + 1) * ITEM); ++r) {
             iv_at[r] = (uint32_t)io.iv_start.size();
             decode_bam_record(base + rec_off[r], tuples[r], io.iv_start, io.iv_len);
           }
         });
         for (size_t r = 0; r < nrec; ++r) {
           const Tuple& t = tuples[r];
+          if (t.flag & 0x900) continue;  // secondary / supplementary (filter.rs:138-140)
+          res.num_detected_primary_alignments += 1;
+          if (!(t.flag & 0x2)) continue;  // not a proper pair (filter.rs:141-147, filter_out = true)
           const ItemOut& io = items[r / ITEM];
           const int32_t* ivs = io.iv_start.data() + iv_at[r];
           const int32_t* ivl = io.iv_len.data() + iv_at[r];
-          if (!(t.flag & 0x900)) res.num_detected_primary_alignments += 1;
-          if (t.flag & 0x900) continue;   // secondary / supplementary (filter.rs:138-140)
-          if (!(t.flag & 0x2)) continue;  // not a proper pair (filter.rs:141-147, filter_out = true)
-          if (t.tid != current_reference) {
-            current_reference = t.tid;
-            first_set.clear();
+          const std::optional<Stored> first = mates.match(t, bam_qname(base + rec_off[r]), [&] {
+            return Stored{t, std::vector<int32_t>(ivs, ivs + t.n_iv), std::vector<int32_t>(ivl, ivl + t.n_iv)};
+          });
+          if (!first) continue;
+          if (have_batch && (used_r + 2 > s.batch_records_ || used_i + first->t.n_iv + t.n_iv > s.batch_intervals_)) flush();
+          if (!have_batch) {
+            acquire(&batch);
+            have_batch = true;
+            used_r = used_i = 0;
           }
-          std::string qname = bam_qname(base + rec_off[r]);
-          auto itf = first_set.find(qname);
-          if (itf == first_set.end()) {
-            if (t.mtid == current_reference) {
-              Stored s;
-              s.t = t;
-              s.iv_start.assign(ivs, ivs + t.n_iv);
-              s.iv_len.assign(ivl, ivl + t.n_iv);
-              first_set.emplace(std::move(qname), std::move(s));
-            }
-          } else {
-            const Stored& s = itf->second;
-            if (have_batch && (used_r + 2 > batch_records_ || used_i + s.t.n_iv + t.n_iv > batch_intervals_)) submit();
-            if (!have_batch) acquire();
-            put_record(s.t, s.iv_start.data(), s.iv_len.data());  // stored first mate at the even index
-            put_record(t, ivs, ivl);
-            first_set.erase(itf);
-          }
+          put(first->t, first->iv_start.data(), first->iv_len.data());
+          put(t, ivs, ivl);
         }
+        begin = q;
       }
-      begin = q;
+      flush();
     }
-    const double t_dec = now_s();
-    submit();
-    ensure_rows(n_rows);
-    res.rows = rows_buf_;
-    uint64_t n_pairs = 0;
-    // A histogram buffer of the device overflowed (very deep coverage over many small contigs): with the sample's tuples still in
-    // device memory the buffers are enlarged and the kernels run again; otherwise the error stands.
-    auto end_sample = [&](cmb_contig_stats* rows_out) {
-      int r2 = cmb_end_sample(ctx_, rows_out, nullptr, 0, &n_pairs);
-      for (int attempt = 0; r2 == CMB_E_CAPACITY && decoded_on_device && attempt < 8; ++attempt) {
+
+    // cmb_end_sample.  A histogram buffer of the device overflowed (very deep coverage over many small contigs): with the
+    // sample's tuples still in device memory the buffers are enlarged and the kernels run again; otherwise the error stands.
+    int end_device_sample(cmb_contig_stats* rows_out, uint64_t& n_pairs) {
+      int rc = cmb_end_sample(s.ctx_, rows_out, nullptr, 0, &n_pairs);
+      for (int attempt = 0; rc == CMB_E_CAPACITY && decoded_on_device && attempt < 8; ++attempt) {
         cmb_read_batch again{};
         uint32_t nr = 0, ni = 0;
-        if (cmb_last_bgzf_batch(ctx_, &again, &nr, &ni) != CMB_OK) break;
+        if (cmb_last_bgzf_batch(s.ctx_, &again, &nr, &ni) != CMB_OK) break;
         if (getenv("CMB_PIPELINE_STATS")) fprintf(stderr, "#capacity_retry\tattempt=%d\n", attempt + 1);
-        if ((r2 = cmb_grow_buffers(ctx_)) != CMB_OK) break;
-        if ((r2 = cmb_begin_sample(ctx_)) != CMB_OK) break;
-        if ((r2 = cmb_submit_device_batch(ctx_, &again, nr, ni)) != CMB_OK) break;
-        r2 = cmb_end_sample(ctx_, rows_out, nullptr, 0, &n_pairs);
+        if ((rc = cmb_grow_buffers(s.ctx_)) != CMB_OK) break;
+        if ((rc = cmb_begin_sample(s.ctx_)) != CMB_OK) break;
+        if ((rc = cmb_submit_device_batch(s.ctx_, &again, nr, ni)) != CMB_OK) break;
+        rc = cmb_end_sample(s.ctx_, rows_out, nullptr, 0, &n_pairs);
       }
-      return r2;
-    };
-    if (shard && group_nccl_) {
-      // rows (and pairs) stay on the device: cmb_allgather_stats completes the table there and copies it back once
-      rc = end_sample(nullptr);
-      if (rc) throw_device_error(ctx_, rc);
-      shard->n_pairs = n_pairs;
-    } else {
-      rc = end_sample(rows_buf_);
-      if (rc) throw_device_error(ctx_, rc);
-      if ((params.want & CMB_WANT_HIST_CSR) && n_pairs) {
-        res.pairs.resize(n_pairs);
-        rc = cmb_fetch_pairs(ctx_, res.pairs.data(), n_pairs);
-        if (rc) throw_device_error(ctx_, rc);
-      }
-      if (shard) {
+      return rc;
+    }
+
+    // The device's per-contig table (and histogram pairs), the gene extras, and the sample's timing.
+    SampleResult end_sample() {
+      const double t_dec = now_s();
+      s.ensure_rows(n_rows);
+      res.rows = s.rows_buf_;
+      uint64_t n_pairs = 0;
+      int rc;
+      if (shard && s.group_nccl_) {
+        // rows (and pairs) stay on the device: cmb_allgather_stats completes the table there and copies it back once
+        rc = end_device_sample(nullptr, n_pairs);
+        if (rc) throw_device_error(s.ctx_, rc);
         shard->n_pairs = n_pairs;
-        local_pairs_ = res.pairs;
+      } else {
+        rc = end_device_sample(s.rows_buf_, n_pairs);
+        if (rc) throw_device_error(s.ctx_, rc);
+        if ((params.want & CMB_WANT_HIST_CSR) && n_pairs) {
+          res.pairs.resize(n_pairs);
+          rc = cmb_fetch_pairs(s.ctx_, res.pairs.data(), n_pairs);
+          if (rc) throw_device_error(s.ctx_, rc);
+        }
+        if (shard) {
+          shard->n_pairs = n_pairs;
+          s.local_pairs_ = res.pairs;
+        }
       }
+      if (s.gene_defs_) {
+        res.contig_seen.assign((size_t)n_ref + 1, 0);
+        rc = cmb_fetch_gene_extras(s.ctx_, res.contig_seen.data(), &res.kept_primary);
+        if (rc) throw_device_error(s.ctx_, rc);
+      }
+      cmb_get_timing(s.ctx_, &res.timing.device);
+      if (!res.timing.device_decode) res.timing.h2d_bytes = 40ull * res.timing.device.n_records + 4 + 8ull * res.timing.device.n_intervals;
+      const double t1 = now_s();
+      res.timing.total_s = t1 - t0;
+      res.timing.decode_s = t_dec - t0 - wait_s;
+      res.timing.submit_wait_s = wait_s;
+      res.timing.end_sample_s = t1 - t_dec;
+      return std::move(res);
     }
-    if (gene_defs_) {
-      res.contig_seen.assign((size_t)n_ref + 1, 0);
-      rc = cmb_fetch_gene_extras(ctx_, res.contig_seen.data(), &res.kept_primary);
-      if (rc) throw_device_error(ctx_, rc);
-    }
-    cmb_get_timing(ctx_, &res.timing.device);
-    if (!res.timing.device_decode) res.timing.h2d_bytes = 40ull * res.timing.device.n_records + 4 + 8ull * res.timing.device.n_intervals;
-    const double t1 = now_s();
-    res.timing.total_s = t1 - t0;
-    res.timing.decode_s = t_dec - t0 - wait_s;
-    res.timing.submit_wait_s = wait_s;
-    res.timing.end_sample_s = t1 - t_dec;
-    return res;
-  }
+  };
 
   std::shared_ptr<Header> hdr_cache_;  // parsed reference list of the previous sample and its raw bytes (n_ref .. first record)
   std::vector<uint8_t> hdr_raw_;

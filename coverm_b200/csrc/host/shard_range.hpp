@@ -15,7 +15,7 @@
 #include <utility>
 #include <vector>
 
-#include "decode_pipeline.hpp"
+#include "bam_source.hpp"
 
 namespace cmbh {
 

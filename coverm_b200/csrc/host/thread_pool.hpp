@@ -3,9 +3,11 @@
 #include <atomic>
 #include <condition_variable>
 #include <cstdint>
+#include <exception>
 #include <functional>
 #include <mutex>
 #include <thread>
+#include <utility>
 #include <vector>
 
 namespace cmbh {
@@ -27,6 +29,7 @@ class ThreadPool {
   int size() const { return n_; }
 
   // Runs fn(index, thread_id) for index in [0, n_items); dynamic scheduling; the caller participates as thread 0.
+  // The first exception fn throws is rethrown here, once every thread is done (the items not started yet are skipped).
   void parallel_for(size_t n_items, const std::function<void(size_t, int)>& fn) {
     if (n_items == 0) return;
     if (n_ == 1 || n_items == 1) {
@@ -46,6 +49,7 @@ class ThreadPool {
     std::unique_lock<std::mutex> lk(mu_);
     done_cv_.wait(lk, [this] { return pending_ == 0; });
     fn_ = nullptr;
+    if (error_) std::rethrow_exception(std::exchange(error_, nullptr));
   }
 
  private:
@@ -53,7 +57,13 @@ class ThreadPool {
     for (;;) {
       size_t i = next_.fetch_add(1);
       if (i >= n_items_) break;
-      (*fn_)(i, tid);
+      try {
+        (*fn_)(i, tid);
+      } catch (...) {
+        std::lock_guard<std::mutex> lk(mu_);
+        if (!error_) error_ = std::current_exception();
+        next_.store(n_items_);
+      }
     }
   }
   void worker(int tid) {
@@ -82,6 +92,7 @@ class ThreadPool {
   int pending_ = 0;
   uint64_t generation_ = 0;
   bool stop_ = false;
+  std::exception_ptr error_;
 };
 
 }  // namespace cmbh
