@@ -2,7 +2,7 @@
 #pragma once
 
 
-constexpr uint32_t SPAN = 32;                   // elements per K2 thread span = one 128-B tile row; contig alignment
+constexpr uint32_t SPAN = 32;                   // elements per span = one 128-B tile row; contig alignment
 constexpr uint32_t K2_THREADS = 256;
 constexpr uint32_t CHUNK = SPAN * K2_THREADS;   // 8192 elements = 32 KB
 constexpr uint32_t CHUNK_BYTES = CHUNK * 4;
@@ -13,8 +13,8 @@ constexpr uint32_t CHUNK_ROWS = CHUNK / ROW_ELEMS;  // 256
 #define CMB_K2_STAGES 2
 #endif
 constexpr uint32_t K2_STAGES = CMB_K2_STAGES;
-constexpr uint32_t K2_WARPS = K2_THREADS / 32;  // 8 = span-bitmap words per chunk
-// Span occupancy bitmap: one bit per span (K1 sets it for every event it adds), so one u32 word per warp of K2 spans.
+constexpr uint32_t K2_WARPS = K2_THREADS / 32;  // 8 = span-bitmap words per chunk = K2 warps per CTA
+// Span occupancy bitmap: one bit per span (K1 sets it for every event it adds), 8 u32 words per chunk.
 constexpr uint32_t BITMAP_SPANS_PER_WORD = 32;
 constexpr uint32_t BITMAP_ELEMS_PER_WORD = BITMAP_SPANS_PER_WORD * SPAN;  // 1024
 #ifndef CMB_K2_MINBLOCKS

@@ -22,10 +22,11 @@
 //                             +1/-1 delta REDs into the arena (contig.rs:166-202), chunk tail sums.
 //   K1b k1b_local/apply       segmented scan of the per-chunk tail sums -> carry_in (so K2 needs no look-back), and the
 //                             exclusive scan of the contigs' bin counts -> bin_base, in the same two launches.
-//   K2  k2_scan_reduce        persistent CTAs, ring of 32 KB chunks: whole-tile TMA (cp.async.bulk.tensor, 128B swizzle)
-//                             + mbarrier for chunks with many non-empty spans, cp.async of just the non-empty 128-B rows
-//                             for the others; blocked 32-element spans per thread, warp-shuffle segmented scan, then every
-//                             O(L) reduction of EST:366-502 in one pass: sum/covered over the end-trimmed window,
+//   K2  k2_scan_reduce        persistent warps, a warp per chunk, work only for the spans that hold events (slots, 32 per
+//                             round): 32-row TMA boxes (cp.async.bulk.tensor, 128B swizzle) + mbarrier for chunks with many
+//                             non-empty spans, cp.async of just the non-empty 128-B rows for the others; warp-shuffle
+//                             segmented scan of the slot totals, the event-free stretches between slots closed as one run
+//                             each, then every O(L) reduction of EST:366-502 in one pass: sum/covered over the end-trimmed window,
 //                             covered over the full contig, window depth histogram as REDs into the contig's bins;
 //                             optionally re-zeroes the arena as it goes.
 //   K3  k3_finalize           per contig: walk its bins, trimmed-mean walk (EST:598-642) and the variance sums
@@ -419,9 +420,11 @@ template <bool HIST, bool CLEAN>
 int launch_k2_variant(cmb_ctx* c, const K2Args& a) {
   int occ = 0;
   if (int rc = k2_blocks_per_sm<HIST, CLEAN>(c, &occ)) return rc;
-  const uint32_t grid = std::min<uint32_t>(c->n_chunks, (uint32_t)(occ * c->sm_count));
+  // a warp per chunk: no more CTAs than it takes to give every chunk its own warp
+  const uint32_t grid = std::min<uint32_t>((c->n_chunks + K2_WARPS - 1) / K2_WARPS, (uint32_t)(occ * c->sm_count));
   if (getenv("CMB_PIPELINE_STATS"))
-    fprintf(stderr, "#k2_grid\tgrid=%u\tblocks_per_sm=%d\tsms=%d\thist=%d\tclean=%d\n", grid, occ, c->sm_count, (int)HIST, (int)CLEAN);
+    fprintf(stderr, "#k2_grid\tgrid=%u\tblocks_per_sm=%d\tsms=%d\thist=%d\tclean=%d\twarps=%u\n", grid, occ, c->sm_count, (int)HIST,
+            (int)CLEAN, grid * K2_WARPS);
   k2_scan_reduce<HIST, CLEAN><<<grid, K2_THREADS, K2_SMEM_BYTES, c->stream>>>(c->tmap, a);
   CU_TRY(c, cudaGetLastError());
   return CMB_OK;
@@ -753,14 +756,14 @@ int cmb_set_reference(cmb_ctx* c, uint32_t n_contigs, const uint64_t* contig_len
   if (small_hist() && (rc = ensure_pool(c, 64, 64))) return rc;  // testing aid: a pool that overflows at once
   c->pool_dirty = false;
   c->arena_dirty = true;
-  // TMA descriptor: the arena as [rows][32] i32, box = one chunk (256 rows x 128 B), 128B swizzle
+  // TMA descriptor: the arena as [rows][32] i32, box = one K2 round (32 rows x 128 B = four 1024-B swizzle atoms), 128B swizzle
   PFN_encodeTiled encode = nullptr;
   cudaDriverEntryPointQueryResult qres;
   CU_TRY(c, cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", (void**)&encode, cudaEnableDefault, &qres));
   if (!encode || qres != cudaDriverEntryPointSuccess) return fail(c, CMB_E_CUDA, "cuTensorMapEncodeTiled not available in this driver");
   cuuint64_t gdim[2] = {ROW_ELEMS, c->arena_elems / ROW_ELEMS};
   cuuint64_t gstride[1] = {ROW_ELEMS * 4};
-  cuuint32_t box[2] = {ROW_ELEMS, CHUNK_ROWS};
+  cuuint32_t box[2] = {ROW_ELEMS, K2_BOX_ROWS};
   cuuint32_t estr[2] = {1, 1};
   CUresult res = encode(&c->tmap, CU_TENSOR_MAP_DATA_TYPE_INT32, 2, r.d_arena.p, gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                         CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);

@@ -1,21 +1,29 @@
-// K2: segmented prefix sum of the delta arena + every O(L) reduction of EST::add_contig, one pass, HBM-bound.
+// K2: segmented prefix sum of the delta arena + every O(L) reduction of EST::add_contig, one pass over the spans that hold
+// events.
 //
-// Persistent CTAs (2 or 3 per SM, 256 threads).  Iteration i of CTA b works on the 8192-element chunk b + i * gridDim.x and
-// keeps a ring of K2_STAGES 32 KB tiles in flight.  Which of a chunk's 256 spans hold any event is known from the span
-// occupancy bitmap K1 sets (8 words per chunk): a chunk with at least K2_DENSE_SPANS such spans is fetched whole with TMA
-// (cp.async.bulk.tensor.2d, 128B swizzle, mbarrier complete_tx); in any other chunk each warp copies only its non-empty
-// 128-byte rows with cp.async into the same swizzled tile positions, and the spans it does not fetch are zero by
-// construction.  A thread owns one 32-element span (8 x LDS.128, conflict-free through the swizzle); contigs start on span
-// boundaries, so a span never straddles two contigs.  Running depth at a span = chunk carry (K1b) + segmented warp/CTA scan
-// of the span totals.  Depth is piecewise constant and deltas are sparse (~1-2 % of positions), so a thread only keeps the
-// span total and a 32-bit mask of its non-zero positions; covered bases, sum of depth and the depth histogram of the
-// end-trimmed window are then accumulated per RUN in a short loop over the set bits (the deltas are re-read from the
-// shared-memory tile, which stays resident until the next iteration's barrier).  The window depth histogram is a dense
+// Persistent warps: warp g of W (8 per CTA) reduces the 8192-element chunks g, g + W, g + 2W, ...  Which of a chunk's 256
+// spans hold any event is known from the span occupancy bitmap K1 sets (8 words per chunk).  Depth is piecewise constant
+// between events, so only those spans need work: a chunk's SLOTS are its occupied spans in order (all 256 spans when it has
+// at least K2_DENSE_SPANS occupied ones), and slot j covers the positions from its span up to the next slot's span, the
+// chunk's end for the last one (cmb_k2_slots.cuh).  The event-free stretch after a slot's last event has that event's depth,
+// so it is closed as one run; positions past the slot's contig's end are padding or contigs without events so far (depth 0).
+// The stretch before the first slot has the chunk's carry-in (K1b) as its depth in the chunk's first contig.
+//
+// Slots go 32 per round, one per lane.  A lane finds its slot's span from the bitmap words (arithmetic only), its contig by
+// bisection, and reads the span's 32 deltas (8 x LDS.128 through the 128-B swizzle), keeping their sum and the mask of
+// non-zero positions.  The depth entering a slot is a segmented (by contig) warp scan of the slot totals, seeded with the
+// previous round's last slot (the chunk's first contig at its carry-in for round 0); no CTA barrier is involved.  Covered
+// bases, sum of depth and the depth histogram of the end-trimmed window are accumulated per run.  The histogram is a dense
 // array of u32 counts per contig in global memory, bins[bin_base[c] + depth] (K1b laid it out: every window depth of c is at
 // most its read count), so a run's count is one fire-and-forget RED; K3 reads the bins in depth order and re-zeroes them.
-// Depth 0 is not added: K3 derives its count from the window length and covered_window.  At config 2's coverage about half
-// of the runs are at depth 0, all of them on one address per contig.
+// Depth 0 is not added: K3 derives its count from the window length and covered_window.
+//
+// Loads: each warp has a ring of K2_STAGES buffers of 32 rows x 128 B laid out as a TMA box with the 128-B swizzle writes
+// them.  A dense chunk's rounds are one 32-row TMA box each (completion on the stage's mbarrier); a sparse round copies its
+// occupied rows with cp.async into rows 0..n-1, four whole 128-B lines per instruction.  The next round's rows, possibly of
+// the next chunk, are requested before the current round is reduced.
 #pragma once
+#include "cmb_k2_slots.cuh"
 
 struct K2Args {
   const uint32_t* off_span;
@@ -25,7 +33,7 @@ struct K2Args {
   cmb_contig_stats* rows;
   uint32_t tid_begin, n_local, n_chunks, excl;
   int32_t* arena;
-  uint32_t* span_bits;   // [n_chunks * K2_WARPS] span occupancy bitmap (K1); word w of a chunk = the spans of its warp w
+  uint32_t* span_bits;   // [n_chunks * 8] span occupancy bitmap (K1); bit b of word w of a chunk = its span 32 w + b
   uint32_t* load_stats;  // [0] += spans loaded, [1] += chunks loaded whole (CMB_PIPELINE_STATS)
   const uint64_t* bin_base;  // [n_local + 1] first bin of each contig (K1b); bin_base[n_local] = bins needed
   uint32_t* bins;            // the bin pool: pool_cap u32 counts, zero outside a sample
@@ -34,7 +42,7 @@ struct K2Args {
   uint32_t* error_flags;
 };
 
-// A chunk with at least this many non-empty spans (of 256) is loaded whole with one TMA tile; sparser chunks row by row.
+// A chunk with at least this many non-empty spans (of 256) is loaded whole, 32 rows per TMA box; sparser chunks row by row.
 // On an H100 80GB HBM3 at 400 W, K2 time moved by under 2 % for thresholds from 96 to 257 (never whole) on both `bench.py
 // --config 2` and `--config ns` (DESIGN.md §4, K2): row copies are not what limits K2 there.  160 sends chunks above ~60 %
 // occupancy down the TMA path.
@@ -42,337 +50,257 @@ struct K2Args {
 #define CMB_K2_DENSE_SPANS 160
 #endif
 constexpr uint32_t K2_DENSE_SPANS = CMB_K2_DENSE_SPANS;
-static_assert(K2_STAGES >= 2, "the refill of a stage is issued one iteration after it was read");
+static_assert(K2_STAGES >= 2, "a round's rows are requested one round before it is reduced");
+static_assert(K2_CHUNK_SPANS == CHUNK_SPANS && K2_WARPS == 8, "a chunk is 8 bitmap words of 32 spans");
 
-constexpr uint32_t K2_SMEM_STAGE_BYTES = K2_STAGES * CHUNK_BYTES;
-constexpr uint32_t K2_SMEM_MISC = 64 /*barriers*/ + 2 * K2_WARPS * 8 /*warp aggregates, double-buffered*/;
+constexpr uint32_t K2_ROUND = 32;                     // slots per round, one per lane
+constexpr uint32_t K2_BUF_BYTES = K2_ROUND * 128;     // one round's rows: 4 KB, whole 1024-B swizzle atoms
+constexpr uint32_t K2_BOX_ROWS = K2_ROUND;            // rows of the TMA box (cmb_set_reference encodes it)
+constexpr uint32_t K2_SMEM_STAGE_BYTES = K2_WARPS * K2_STAGES * K2_BUF_BYTES;
+constexpr uint32_t K2_SMEM_MISC = K2_WARPS * K2_STAGES * 8 /*an mbarrier per (warp, stage)*/ + K2_WARPS * 64 /*bitmap words*/;
 constexpr uint32_t K2_SMEM_BYTES = K2_SMEM_STAGE_BYTES + K2_SMEM_MISC;
+
+__device__ __forceinline__ uint32_t k2_rounds(uint32_t pop, bool dense) { return dense ? CHUNK_SPANS / K2_ROUND : (pop + K2_ROUND - 1) / K2_ROUND; }
 
 template <bool HIST, bool CLEAN>
 __global__ void __launch_bounds__(K2_THREADS, CMB_K2_MINBLOCKS) k2_scan_reduce(const __grid_constant__ CUtensorMap tmap, const K2Args a) {
-  extern __shared__ __align__(1024) uint8_t smem[];  // stage tiles need the 1024 B swizzle-atom alignment
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem + K2_SMEM_STAGE_BYTES);
-  int2* wagg2 = reinterpret_cast<int2*>(smem + K2_SMEM_STAGE_BYTES + 64);
+  extern __shared__ __align__(1024) uint8_t smem[];  // the buffers need the 1024 B swizzle-atom alignment
+  const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  uint8_t* ring = smem + warp * K2_STAGES * K2_BUF_BYTES;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + K2_SMEM_STAGE_BYTES) + warp * K2_STAGES;
+  // the 8 bitmap words of the chunk being fetched and of the one being reduced (in shared memory rather than registers: K2
+  // runs at the 80-register cap)
+  uint32_t* words = reinterpret_cast<uint32_t*>(smem + K2_SMEM_STAGE_BYTES + K2_WARPS * K2_STAGES * 8) + warp * 16;
+  uint32_t(&fw)[8] = *reinterpret_cast<uint32_t(*)[8]>(words);
+  uint32_t(&w)[8] = *reinterpret_cast<uint32_t(*)[8]>(words + 8);
 
-  const uint32_t t = threadIdx.x, lane = t & 31, warp = t >> 5;
   // The pool is sized before the launch from a bound of bin_base[n_local]; when it is still too small (cmb_grow_buffers
   // then grows it to exactly that) no bin is added and K3 reads none.
   const bool hist = HIST && __ldg(a.bin_base + a.n_local) <= a.pool_cap;
-  if (HIST && !hist && blockIdx.x == 0 && t == 0) atomicOr(a.error_flags, ERR_CAPACITY);
+  if (HIST && !hist && blockIdx.x == 0 && threadIdx.x == 0) atomicOr(a.error_flags, ERR_CAPACITY);
 
-  // Static schedule: iteration i of CTA b works on chunk b + i * gridDim.x.  Every thread knows its next chunk, so the chunk's
-  // metadata (first / last contig, carry-in, bitmap words) is requested ahead and the dependent lookups (contig of the span,
-  // its start and length) can start before the tile has even arrived.
-  auto chunk_of = [&](uint32_t i) -> uint32_t { return blockIdx.x + i * gridDim.x; };
+  const uint32_t W = gridDim.x * K2_WARPS, g = blockIdx.x * K2_WARPS + warp;
   // word `lane` (lanes 0..7) of chunk ck's span bitmap
-  auto load_bits = [&](uint32_t ck) -> uint32_t {
-    return ck < a.n_chunks && lane < K2_WARPS ? a.span_bits[ck * K2_WARPS + lane] : 0u;
+  auto load_word = [&](uint32_t ck) -> uint32_t { return ck < a.n_chunks && lane < K2_WARPS ? a.span_bits[ck * K2_WARPS + lane] : 0u; };
+  // lanes 0..7 put their words of a chunk into `to` for the whole warp; returns the chunk's popcount
+  auto spread = [&](uint32_t word, uint32_t* to) -> uint32_t {
+    __syncwarp();  // every lane is done with the previous chunk's words
+    if (lane < K2_WARPS) to[lane] = word;
+    __syncwarp();
+    return __reduce_add_sync(FULL, __popc(word));
   };
-  uint32_t n_loaded = 0, n_dense = 0;  // thread 0: what this CTA fetched (load_stats)
-  // All threads: start loading chunk ck into stage s.  `bits` is load_bits(ck).  Every thread commits one cp.async group per
-  // call, so that cp.async.wait_group counts the same way everywhere.  Returns the warp's spans that the stage will hold.
-  auto fill = [&](uint32_t s, uint32_t ck, uint32_t bits) -> uint32_t {
-    uint32_t have = 0;
-    if (ck < a.n_chunks) {
-      const uint32_t pop = __reduce_add_sync(FULL, __popc(bits));  // the same on every thread: a CTA-uniform decision
-      const uint32_t own = __shfl_sync(FULL, bits, warp);
-      const bool dense = pop >= K2_DENSE_SPANS;
-      uint8_t* tile = smem + s * CHUNK_BYTES;
-      if (t == 0) {
-        const uint32_t bar = smem_u32(full + s);
-        if (dense) {
-          fence_proxy_async_smem();  // the stage's previous reads and cp.async writes (ordered by the CTA barrier) come first
-          mbar_arrive_expect_tx(bar, CHUNK_BYTES);
-          tma_load_2d(smem_u32(tile), &tmap, 0, (int32_t)(ck * CHUNK_ROWS), bar);
-        } else {
-          mbar_arrive(bar);  // keeps the barrier's phase in step with the whole-tile stages
-        }
-        n_loaded += dense ? CHUNK_SPANS : pop;
-        n_dense += dense;
+
+  if (lane == 0) {
+    for (uint32_t s = 0; s < K2_STAGES; ++s) mbar_init(smem_u32(bars + s), 1);
+    fence_barrier_init();
+  }
+  __syncwarp();
+
+  // ---- the fetch cursor: round fr of chunk fk is the next one whose rows are requested.  It runs K2_STAGES - 1
+  //      rounds ahead of the reduction, through the same chunks and rounds, skipping the chunks that have none.
+  uint32_t fk = g, fr = 0, fpop = 0;
+  bool fdense = false;
+  uint32_t f_word = load_word(fk);      // bitmap word of chunk fk, requested a chunk ahead
+  uint32_t n_loaded = 0, n_dense = 0;   // what this warp fetched (load_stats)
+  auto f_enter = [&]() {
+    for (; fk < a.n_chunks; fk += W) {
+      const uint32_t word = f_word;
+      f_word = load_word(fk + W);
+      fpop = spread(word, fw);
+      fdense = fpop >= K2_DENSE_SPANS;
+      fr = 0;
+      if (k2_rounds(fpop, fdense)) {
+        n_loaded += fdense ? CHUNK_SPANS : fpop;
+        n_dense += fdense;
+        return;
       }
-      if (dense) {
-        have = FULL;
-      } else {
-        // The warp copies its own non-empty rows, four per instruction: lanes 8q..8q+7 take the eight 16-byte units of the
-        // q-th row of the round, so every instruction moves four whole 128-byte lines.  The rows land where the TMA box would
-        // put them (unit j of row r at r * 128 + (j ^ (r & 7)) * 16).  A thread lets other lanes write only its own row and
-        // reads no other row, so a stage needs no CTA-wide completion; the warp waits for its group and syncs before reading.
-        have = own;
-        uint32_t m = own;
-        const uint32_t q = lane >> 3, unit = lane & 7;
-        const int4* src = reinterpret_cast<const int4*>(a.arena + (uint64_t)ck * CHUNK + (uint64_t)warp * 32 * SPAN) + unit;
-        while (m) {
-          uint32_t r = 32;
-#pragma unroll
-          for (uint32_t k = 0; k < 4; ++k) {
-            if (k == q && m) r = (uint32_t)__ffs(m) - 1;
-            m &= m - 1;
-          }
-          if (r < 32) {
-            const uint32_t row = warp * 32 + r;
-            cp_async_16(smem_u32(tile + row * 128 + ((unit ^ (row & 7)) << 4)), src + r * (SPAN / 4));
-          }
+    }
+  };
+  // Request the fetch cursor's round, the warp's fi-th, into stage fi % K2_STAGES and advance the cursor.  Every lane commits
+  // one cp.async group per call (empty past the last round), so that cp.async.wait_group counts the same way on every lane.
+  auto fill = [&](uint32_t fi) {
+    if (fk < a.n_chunks) {
+      uint8_t* buf = ring + (fi % K2_STAGES) * K2_BUF_BYTES;
+      const uint32_t bar = smem_u32(bars + fi % K2_STAGES);
+      if (fdense) {
+        if (lane == 0) {
+          fence_proxy_async_smem();  // the stage's earlier reads and cp.async writes (ordered by __syncwarp) come first
+          mbar_arrive_expect_tx(bar, K2_BUF_BYTES);
+          tma_load_2d(smem_u32(buf), &tmap, 0, (int32_t)(fk * CHUNK_ROWS + fr * K2_BOX_ROWS), bar);
         }
+      } else {
+        // lanes 8q..8q+7 take the eight 16-byte units of row r0 + q, so every instruction moves four whole 128-byte lines;
+        // unit u of row r lands at r * 128 + (u ^ (r & 7)) * 16, where the TMA box would put it
+        const uint32_t n = min(K2_ROUND, fpop - fr * K2_ROUND);
+        const uint32_t sp = k2_slot_span(fw, fr * K2_ROUND + lane, false);
+        const uint32_t q = lane >> 3, unit = lane & 7;
+        const int4* src = reinterpret_cast<const int4*>(a.arena + (uint64_t)fk * CHUNK) + unit;
+        for (uint32_t r0 = 0; r0 < n; r0 += 4) {
+          const uint32_t row = r0 + q;
+          const uint32_t rsp = __shfl_sync(FULL, sp, row & 31);
+          if (row < n) cp_async_16(smem_u32(buf + row * 128 + ((unit ^ (row & 7)) << 4)), src + rsp * (SPAN / 4));
+        }
+        if (lane == 0) mbar_arrive(bar);  // keeps the barrier's phase in step with the TMA stages
+      }
+      if (++fr == k2_rounds(fpop, fdense)) {
+        fk += W;
+        f_enter();
       }
     }
     cp_async_commit();
-    return have;
+  };
+  f_enter();
+  for (uint32_t p = 0; p + 1 < K2_STAGES; ++p) fill(p);
+
+  const uint32_t E = a.excl;
+  // one contig's share of a warp's runs: the REDs into its row and its bin_hi
+  auto flush = [&](uint32_t c, uint32_t sf, uint32_t sw, uint64_t sd, uint32_t top) {
+    cmb_contig_stats* rowp = a.rows + a.tid_begin + c;
+    if (sf) atomicAdd((unsigned long long*)&rowp->covered_full, (unsigned long long)sf);
+    if (sw) atomicAdd((unsigned long long*)&rowp->covered_window, (unsigned long long)sw);
+    if (sd) atomicAdd((unsigned long long*)&rowp->sum_depth_window, (unsigned long long)sd);
+    if (top) atomicMax(a.bin_hi + c, top);
+  };
+  // a run's window count into bin `depth` of the contig whose bins are [bin0, bin1)
+  auto bin_add = [&](uint64_t bin0, uint64_t bin1, int depth, uint32_t cnt, uint32_t& top) {
+    // 0 <= depth <= bound = bin1 - bin0 - 1 for a consistent arena (every -1 follows its +1 within the contig, and a record
+    // adds at most 1 at any position)
+    if (depth < 0 || (uint64_t)depth >= bin1 - bin0) {
+      atomicOr(a.error_flags, ERR_INTERNAL);
+      return;
+    }
+    atomicAdd(a.bins + bin0 + (uint32_t)depth, cnt);
+    top = max(top, (uint32_t)depth);
   };
 
-  if (t == 0) {
-    for (uint32_t s = 0; s < K2_STAGES; ++s) mbar_init(smem_u32(full + s), 1);
-    fence_barrier_init();
-  }
-  __syncthreads();
-  // have[k] / own[k]: the spans of this warp that stage k holds / the bitmap word of this warp for the chunk in stage k
-  uint32_t have[K2_STAGES], own[K2_STAGES];
-#pragma unroll
-  for (uint32_t s = 0; s < K2_STAGES; ++s) {
-    const uint32_t bits = load_bits(chunk_of(s));
-    own[s] = __shfl_sync(FULL, bits, warp);
-    have[s] = fill(s, chunk_of(s), bits);
-  }
-  uint32_t n_bits = load_bits(chunk_of(K2_STAGES));  // the bitmap of the next chunk to fill, requested an iteration ahead
-  __syncthreads();
-
-  constexpr uint32_t UNITS = SPAN / 4;  // 16-byte units per span
-  const uint32_t row = t;               // this thread's span is tile row t
-  // byte offset inside a stage tile of element e of this thread's span
-  auto elem_off = [&](uint32_t e) -> uint32_t { return row * 128 + (((e >> 2) ^ (row & 7)) << 4) + ((e & 3) << 2); };
-  const uint32_t E = a.excl;
-  uint32_t n_cf = 0, n_cl = 0;  // metadata of the NEXT iteration's chunk, requested an iteration ahead
+  uint32_t c_word = load_word(g);  // the next chunk's bitmap word and metadata, requested a chunk ahead
+  uint32_t n_cf = 0, n_cl = 0;
   int n_cin = 0;
-  if (chunk_of(0) < a.n_chunks) {
-    n_cf = __ldg(a.chunk_first + chunk_of(0));
-    n_cl = __ldg(a.chunk_first + chunk_of(0) + 1);
-    n_cin = __ldg(a.carry_in + chunk_of(0));
+  if (g < a.n_chunks) {
+    n_cf = __ldg(a.chunk_first + g);
+    n_cl = __ldg(a.chunk_first + g + 1);
+    n_cin = __ldg(a.carry_in + g);
   }
-  uint32_t it = 0;
-
-  for (;; ++it) {
-    const uint32_t s = it % K2_STAGES;
-    const uint32_t chunk = chunk_of(it);
-    if (chunk >= a.n_chunks) break;
-    const uint32_t cf = n_cf, cl = n_cl;
+  uint32_t i = 0;  // rounds reduced by this warp
+  for (uint32_t k = g; k < a.n_chunks; k += W) {
+    const uint32_t word = c_word, cf = n_cf, cl = n_cl;
     const int cin = n_cin;
-    {
-      const uint32_t nx = chunk_of(it + 1);
-      if (nx < a.n_chunks) {
-        n_cf = __ldg(a.chunk_first + nx);
-        n_cl = __ldg(a.chunk_first + nx + 1);
-        n_cin = __ldg(a.carry_in + nx);
-      }
+    c_word = load_word(k + W);
+    if (k + W < a.n_chunks) {
+      n_cf = __ldg(a.chunk_first + k + W);
+      n_cl = __ldg(a.chunk_first + k + W + 1);
+      n_cin = __ldg(a.carry_in + k + W);
     }
-    // ---- which contig owns this thread's span (needs no tile data: these loads fly while the tile arrives and is scanned)
-    const uint32_t span = chunk * CHUNK_SPANS + t;
-    uint32_t c;
-    {
-      uint32_t lo = cf, hi = cl;
-      while (lo < hi) {
-        const uint32_t mid = (lo + hi + 1) >> 1;
-        if (__ldg(a.off_span + mid) <= span) lo = mid;
-        else hi = mid - 1;
-      }
-      c = lo;
-    }
-    const uint32_t cstart = __ldg(a.off_span + c);
-    const uint32_t L = __ldg(a.len + c);
-    uint64_t bin0 = 0, bin1 = 0;  // this contig's bins
-    if (hist) {
-      bin0 = __ldg(a.bin_base + c);
-      bin1 = __ldg(a.bin_base + c + 1);
-    }
-    uint32_t s_have = 0, s_own = 0;
-#pragma unroll
-    for (uint32_t k = 0; k < K2_STAGES; ++k)
-      if (k == s) {
-        s_have = have[k];
-        s_own = own[k];
-      }
-    mbar_wait(smem_u32(full + s), (it / K2_STAGES) & 1);
-    cp_async_wait<K2_STAGES - 2>();  // this thread's copies into stage s (only later fills may still be in flight)
-    __syncwarp();                    // ... and those of the other lanes of its warp
-    if (CLEAN && lane == 0 && s_own) a.span_bits[chunk * K2_WARPS + warp] = 0;
-    int2* wagg = wagg2 + (it & 1) * K2_WARPS;
-
-    // ---- SPAN consecutive deltas per thread: LDS.128s through the 128B swizzle (conflict-free).
-    //      Only their sum and the mask of non-zero positions stay in registers.  A span the stage does not hold is all zero.
-    const uint8_t* tilep = smem + s * CHUNK_BYTES;
-    int total = 0;
-    uint32_t ev = 0;
-    if ((s_have >> lane) & 1u) {
-      int4* g = reinterpret_cast<int4*>(a.arena + (uint64_t)span * SPAN);
-#pragma unroll
-      for (uint32_t j = 0; j < UNITS; ++j) {
-        const int4 q = *reinterpret_cast<const int4*>(tilep + row * 128 + ((j ^ (row & 7)) << 4));
-        const uint32_t e4 = (q.x != 0 ? 1u : 0u) | (q.y != 0 ? 2u : 0u) | (q.z != 0 ? 4u : 0u) | (q.w != 0 ? 8u : 0u);
-        total += (q.x + q.y) + (q.z + q.w);
-        ev |= e4 << (4 * j);
-        if (CLEAN && e4) g[j] = make_int4(0, 0, 0, 0);  // re-zero only the 16 B units that hold an event
-      }
-    }
-
-    const bool is_head = span == cstart;
-    const uint32_t rel = (span - cstart) * SPAN;  // position in the contig of the span's first element
-    const uint32_t n_in = rel >= L ? 0u : min(SPAN, L - rel);
-    uint32_t w0 = 0, w1 = 0;
-    if (2ull * E < L) {
-      const uint32_t ws = E, we = L - E;
-      w0 = rel >= ws ? 0u : min(SPAN, ws - rel);
-      w1 = rel >= we ? 0u : min(SPAN, we - rel);
-      if (w1 < w0) w1 = w0;
-    }
-
-    // ---- segmented (by contig head) inclusive scan of span totals across the warp
-    int val = total;
-    int flg = is_head;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-      const int ov = __shfl_up_sync(FULL, val, d);
-      const int of = __shfl_up_sync(FULL, flg, d);
-      if ((int)lane >= d) {
-        if (!flg) val += ov;
-        flg |= of;
-      }
-    }
-    int pval = __shfl_up_sync(FULL, val, 1), pflg = __shfl_up_sync(FULL, flg, 1);
-    if (lane == 0) {
-      pval = 0;
-      pflg = 0;
-    }
-    if (lane == 31) wagg[warp] = make_int2(val, flg);
-    __syncthreads();  // warp aggregates visible; the previous iteration's tile reads are complete
-    if (it > 0) {
-      // refill the stage of the previous iteration (read until this barrier)
-      const uint32_t rs = (it - 1) % K2_STAGES, rk = chunk_of(it - 1 + K2_STAGES);
-      const uint32_t r_own = __shfl_sync(FULL, n_bits, warp);
-      const uint32_t r_have = fill(rs, rk, n_bits);
-#pragma unroll
-      for (uint32_t k = 0; k < K2_STAGES; ++k)
-        if (k == rs) {
-          have[k] = r_have;
-          own[k] = r_own;
+    const uint32_t pop = spread(word, w);
+    const bool dense = pop >= K2_DENSE_SPANS;
+    const uint32_t nr = k2_rounds(pop, dense), nslots = dense ? CHUNK_SPANS : pop;
+    const uint32_t span0 = k * CHUNK_SPANS;
+    uint32_t pc = cf, c_first = 0xffffffffu;  // contig of the previous round's last slot; of the chunk's first slot
+    int pd = cin;                             // depth leaving the previous round's last slot
+    for (uint32_t r = 0; r < nr; ++r, ++i) {
+      __syncwarp();  // every lane is done with the stage that the fill below overwrites
+      fill(i + K2_STAGES - 1);
+      const uint32_t j = r * K2_ROUND + lane;
+      const bool valid = j < nslots;
+      const uint32_t s = k2_slot_span(w, j, dense), sn = k2_slot_span(w, j + 1, dense);
+      // ---- the slot's contig, start, window and bins (no tile data needed: these loads fly while the rows arrive)
+      uint32_t c = 0xffffffffu, cstart = 0;
+      K2Win win{0u, 0u, 0u};
+      uint64_t bin0 = 0, bin1 = 0;
+      if (valid) {
+        uint32_t lo = cf, hi = cl;
+        while (lo < hi) {
+          const uint32_t mid = (lo + hi + 1) >> 1;
+          if (__ldg(a.off_span + mid) <= span0 + s) lo = mid;
+          else hi = mid - 1;
         }
-      n_bits = load_bits(chunk_of(it + K2_STAGES));
-    }
-
-    int wv, wf;
-    {
-      const int2 wa = lane < K2_WARPS ? wagg[lane] : make_int2(0, 0);
-      wv = wa.x;
-      wf = wa.y;
-#pragma unroll
-      for (int d = 1; d < (int)K2_WARPS; d <<= 1) {
-        const int ov = __shfl_up_sync(FULL, wv, d);
-        const int of = __shfl_up_sync(FULL, wf, d);
-        if ((int)lane >= d) {
-          if (!wf) wv += ov;
-          wf |= of;
+        c = lo;
+        cstart = __ldg(a.off_span + c);
+        win = k2_window(__ldg(a.len + c), E);
+        if (hist) {
+          bin0 = __ldg(a.bin_base + c);
+          bin1 = __ldg(a.bin_base + c + 1);
         }
       }
-      const int src = warp ? (int)warp - 1 : 0;
-      wv = __shfl_sync(FULL, wv, src);
-      wf = __shfl_sync(FULL, wf, src);
-      if (warp == 0) {
-        wv = 0;
-        wf = 0;
-      }
-    }
-    int carry;
-    if (is_head) carry = 0;
-    else if (pflg) carry = pval;
-    else if (wf) carry = wv + pval;
-    else carry = cin + wv + pval;
-
-    // ---- reductions over this span (EST:393-404, 447-465, 494-501), run by run
-    uint32_t cov_full = 0, cov_win = 0;
-    uint64_t sum_win = 0;
-    uint32_t bin_top = 0;  // highest depth this thread added to contig c's bins
-    auto hist_add = [&](int depth, uint32_t cnt) {
-      // 0 <= depth <= bound = bin1 - bin0 - 1 for a consistent arena (every -1 follows its +1 within the contig, and a
-      // record adds at most 1 at any position)
-      if (depth < 0 || (uint64_t)depth >= bin1 - bin0) {
-        atomicOr(a.error_flags, ERR_INTERNAL);
-        return;
-      }
-      atomicAdd(a.bins + bin0 + (uint32_t)depth, cnt);
-      bin_top = max(bin_top, (uint32_t)depth);
-    };
-    // a run [from, to) of the span at one depth, clipped to the contig and to its end-trimmed window
-    auto close_run = [&](int depth, uint32_t from, uint32_t to) {
-      const uint32_t nc = min(to, n_in) - min(from, n_in);
-      const uint32_t nw = min(max(to, w0), w1) - min(max(from, w0), w1);
-      if (depth > 0) {
-        cov_full += nc;
-        cov_win += nw;
-      }
-      if (nw) {
-        sum_win += (uint64_t)(int64_t)depth * nw;
-        if (hist && depth != 0) hist_add(depth, nw);
-      }
-    };
-    if (ev) {
-      int depth = carry;
-      uint32_t from = 0;
-      uint32_t m = ev;
-      while (m) {
-        const uint32_t j = (uint32_t)__ffs((int)m) - 1;
-        m &= m - 1;
-        close_run(depth, from, j);
-        depth += *reinterpret_cast<const int*>(tilep + elem_off(j));  // the delta at position j
-        from = j;
-      }
-      close_run(depth, from, SPAN);
-    } else {  // no event in the span: constant depth
-      const uint32_t nc = n_in, nw = w1 - w0;
-      if (carry > 0) {
-        cov_full += nc;
-        cov_win += nw;
-      }
-      sum_win += (uint64_t)(int64_t)carry * nw;
-    }
-    if (hist) {
-      // event-free spans: one RED per distinct (contig, depth) of the warp, added by the group's first lane (usually 1-3 groups)
-      const uint32_t nw = w1 - w0;
-      uint32_t cm = __ballot_sync(FULL, ev == 0 && nw > 0 && carry != 0);
-      while (cm) {
-        const int leader = __ffs(cm) - 1;
-        const int d0 = __shfl_sync(FULL, carry, leader);
-        const uint32_t c0 = __shfl_sync(FULL, c, leader);
-        const bool same = ((cm >> lane) & 1u) && carry == d0 && c == c0;
-        const uint32_t m = __ballot_sync(FULL, same);
-        if (same) {
-          const uint32_t tot = __reduce_add_sync(m, nw);
-          if ((int)lane == leader) hist_add(carry, tot);
+      const uint32_t st = i % K2_STAGES;
+      mbar_wait(smem_u32(bars + st), (i / K2_STAGES) & 1);
+      cp_async_wait<K2_STAGES - 1>();  // this lane's copies into stage st (only the fill above may still be in flight)
+      __syncwarp();                    // ... and those of the other lanes
+      // ---- the slot's 32 deltas (row `lane`): only their sum and the mask of non-zero positions stay in registers
+      const uint8_t* row = ring + st * K2_BUF_BYTES + lane * 128;
+      int total = 0;
+      uint32_t ev = 0;
+      if (valid) {
+        int4* gsp = reinterpret_cast<int4*>(a.arena + (uint64_t)(span0 + s) * SPAN);
+#pragma unroll
+        for (uint32_t u = 0; u < SPAN / 4; ++u) {
+          const int4 v = *reinterpret_cast<const int4*>(row + ((u ^ (lane & 7)) << 4));
+          const uint32_t e4 = (v.x != 0 ? 1u : 0u) | (v.y != 0 ? 2u : 0u) | (v.z != 0 ? 4u : 0u) | (v.w != 0 ? 8u : 0u);
+          total += (v.x + v.y) + (v.z + v.w);
+          ev |= e4 << (4 * u);
+          if (CLEAN && e4) gsp[u] = make_int4(0, 0, 0, 0);  // re-zero only the 16 B units that hold an event
         }
-        cm &= ~m;
       }
-    }
-
-    // ---- per-contig accumulation: one RED triple (and the bin_hi max) per (warp, contig)
-    {
-      const uint32_t c0 = __shfl_sync(FULL, c, 0);
-      if (__all_sync(FULL, c == c0)) {
-        const uint32_t sf = __reduce_add_sync(FULL, cov_full), sw = __reduce_add_sync(FULL, cov_win);
-        const uint64_t sd = warp_sum_u64(sum_win);
-        const uint32_t top = hist ? __reduce_max_sync(FULL, bin_top) : 0u;
-        if (lane == 0) {
-          cmb_contig_stats* rowp2 = a.rows + a.tid_begin + c0;
-          if (sf) atomicAdd((unsigned long long*)&rowp2->covered_full, (unsigned long long)sf);
-          if (sw) atomicAdd((unsigned long long*)&rowp2->covered_window, (unsigned long long)sw);
-          if (sd) atomicAdd((unsigned long long*)&rowp2->sum_depth_window, (unsigned long long)sd);
-          if (top) atomicMax(a.bin_hi + c0, top);
+      // ---- depth entering the slot: segmented (by contig) exclusive scan of the slot totals, seeded from the previous slot
+      int incl = total;
+#pragma unroll
+      for (uint32_t d = 1; d < 32; d <<= 1) {
+        const int ov = __shfl_up_sync(FULL, incl, d);
+        const uint32_t oc = __shfl_up_sync(FULL, c, d);
+        if (lane >= d && oc == c) incl += ov;
+      }
+      const int depth = incl - total + (c == pc ? pd : 0);
+      // ---- the slot's runs; the chunk's first slot also takes the chunk's head when it is in the head's contig
+      const uint32_t rel = (span0 + s - cstart) * SPAN;
+      const uint32_t from = j == 0 && c == cf ? (span0 - cstart) * SPAN : rel;
+      const uint32_t to = rel + (sn - s) * SPAN;
+      K2Acc acc{0u, 0u, 0ull};
+      uint32_t top = 0;
+      int out = 0;
+      if (valid)
+        out = k2_slot_runs(
+            acc, win, depth, ev, rel, from, to,
+            [&](uint32_t e) { return *reinterpret_cast<const int*>(row + (((e >> 2) ^ (lane & 7)) << 4) + ((e & 3) << 2)); },
+            [&](int d, uint32_t n) {
+              if (hist) bin_add(bin0, bin1, d, n, top);
+            });
+      pc = __shfl_sync(FULL, c, 31);
+      pd = __shfl_sync(FULL, out, 31);
+      if (r == 0) c_first = __shfl_sync(FULL, c, 0);
+      // ---- per-contig REDs: lanes are in contig order; the first lane of each contig's lanes adds their sums
+      uint32_t sf = acc.cov_full, sw = acc.cov_win;
+      uint64_t sd = acc.sum_win;
+#pragma unroll
+      for (uint32_t d = 1; d < 32; d <<= 1) {
+        const uint32_t of = __shfl_down_sync(FULL, sf, d), ow = __shfl_down_sync(FULL, sw, d);
+        const uint64_t od = __shfl_down_sync(FULL, sd, d);
+        const uint32_t ot = HIST ? __shfl_down_sync(FULL, top, d) : 0u;
+        const uint32_t oc = __shfl_down_sync(FULL, c, d);
+        if (lane + d < 32 && oc == c) {
+          sf += of;
+          sw += ow;
+          sd += od;
+          top = max(top, ot);
         }
-      } else {
-        cmb_contig_stats* rowp2 = a.rows + a.tid_begin + c;
-        if (cov_full) atomicAdd((unsigned long long*)&rowp2->covered_full, (unsigned long long)cov_full);
-        if (cov_win) atomicAdd((unsigned long long*)&rowp2->covered_window, (unsigned long long)cov_win);
-        if (sum_win) atomicAdd((unsigned long long*)&rowp2->sum_depth_window, (unsigned long long)sum_win);
-        if (bin_top) atomicMax(a.bin_hi + c, bin_top);
       }
+      const uint32_t prev_c = __shfl_up_sync(FULL, c, 1);
+      if (valid && (lane == 0 || prev_c != c)) flush(c, sf, sw, sd, top);
     }
+    // ---- the chunk's head when no slot took it: from the chunk start to the first slot (the whole chunk if it has none),
+    //      at the carry-in, in the chunk's first contig
+    if (lane == 0 && cin != 0 && c_first != cf) {
+      const uint32_t cstart = __ldg(a.off_span + cf);
+      const K2Win win = k2_window(__ldg(a.len + cf), E);
+      const uint32_t s0 = k2_slot_span(w, 0, dense);
+      K2Acc acc{0u, 0u, 0ull};
+      uint32_t top = 0;
+      const uint32_t nw = k2_close_run(acc, win, cin, (span0 - cstart) * SPAN, (span0 + s0 - cstart) * SPAN);
+      if (hist && nw) bin_add(__ldg(a.bin_base + cf), __ldg(a.bin_base + cf + 1), cin, nw, top);
+      flush(cf, acc.cov_full, acc.cov_win, acc.sum_win, top);
+    }
+    if (CLEAN && word) a.span_bits[k * K2_WARPS + lane] = 0;  // lanes 0..7 (the others hold no word)
   }
-  if (t == 0 && n_loaded) {
+  if (lane == 0 && n_loaded) {
     atomicAdd(a.load_stats + 0, n_loaded);
     atomicAdd(a.load_stats + 1, n_dense);
   }

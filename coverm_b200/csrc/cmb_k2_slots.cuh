@@ -1,0 +1,119 @@
+// K2's per-slot arithmetic as plain integer code, shared by k2_scan_reduce and tests/native/k2_slots_check.cpp (which
+// compiles it with g++ and walks random arenas in the kernel's order against a per-position prefix sum).
+//
+// A chunk's slots are all 256 of its spans when it is dense, else only its occupied spans, in order.  Slot j covers the
+// positions from its span's start up to the next slot's span (the chunk's end for the last slot): past the span's last
+// event the depth stays constant, so the event-free spans after a slot are counted with the slot's last run.
+#pragma once
+#include <stdint.h>
+
+#ifdef __CUDACC__
+#define K2_HD __host__ __device__ __forceinline__
+#else
+#define K2_HD inline
+#endif
+
+constexpr uint32_t K2_CHUNK_SPANS = 256;  // spans per chunk = 8 bitmap words of 32
+
+K2_HD uint32_t k2_popc(uint32_t x) {
+#ifdef __CUDA_ARCH__
+  return __popc(x);
+#else
+  return (uint32_t)__builtin_popcount(x);
+#endif
+}
+
+K2_HD uint32_t k2_low_bit(uint32_t x) {  // x != 0
+#ifdef __CUDA_ARCH__
+  return (uint32_t)__ffs((int)x) - 1u;
+#else
+  return (uint32_t)__builtin_ctz(x);
+#endif
+}
+
+// Position of the n-th (from 0) set bit of x; n < popcount(x).  Five halving steps, the same code on host and device.
+K2_HD uint32_t k2_nth_bit(uint32_t x, uint32_t n) {
+  uint32_t pos = 0;
+#pragma unroll
+  for (uint32_t w = 16; w; w >>= 1) {
+    const uint32_t lo = k2_popc(x & ((1u << w) - 1u));
+    if (n >= lo) {
+      n -= lo;
+      x >>= w;
+      pos += w;
+    }
+  }
+  return pos;
+}
+
+// Span (0..255) of slot j of a chunk with bitmap words w[0..7]; K2_CHUNK_SPANS when there is no slot j.
+K2_HD uint32_t k2_slot_span(const uint32_t (&w)[8], uint32_t j, bool dense) {
+  if (dense) return j < K2_CHUNK_SPANS ? j : K2_CHUNK_SPANS;
+  uint32_t base = 0, word = 0, rem = j;
+  bool found = false;
+#pragma unroll
+  for (uint32_t q = 0; q < 8; ++q) {
+    const uint32_t p = k2_popc(w[q]);
+    if (!found) {
+      if (rem < p) {
+        found = true;
+        base = 32 * q;
+        word = w[q];
+      } else {
+        rem -= p;
+      }
+    }
+  }
+  return found ? base + k2_nth_bit(word, rem) : K2_CHUNK_SPANS;
+}
+
+// A contig's length and its end-trimmed window [w0, w1) (empty when 2E >= L), in contig coordinates.
+struct K2Win {
+  uint32_t L, w0, w1;
+};
+K2_HD K2Win k2_window(uint32_t L, uint32_t E) {
+  K2Win w{L, 0u, 0u};
+  if (2ull * E < L) {
+    w.w0 = E;
+    w.w1 = L - E;
+  }
+  return w;
+}
+
+// What a contig gains from its runs (EST:393-404, 447-465, 494-501).
+struct K2Acc {
+  uint32_t cov_full, cov_win;
+  uint64_t sum_win;
+};
+
+// The run [from, to) at `depth`, clipped to [0, L) and to the window; returns its window positions (its histogram count).
+K2_HD uint32_t k2_close_run(K2Acc& a, const K2Win& w, int depth, uint32_t from, uint32_t to) {
+  const uint32_t nc = (to < w.L ? to : w.L) - (from < w.L ? from : w.L);
+  const uint32_t t1 = to < w.w0 ? w.w0 : (to > w.w1 ? w.w1 : to), f1 = from < w.w0 ? w.w0 : (from > w.w1 ? w.w1 : from);
+  const uint32_t nw = t1 - f1;
+  if (depth > 0) {
+    a.cov_full += nc;
+    a.cov_win += nw;
+  }
+  a.sum_win += (uint64_t)(int64_t)depth * nw;
+  return nw;
+}
+
+// The runs of one slot: `from` .. `to` in contig coordinates, `rel` the position of its span's first element, `ev` the
+// positions of that span with a delta (delta(j) reads it), `depth` the depth entering the slot.  hist(depth, n) is called
+// for every run at a depth other than 0 with n > 0 window positions.  Returns the depth leaving the slot.
+template <class Delta, class Hist>
+K2_HD int k2_slot_runs(K2Acc& a, const K2Win& w, int depth, uint32_t ev, uint32_t rel, uint32_t from, uint32_t to, Delta delta,
+                       Hist hist) {
+  while (ev) {
+    const uint32_t j = k2_low_bit(ev);
+    ev &= ev - 1;
+    const uint32_t nw = k2_close_run(a, w, depth, from, rel + j);
+    if (nw && depth != 0) hist(depth, nw);
+    depth += delta(j);
+    from = rel + j;
+  }
+  const uint32_t nw = k2_close_run(a, w, depth, from, to);
+  if (nw && depth != 0) hist(depth, nw);
+  return depth;
+}
