@@ -245,7 +245,9 @@ struct cmb_ctx {
     Buf<uint32_t> d_pair_next;
     Buf<unsigned long long> d_pair_tag;
     Buf<uint32_t> d_pair_head;
+    Buf<uint2> d_pair_order;  // kd_pair_order: per PAIR_ORDER_CHUNK records, their first and last eligible tid
     const int32_t* last_mate = nullptr;
+    bool last_mate_inverse = false;  // last_mate was matched for `coverm filter --inverse` (unmapped records not eligible)
     uint32_t last_excl_n = 0xffffffffu;
     const uint8_t* last_infl_base = nullptr;  // biased base of the inflated stream of the last decode
     // coverm filter
@@ -541,6 +543,51 @@ int collect_errors_and_timing(cmb_ctx* c, uint32_t* counters_out) {
   if (e & ERR_INTERNAL)
     return fail(c, CMB_E_CUDA, "internal error: running depth below 0 or above the read count (inconsistent delta arena, or a "
                 "record whose aligned blocks overlap)");
+  return CMB_OK;
+}
+
+// Mate matching over the resident inflated stream (cmb_pairs.cuh); sets d.last_mate.  filter_out: ReferenceSortedBamFilter's
+// (false only for `coverm filter --inverse`).  Declines when the stream needs the host's file-order walk.
+int match_mates(cmb_ctx* c, const uint8_t* infl_base, uint32_t n_rec, bool filter_out, const char* who) {
+  auto& d = c->dec;
+  int rc;
+  d.last_mate = nullptr;
+  d.filter_planned = false;
+  if (d.d_pair_key.cap < n_rec) {  // growing: give the filter's buffers back first (cmb_filter_plan sizes them again)
+    d.d_filter_anchor.release();
+    d.d_filter_role.release();
+    d.d_filter_out.release();
+  }
+  const size_t want = with_slack(n_rec);
+  const uint32_t n_chunks = (n_rec + PAIR_ORDER_CHUNK - 1) / PAIR_ORDER_CHUNK;
+  if ((rc = d.d_pair_key.ensure(c, n_rec, want)) || (rc = d.d_pair_mate.ensure(c, n_rec, want)) || (rc = d.d_pair_next.ensure(c, n_rec, want)) ||
+      (rc = d.d_pair_order.ensure(c, n_chunks, with_slack(n_chunks))))
+    return rc;
+  size_t table = 1u << 16;
+  while (table < 2 * (size_t)n_rec) table <<= 1;
+  if ((rc = d.d_pair_tag.ensure(c, table)) || (rc = d.d_pair_head.ensure(c, table))) return rc;
+  CU_TRY(c, cudaMemsetAsync(d.d_pair_tag, 0, 8 * table, c->stream));
+  CU_TRY(c, cudaMemsetAsync(d.d_pair_head, 0xff, 4 * table, c->stream));
+  CU_TRY(c, cudaMemsetAsync(d.d_cnt + 1, 0, 4, c->stream));
+  PairArgs pa{};
+  pa.data = infl_base; pa.rec_off = d.d_rec_off; pa.n_records = n_rec; pa.key = d.d_pair_key; pa.mate = d.d_pair_mate;
+  pa.next = d.d_pair_next; pa.slot_tag = d.d_pair_tag; pa.slot_head = d.d_pair_head; pa.table_mask = (uint32_t)(table - 1);
+  pa.flags = d.d_cnt + 1; pa.order = d.d_pair_order; pa.filter_out = filter_out ? 1 : 0;
+  const uint32_t gr = (n_rec + 255) / 256;
+  kd_pair_keys<<<gr, 256, 0, c->stream>>>(pa);
+  kd_pair_order<<<(n_chunks + 255) / 256, 256, 0, c->stream>>>(pa);
+  kd_pair_order_fold<<<1, 1024, 0, c->stream>>>(d.d_pair_order, n_chunks, pa.flags);
+  kd_pair_insert<<<gr, 256, 0, c->stream>>>(pa);
+  kd_pair_resolve<<<(uint32_t)((table + 255) / 256), 256, 0, c->stream>>>(pa);
+  CU_TRY(c, cudaGetLastError());
+  uint32_t flags = 0;
+  CU_TRY(c, cudaMemcpyAsync(&flags, d.d_cnt + 1, 4, cudaMemcpyDeviceToHost, c->stream));
+  CU_TRY(c, cudaStreamSynchronize(c->stream));
+  if (flags)
+    return fail(c, CMB_E_DECLINED, "%s: mate matching gave up (flags %u: %s)", who, flags,
+                (flags & DEC_ERR_PAIR_ORDER) ? "the proper-pair records' reference ids are not sorted" : "too many records of one name");
+  d.last_mate = d.d_pair_mate;
+  d.last_mate_inverse = !filter_out;
   return CMB_OK;
 }
 
@@ -887,6 +934,9 @@ int cmb_submit_device_batch(cmb_ctx* c, const cmb_read_batch* dev, uint32_t n_re
   CU_TRY(c, cudaSetDevice(c->device));
   // re-submitting the tuples of the last device decode (cmb_last_bgzf_batch) in pair mode: its mate table goes with it
   const bool is_last = c->dec.last_valid && (const void*)dev->tid == c->dec.d_tuple_slab;
+  if (is_last && c->mode.filter_pairs && (!c->dec.last_mate || c->dec.last_mate_inverse)) {  // decoded by cmb_decode_bgzf
+    if (int rc = match_mates(c, c->dec.last_infl_base, c->dec.last_n_rec, true, "cmb_submit_device_batch")) return rc;
+  }
   const int32_t* mate = (is_last && c->dec.last_mate && c->mode.filter_pairs) ? c->dec.last_mate : nullptr;
   return launch_k1(c, *dev, n_records, n_intervals, is_last ? c->dec.last_excl_n : 0xffffffffu, mate);
 }
@@ -1697,37 +1747,11 @@ int BgzfCall::extract() {
   d.last_valid = true;
   d.last_mate = nullptr;
   d.last_infl_base = infl_base;
-  // mate matching on the device (filter.rs:117-233; cmb_pairs.cuh): for coverage when the pair thresholds apply; for
-  // `coverm filter` whenever the filter's pair path runs (everything but "single-read thresholds only", filter.rs:88)
-  const bool need_mates = decode_only ? !(c->mode.filter_single_reads && !c->mode.filter_pairs) : (bool)c->mode.filter_pairs;
-  if (need_mates) {
-    if (d.d_pair_key.cap < n_rec) {  // growing: give the filter's buffers back first (cmb_filter_plan sizes them again)
-      d.d_filter_anchor.release();
-      d.d_filter_role.release();
-      d.d_filter_out.release();
-    }
-    const size_t want = with_slack(n_rec);
-    if ((rc = d.d_pair_key.ensure(c, n_rec, want)) || (rc = d.d_pair_mate.ensure(c, n_rec, want)) || (rc = d.d_pair_next.ensure(c, n_rec, want)))
-      return rc;
-    size_t table = 1u << 16;
-    while (table < 2 * (size_t)n_rec) table <<= 1;
-    if ((rc = d.d_pair_tag.ensure(c, table)) || (rc = d.d_pair_head.ensure(c, table))) return rc;
-    CU_TRY(c, cudaMemsetAsync(d.d_pair_tag, 0, 8 * table, c->stream));
-    CU_TRY(c, cudaMemsetAsync(d.d_pair_head, 0xff, 4 * table, c->stream));
-    PairArgs pa{};
-    pa.data = infl_base; pa.rec_off = d.d_rec_off; pa.n_records = (uint32_t)n_rec; pa.key = d.d_pair_key; pa.mate = d.d_pair_mate;
-    pa.next = d.d_pair_next; pa.slot_tag = d.d_pair_tag; pa.slot_head = d.d_pair_head; pa.table_mask = (uint32_t)(table - 1);
-    pa.flags = d.d_cnt + 1;
-    const uint32_t gr = (uint32_t)((n_rec + 255) / 256);
-    kd_pair_keys<<<gr, 256, 0, c->stream>>>(pa);
-    kd_pair_insert<<<gr, 256, 0, c->stream>>>(pa);
-    kd_pair_resolve<<<(uint32_t)((table + 255) / 256), 256, 0, c->stream>>>(pa);
-    CU_TRY(c, cudaGetLastError());
-    out->n_launches += 3;
-    CU_TRY(c, cudaMemcpyAsync(h_cnt, d.d_cnt, 64, cudaMemcpyDeviceToHost, c->stream));
-    CU_TRY(c, cudaStreamSynchronize(c->stream));
-    if (h_cnt[1]) return fail(c, CMB_E_DECLINED, "cmb_submit_bgzf: mate matching gave up (flags %u)", h_cnt[1]);
-    d.last_mate = d.d_pair_mate;
+  // mate matching on the device (filter.rs:117-233; cmb_pairs.cuh) for coverage when the pair thresholds apply; `coverm
+  // filter` matches in cmb_filter_plan, where --inverse (which decides the eligible records) is known
+  if (!decode_only && c->mode.filter_pairs) {
+    if ((rc = match_mates(c, infl_base, (uint32_t)n_rec, true, "cmb_submit_bgzf"))) return rc;
+    out->n_launches += 5;
   }
   CU_TRY(c, cudaEventRecord(d.ev[4], c->stream));
   if (c->n_local && !decode_only) {
@@ -1822,8 +1846,8 @@ extern "C" int cmb_filter_plan(cmb_ctx* c, int inverse, uint64_t* n_records, uin
     return CMB_OK;
   }
   const bool pair_path = !(c->mode.filter_single_reads && !c->mode.filter_pairs);
-  if (pair_path && !d.last_mate) return fail(c, CMB_E_ARG, "cmb_filter_plan: the sample was decoded without mate matching (set the parameters before cmb_decode_bgzf)");
   int rc;
+  if (pair_path && (rc = match_mates(c, d.last_infl_base, n, !inverse, "cmb_filter_plan"))) return rc;
   if ((rc = d.d_filter_anchor.ensure(c, (size_t)n + 1, with_slack(n))) || (rc = d.d_filter_role.ensure(c, (size_t)n + 1, with_slack(n))))
     return rc;
   cmb_read_batch tb;

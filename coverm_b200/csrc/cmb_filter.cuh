@@ -7,6 +7,7 @@
 // Every emitted record is given an anchor (the file position at which the reference returns it) and a rank inside the anchor;
 // an exclusive scan of the bytes per anchor gives each record its place in the output, which kf_gather then fills.
 #pragma once
+#include "cmb_filter_preds.cuh"
 
 struct FilterArgs {
   const uint8_t* data;

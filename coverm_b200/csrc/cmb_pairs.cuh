@@ -3,21 +3,27 @@
 //
 // The reference walks the records in file order with a BTreeMap `first_set` of qname -> stored first mate that is
 // cleared whenever the reference id of an eligible record changes:
-//     eligible  = !secondary && !supplementary && proper_pair                         (filter.rs:138-147, filter_out = true)
+//     eligible  = !secondary && !supplementary && proper_pair, and mapped when filter_out is false (filter.rs:133-147:
+//                 `coverm filter --inverse` returns an unmapped record at once, before it can reach first_set)
 //     not found : stored[qname] = record, but only if record.mtid == current tid      (filter.rs:166-176)
 //     found     : the pair (stored, record) is tested and, if it passes, both are emitted (filter.rs:185-219)
-// Per (tid, qname) that is a two-state machine over the eligible records in file order, and different keys never
-// interact -- so it parallelises over keys:
-//   kd_pair_keys     one thread per record: eligibility, a 64-bit hash of (tid, qname), mate[i] = -1
-//   kd_pair_insert   eligible records enter an open-addressing table keyed by the hash (atomicCAS on the tag); the
-//                    records of a key form a linked list (atomicExch on the head)
-//   kd_pair_resolve  one thread per table slot: collect the list, sort it by record index (= file order), split it by
-//                    EXACT (tid, qname) (hash collisions cost time, never correctness), run the state machine and write
-//                    mate[first] = second, mate[second] = first
+// When the tids of the eligible records are non-decreasing in file order, every tid's eligible records form one run, the set
+// is cleared exactly between runs, and the walk is a two-state machine per (tid, qname) over that key's eligible records in
+// file order: different keys never interact.  A stream whose eligible tids go down somewhere is declined
+// (DEC_ERR_PAIR_ORDER) and the host's HostMates walks it in file order instead; a reference-sorted file never is (the
+// unsigned comparison puts unplaced records, tid -1, last).  Otherwise the matching parallelises over keys:
+//   kd_pair_keys       one thread per record: eligibility, a 64-bit hash of (tid, qname), mate[i] = -1
+//   kd_pair_order      one thread per PAIR_ORDER_CHUNK records: the chunk's first and last eligible tid, and whether they
+//                      go down inside it; kd_pair_order_fold then compares every chunk with the largest tid before it
+//   kd_pair_insert     eligible records enter an open-addressing table keyed by the hash (atomicCAS on the tag); the
+//                      records of a key form a linked list (atomicExch on the head)
+//   kd_pair_resolve    one thread per table slot: collect the list, sort it by record index (= file order), split it by
+//                      EXACT (tid, qname) (hash collisions cost time, never correctness), run the state machine and write
+//                      mate[first] = second, mate[second] = first
 // K1 then evaluates the pair predicates with the partner's columns (mate[i] instead of the host path's i ^ 1 layout);
 // records stay in file order.  The emitted order of the reference (stored mate first, at the second mate's position) is
-// irrelevant downstream: both mates carry the same tid, and no eligible record of another tid can lie between them (it
-// would have cleared the set), so the sortedness check (contig.rs:129-132) over the kept records in file order fails
+// irrelevant downstream: both mates carry the same tid, and no eligible record of another tid can lie between them (the
+// eligible tids are non-decreasing), so the sortedness check (contig.rs:129-132) over the kept records in file order fails
 // exactly when it fails over the emitted stream.
 #pragma once
 
@@ -32,10 +38,14 @@ struct PairArgs {
   uint32_t* slot_head;           // table: list head (0xffffffff = nil)
   uint32_t table_mask;           // table size - 1 (power of two)
   uint32_t* flags;               // [0] error bits (DEC_ERR_*)
+  uint2* order;                  // per PAIR_ORDER_CHUNK records: {first, last} eligible tid (unsigned; {~0u, 0} = none)
+  uint8_t filter_out;            // ReferenceSortedBamFilter's filter_out: 0 for `coverm filter --inverse`
 };
 constexpr uint32_t PAIR_NIL = 0xffffffffu;
 constexpr uint32_t PAIR_MAX_GROUP = 24;       // eligible records sharing one table slot; more -> the stream is declined
-constexpr uint32_t DEC_ERR_PAIRS = 8u;
+constexpr uint32_t PAIR_ORDER_CHUNK = 64;     // records per kd_pair_order thread
+constexpr uint32_t DEC_ERR_PAIRS = 8u;        // a table slot holds more than PAIR_MAX_GROUP eligible records
+constexpr uint32_t DEC_ERR_PAIR_ORDER = 16u;  // the tids of the eligible records go down somewhere in file order
 
 __device__ __forceinline__ uint64_t pair_mix(uint64_t h) {  // splitmix64 finaliser
   h ^= h >> 30;
@@ -55,7 +65,7 @@ __global__ void __launch_bounds__(256) kd_pair_keys(const PairArgs a) {
   const uint32_t l_read_name = w2 & 0xff;
   a.mate[i] = -1;
   a.next[i] = PAIR_NIL;
-  const bool eligible = !(flag & 0x900) && (flag & 0x2);
+  const bool eligible = !(flag & 0x900) && (flag & 0x2) && (a.filter_out || !(flag & 0x4));
   uint64_t h = 0;
   if (eligible) {
     h = 0xcbf29ce484222325ull ^ ((uint64_t)tid * 0x9e3779b97f4a7c15ull);
@@ -66,6 +76,47 @@ __global__ void __launch_bounds__(256) kd_pair_keys(const PairArgs a) {
     if (h == 0) h = 1;
   }
   a.key[i] = h;
+}
+
+// Eligible tids in file order, compared as unsigned: a chunk's first and last, and a flag when they go down inside it.
+__global__ void __launch_bounds__(256) kd_pair_order(const PairArgs a) {
+  const uint32_t c = blockIdx.x * 256 + threadIdx.x;
+  const uint32_t i0 = c * PAIR_ORDER_CHUNK;
+  if (i0 >= a.n_records) return;
+  const uint32_t i1 = min(a.n_records, i0 + PAIR_ORDER_CHUNK);
+  uint32_t first = 0xffffffffu, last = 0;
+  bool any = false, down = false;
+  for (uint32_t i = i0; i < i1; ++i) {
+    if (!a.key[i]) continue;
+    const uint32_t tid = ldu32(a.data + a.rec_off[i] + 4);
+    if (!any) first = tid;
+    down = down || (any && tid < last);
+    any = true;
+    last = tid;
+  }
+  a.order[c] = make_uint2(first, last);
+  if (down) atomicOr(a.flags, DEC_ERR_PAIR_ORDER);
+}
+
+// Across chunks (one CTA): chunk c's first eligible tid must be >= the last eligible tid of every chunk before it.
+__global__ void __launch_bounds__(1024) kd_pair_order_fold(const uint2* order, uint32_t n_chunks, uint32_t* flags) {
+  __shared__ uint32_t s_max[1024];
+  const uint32_t t = threadIdx.x;
+  const uint32_t per = (n_chunks + 1023) / 1024;
+  const uint32_t c0 = min(n_chunks, t * per), c1 = min(n_chunks, c0 + per);
+  uint32_t lmax = 0;
+  bool bad = false;
+  for (uint32_t c = c0; c < c1; ++c) {
+    const uint2 r = order[c];
+    bad = bad || r.x < lmax;
+    lmax = max(lmax, r.y);
+  }
+  s_max[t] = lmax;
+  __syncthreads();
+  uint32_t before = 0;
+  for (uint32_t k = 0; k < t; ++k) before = max(before, s_max[k]);
+  for (uint32_t c = c0; c < c1 && !bad; ++c) bad = order[c].x < before;
+  if (bad) atomicOr(flags, DEC_ERR_PAIR_ORDER);
 }
 
 __global__ void __launch_bounds__(256) kd_pair_insert(const PairArgs a) {

@@ -160,10 +160,10 @@ inline FilterRun filter_one_input(DeviceSession& session, const InputSpec& in, c
     const BgzfInput bi(bx, (uint32_t)h.header->names.size(), h.records_at, session.pool().size());
     cmb_bgzf_result br{};
     rc = cmb_decode_bgzf(ctx, &bi.in, &br);
+    uint64_t n_rec = 0, n_bytes = 0;
+    // the plan declines a stream whose mates the device cannot match in file order (cmb_pairs.cuh): the host loop takes it
+    if (rc == CMB_OK) rc = cmb_filter_plan(ctx, inverse ? 1 : 0, &n_rec, &n_bytes);
     if (rc == CMB_OK) {
-      uint64_t n_rec = 0, n_bytes = 0;
-      rc = cmb_filter_plan(ctx, inverse ? 1 : 0, &n_rec, &n_bytes);
-      if (rc) throw_device_error(ctx, rc);
       run.records.resize(n_bytes);
       rc = cmb_filter_fetch(ctx, run.records.data(), n_bytes);
       if (rc) throw_device_error(ctx, rc);
@@ -172,6 +172,7 @@ inline FilterRun filter_one_input(DeviceSession& session, const InputSpec& in, c
       return run;
     }
     if (rc != CMB_E_DECLINED) throw_device_error(ctx, rc);
+    if (getenv("CMB_PIPELINE_STATS")) fprintf(stderr, "#device_decode\tdeclined: %s\n", cmb_last_error(ctx));
   }
   // host fallback: the whole record stream in memory, then the reference's loop
   while (stream.fill(buf)) {

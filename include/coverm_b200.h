@@ -268,10 +268,12 @@ typedef struct cmb_bgzf_result {
 } cmb_bgzf_result;
 int cmb_submit_bgzf(cmb_ctx* ctx, const cmb_bgzf_input* in, cmb_bgzf_result* out);
 /* ---- `coverm filter` (src/bin/coverm.rs:408-472): ReferenceSortedBamFilter (src/filter.rs:36-234) as a record sink ----
- * cmb_decode_bgzf is cmb_submit_bgzf without the accumulation: the sample is inflated, its records located and reduced to
- * tuples, mates matched when the pair path of the filter applies -- and everything stays in device memory.  It needs
- * cmb_set_params (thresholds, flag includes; `filtering` = 1) but no reference and no cmb_begin_sample.
- * cmb_filter_plan then decides, per record, whether the filter returns it (inverse = `--inverse`, i.e. filter_out = false)
+ * cmb_decode_bgzf is cmb_submit_bgzf without the accumulation: the sample is inflated and its records located and reduced to
+ * tuples -- and everything stays in device memory.  It needs cmb_set_params (thresholds, flag includes; `filtering` = 1) but
+ * no reference and no cmb_begin_sample.
+ * cmb_filter_plan then matches mates when the pair path of the filter applies (CMB_E_DECLINED when the stream's proper-pair
+ * records are not sorted by reference id: the caller runs the filter on the host), decides, per record, whether the filter
+ * returns it (inverse = `--inverse`, i.e. filter_out = false)
  * and lays the returned records out in the reference's order -- file order, except that a passing pair comes out as
  * (stored first mate, second mate) at the second mate's position; cmb_filter_fetch copies them (each with its 4-byte
  * block_size, ready to be written into a BAM stream) to the caller.  CMB_E_NM: the reference would have panicked in nm(). */

@@ -14,7 +14,7 @@ occupies max(1, ceil(L / 32)) 32-element spans of the arena, 256 spans make a ch
 kept, in-shard record falls in it -- a +1 and a -1 that cancel still occupy it.  A chunk with at least D occupied spans is
 loaded whole (256 spans), any other one span by span.
 
-Pair filtering is not modelled (the pair path has its own parity tests): `filtering` must select the single-read filter.
+Pair filtering is not modelled here (tests/pair_reference.py models it): `filtering` must select the single-read filter.
 """
 import math
 
