@@ -497,7 +497,8 @@ int run_end_of_sample(cmb_ctx* c) {
     k.bin_base = r.d_bin_base; k.bins = r.d_bins; k.pool_cap = r.d_bins.cap; k.bin_hi = r.d_bin_hi;
     k.pairs = r.d_pairs; k.pair_count = (unsigned long long*)(c->d_counters + 4); k.pair_capacity = r.d_pairs.cap;
     k.want_csr = csr; k.all_rows = c->gene_mode ? 1u : 0u; k.error_flags = c->d_counters + 0;
-    const uint32_t grid = (c->n_local + K3_WARPS - 1) / K3_WARPS;  // one warp per contig
+    const uint32_t per_block = K3_WARPS * K3_CONTIGS_PER_WARP;
+    const uint32_t grid = (c->n_local + per_block - 1) / per_block;
     k3_finalize<<<grid, K3_THREADS, 0, c->stream>>>(k);
     CU_TRY(c, cudaGetLastError());
     c->timing.k3_launches = 1;

@@ -80,7 +80,7 @@ __global__ void __launch_bounds__(K1_THREADS, CMB_K1_MINBLOCKS) k1_filter_accumu
     ive = a.iv_begin[i + 1];
   }
 #if CMB_K1_PREFETCH
-  // K1 is latency-bound (a thread's loads form the chain columns -> intervals -> segment table -> REDs).  The segment of a
+  // A thread's loads form the chain columns -> intervals -> segment table -> REDs.  The segment of a
   // record depends on its tid only and its first aligned block on iv_begin only, so both are requested here, before the
   // filter arithmetic and the block-wide sortedness scan, and are in registers by the time the events are added.
   uint32_t pre_L = 0, pre_off0 = 0, pre_off1 = 0;
@@ -286,46 +286,46 @@ __global__ void __launch_bounds__(K1_THREADS, CMB_K1_MINBLOCKS) k1_filter_accumu
 
   const bool mine = keep && (uint32_t)tid >= a.tid_begin && (uint32_t)tid < a.tid_end;
   // ---- per-contig read counters (contig.rs:157-159, 204-211; genome.rs:173-174, 220-223, 677-682, 724-727)
+  //      One set of REDs per run of a warp's counted records with the same contig: records are sorted, so a warp's 32 records
+  //      fall in a few runs, and per-lane REDs would queue up in L2 on the same row.  Records that are not counted (filtered
+  //      out, other ranks' contigs) do not break a run.  A run starts at a counted lane whose contig differs from the previous
+  //      counted lane's, so unsorted input (ERR_UNSORTED) only splits a contig into more runs; the adds commute.
   {
-    const bool primary = !secondary && !supplementary;
-    const uint64_t c_rec = mine ? 1 : 0, c_pri = (mine && primary) ? 1 : 0, c_ns = (mine && !supplementary) ? 1 : 0;
-    const uint64_t c_edit = mine ? r.nm : 0, c_indel = mine ? (uint64_t)ins + r.del : 0;
-    double idn = 0.0;
-    if (mine && r.aligned > 0) idn = ((double)r.aligned - (double)r.nm) / (double)r.aligned;
-    const double id_pri = primary ? idn : 0.0, id_ns = !supplementary ? idn : 0.0;
     const uint32_t mine_mask = __ballot_sync(FULL, mine);
     if (mine_mask) {
-      const int leader = __ffs(mine_mask) - 1;
-      const int ltid = __shfl_sync(FULL, tid, leader);
-      const bool uniform = __all_sync(FULL, !mine || tid == ltid);
-      if (uniform) {
-        const uint64_t s_rec = warp_sum_u64(c_rec), s_pri = warp_sum_u64(c_pri), s_ns = warp_sum_u64(c_ns),
-                       s_edit = warp_sum_u64(c_edit), s_indel = warp_sum_u64(c_indel);
-        double s_idp = id_pri, s_idn = id_ns;
+      const bool primary = !secondary && !supplementary;
+      const uint32_t below = mine_mask & ((1u << lane) - 1);
+      const int prev_tid = __shfl_sync(FULL, tid, below ? 31 - __clz(below) : lane);  // the previous counted lane's
+      const uint32_t heads = __ballot_sync(FULL, mine && (!below || prev_tid != tid)) | 1u;  // lane 0 ends uncounted lanes
+      const uint32_t after = heads & ~((2u << lane) - 1);  // heads above this lane (2u << 31 == 0: none above lane 31)
+      const uint32_t run_end = after ? __ffs(after) - 1 : 32;  // one past the last lane of this lane's run
+      const uint32_t run = (run_end == 32 ? FULL : (1u << run_end) - 1) & ~((1u << lane) - 1);  // the run, seen from its head
+      uint64_t s_edit = mine ? r.nm : 0, s_indel = mine ? (uint64_t)ins + r.del : 0;  // a warp's sum may pass 2^32
+      double idn = 0.0;
+      if (mine && r.aligned > 0) idn = ((double)r.aligned - (double)r.nm) / (double)r.aligned;
+      double s_idp = primary ? idn : 0.0, s_idn = !supplementary ? idn : 0.0;
 #pragma unroll
-        for (int d = 16; d > 0; d >>= 1) {
-          s_idp += __shfl_xor_sync(FULL, s_idp, d);
-          s_idn += __shfl_xor_sync(FULL, s_idn, d);
+      for (uint32_t d = 1; d < 32; d <<= 1) {  // segmented: lane l ends up with the sums of lanes l .. run_end-1
+        const uint64_t oe = __shfl_down_sync(FULL, s_edit, d), oi = __shfl_down_sync(FULL, s_indel, d);
+        const double op = __shfl_down_sync(FULL, s_idp, d), on = __shfl_down_sync(FULL, s_idn, d);
+        if (lane + d < run_end) {
+          s_edit += oe;
+          s_indel += oi;
+          s_idp += op;
+          s_idn += on;
         }
-        if ((int)lane == leader) {
-          cmb_contig_stats* row = a.rows + ltid;
-          atomicAdd((unsigned long long*)&row->n_records, (unsigned long long)s_rec);
-          if (s_pri) atomicAdd((unsigned long long*)&row->n_primary, (unsigned long long)s_pri);
-          if (s_ns) atomicAdd((unsigned long long*)&row->n_nonsupp, (unsigned long long)s_ns);
-          if (s_edit) atomicAdd((unsigned long long*)&row->sum_edit, (unsigned long long)s_edit);
-          if (s_indel) atomicAdd((unsigned long long*)&row->sum_indel, (unsigned long long)s_indel);
-          if (s_idp != 0.0) atomicAdd(&row->sum_identity_primary, s_idp);
-          if (s_idn != 0.0) atomicAdd(&row->sum_identity_nonsupp, s_idn);
-        }
-      } else if (mine) {
+      }
+      const uint32_t s_rec = __popc(mine_mask & run), s_pri = __popc(__ballot_sync(FULL, mine && primary) & run),
+                     s_ns = __popc(__ballot_sync(FULL, mine && !supplementary) & run);
+      if (mine && (heads >> lane & 1)) {
         cmb_contig_stats* row = a.rows + tid;
-        atomicAdd((unsigned long long*)&row->n_records, 1ull);
-        if (c_pri) atomicAdd((unsigned long long*)&row->n_primary, 1ull);
-        if (c_ns) atomicAdd((unsigned long long*)&row->n_nonsupp, 1ull);
-        if (c_edit) atomicAdd((unsigned long long*)&row->sum_edit, (unsigned long long)c_edit);
-        if (c_indel) atomicAdd((unsigned long long*)&row->sum_indel, (unsigned long long)c_indel);
-        if (id_pri != 0.0) atomicAdd(&row->sum_identity_primary, id_pri);
-        if (id_ns != 0.0) atomicAdd(&row->sum_identity_nonsupp, id_ns);
+        atomicAdd((unsigned long long*)&row->n_records, (unsigned long long)s_rec);
+        if (s_pri) atomicAdd((unsigned long long*)&row->n_primary, (unsigned long long)s_pri);
+        if (s_ns) atomicAdd((unsigned long long*)&row->n_nonsupp, (unsigned long long)s_ns);
+        if (s_edit) atomicAdd((unsigned long long*)&row->sum_edit, (unsigned long long)s_edit);
+        if (s_indel) atomicAdd((unsigned long long*)&row->sum_indel, (unsigned long long)s_indel);
+        if (s_idp != 0.0) atomicAdd(&row->sum_identity_primary, s_idp);
+        if (s_idn != 0.0) atomicAdd(&row->sum_identity_nonsupp, s_idn);
       }
     }
   }
