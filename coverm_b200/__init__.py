@@ -104,7 +104,7 @@ class HostResult(C.Structure):
 DEVICE_SYMBOLS = ["cmb_abi_version", "cmb_create", "cmb_destroy", "cmb_last_error", "cmb_set_reference",
                   "cmb_set_params", "cmb_begin_sample", "cmb_acquire_batch", "cmb_submit_batch",
                   "cmb_submit_device_batch", "cmb_submit_bgzf", "cmb_decode_bgzf", "cmb_filter_plan", "cmb_filter_fetch", "cmb_set_genes",
-                  "cmb_fetch_gene_extras", "cmb_grow_buffers", "cmb_last_bgzf_batch", "cmb_end_sample", "cmb_comm_unique_id",
+                  "cmb_set_genes_range", "cmb_fetch_gene_extras", "cmb_grow_buffers", "cmb_last_bgzf_batch", "cmb_end_sample", "cmb_comm_unique_id",
                   "cmb_comm_init", "cmb_comm_init_local", "cmb_comm_destroy", "cmb_comm_allgather", "cmb_allgather_stats", "cmb_kept_tid_range", "cmb_fetch_pairs", "cmb_end_sample_device",
                   "cmb_get_timing", "cmb_stream", "cmb_host_alloc", "cmb_host_free", "cmb_nvtx_push", "cmb_nvtx_pop"]
 class Tuples(C.Structure):
@@ -187,6 +187,9 @@ def load_library(path=None):
     lib.cmb_end_sample.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]
     lib.cmb_fetch_pairs.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64]
     lib.cmb_set_genes.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(C.c_uint64), C.c_uint32, C.POINTER(Gene)]
+    if hasattr(lib, "cmb_set_genes_range"):  # libcoverm_b200 has it; the CPU emulator of the ABI used by tests may not
+        lib.cmb_set_genes_range.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(C.c_uint64), C.c_uint32, C.POINTER(Gene), C.c_uint32,
+                                            C.c_uint32]
     lib.cmb_fetch_gene_extras.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64)]
     lib.cmb_end_sample_device.argtypes = [C.c_void_p, C.POINTER(C.c_void_p)]
     lib.cmb_get_timing.argtypes = [C.c_void_p, C.POINTER(SampleTiming)]
@@ -371,14 +374,21 @@ class DeviceContext:
         self._check(self._lib.cmb_set_reference(self._h, self.n_contigs, lens.ctypes.data_as(C.POINTER(C.c_uint64)),
                                                 tid_begin, tid_end), "cmb_set_reference")
 
-    def set_genes(self, contig_lens, genes):
+    def set_genes(self, contig_lens, genes, tid_begin=None, tid_end=None):
         """Per-gene segments instead of contigs (cmb_set_genes): `genes` is a sequence of (tid, start, end) sorted by
-        (tid, start).  Result rows are then one per gene (one placeholder row when there are none)."""
+        (tid, start).  Result rows are then one per gene (one placeholder row when there are none).  With `tid_begin` /
+        `tid_end` (cmb_set_genes_range) only the records of those contigs count, and only their genes' rows are filled."""
         import numpy as np
         lens = np.ascontiguousarray(contig_lens, dtype=np.uint64)
         arr = (Gene * max(1, len(genes)))(*[Gene(*g) for g in genes])
-        self._check(self._lib.cmb_set_genes(self._h, len(lens), lens.ctypes.data_as(C.POINTER(C.c_uint64)), len(genes), arr),
-                    "cmb_set_genes")
+        lens_p = lens.ctypes.data_as(C.POINTER(C.c_uint64))
+        if tid_begin is None and tid_end is None:
+            self._check(self._lib.cmb_set_genes(self._h, len(lens), lens_p, len(genes), arr), "cmb_set_genes")
+        else:
+            tid_begin = 0 if tid_begin is None else tid_begin
+            tid_end = len(lens) if tid_end is None else tid_end
+            self._check(self._lib.cmb_set_genes_range(self._h, len(lens), lens_p, len(genes), arr, tid_begin, tid_end),
+                        "cmb_set_genes_range")
         self.n_contigs = max(1, len(genes))
         self.n_ref_contigs = len(lens)
 

@@ -210,6 +210,8 @@ struct cmb_ctx {
   uint32_t block_minmax_used = 0;
   bool gene_mode = false;
   uint32_t n_ref_contigs = 0;  // contigs of the BAM header (== n_contigs outside gene mode)
+  // gene mode: the contigs whose records this context counts (cmb_set_genes_range); tid_begin / tid_end are then its genes
+  uint32_t gene_tid_begin = 0, gene_tid_end = 0;
   CUtensorMap tmap{};
   bool arena_dirty = true;
   bool pool_dirty = false;  // a sample ended with an error: bins / bin_hi may hold counts (cmb_begin_sample zeroes them)
@@ -356,6 +358,10 @@ void free_reference(cmb_ctx* c) {
   c->gene_mode = false;
 }
 
+// Whether K1 has work: a context with no local segment has none, except in gene mode, where owned contigs without genes still
+// set contig_seen, count kept_primary and take part in the sortedness check.
+bool k1_active(const cmb_ctx* c) { return c->n_local || (c->gene_mode && c->gene_tid_begin < c->gene_tid_end); }
+
 int launch_k1(cmb_ctx* c, const cmb_read_batch& b, uint32_t n_records, uint32_t n_intervals, uint32_t excl_n = 0xffffffffu,
               const int32_t* mate = nullptr) {
   if (n_records == 0) return CMB_OK;
@@ -374,7 +380,9 @@ int launch_k1(cmb_ctx* c, const cmb_read_batch& b, uint32_t n_records, uint32_t 
   a.n = n_records;
   a.off_span = r.d_off_span; a.len = r.d_len;
   a.n_contigs = c->gene_mode ? c->n_ref_contigs : c->n_contigs; a.tid_begin = c->tid_begin; a.tid_end = c->tid_end;
+  a.seg_begin = c->tid_begin;
   if (c->gene_mode) {
+    a.tid_begin = c->gene_tid_begin; a.tid_end = c->gene_tid_end;
     a.gene_first = r.d_gene_first; a.gene_start = r.d_gene_start; a.gene_end = r.d_gene_end; a.gene_maxlen = r.d_gene_maxlen;
     a.contig_len = r.d_contig_len32; a.contig_seen = r.d_contig_seen; a.kept_primary = (unsigned long long*)(c->d_counters + 8);
     a.gene_bound = r.d_gene_bound;
@@ -692,9 +700,12 @@ void cmb_destroy(cmb_ctx* c) {
   delete c;  // frees every buffer (the device is still current)
 }
 
-int cmb_set_genes(cmb_ctx* c, uint32_t n_contigs, const uint64_t* contig_len, uint32_t n_genes, const cmb_gene* genes) {
+// cmb_set_genes (whole = true: every contig, every gene) and cmb_set_genes_range (the contigs [tid_begin, tid_end) and their genes)
+static int set_genes(cmb_ctx* c, uint32_t n_contigs, const uint64_t* contig_len, uint32_t n_genes, const cmb_gene* genes, uint32_t tid_begin,
+              uint32_t tid_end, bool whole) {
   if (!c || (!contig_len && n_contigs) || (!genes && n_genes)) return fail(c, CMB_E_ARG, "cmb_set_genes: null argument");
   if (c->in_sample) return fail(c, CMB_E_ARG, "cmb_set_genes: a sample is in progress");
+  if (tid_begin > tid_end || tid_end > n_contigs) return fail(c, CMB_E_ARG, "cmb_set_genes_range: bad contig range");
   std::vector<uint64_t> seg_len(std::max<uint32_t>(1, n_genes), 1);
   std::vector<uint32_t> first((size_t)n_contigs + 1, 0), gs(std::max<uint32_t>(1, n_genes)), ge(std::max<uint32_t>(1, n_genes)), maxlen(std::max<uint32_t>(1, n_contigs), 0), clen(std::max<uint32_t>(1, n_contigs), 0);
   for (uint32_t t = 0; t < n_contigs; ++t) {
@@ -714,17 +725,22 @@ int cmb_set_genes(cmb_ctx* c, uint32_t n_contigs, const uint64_t* contig_len, ui
   }
   for (uint32_t t = 0; t < n_contigs; ++t) first[t + 1] += first[t];
   // the arena, rows and histogram buffers are laid out over the genes exactly as over contigs (a placeholder segment keeps an
-  // empty gene set well-formed)
+  // empty gene set well-formed).  A contig range owns the genes of its contigs, [first[tid_begin], first[tid_end]); the range
+  // that ends with the last contig also owns the placeholder, so consecutive ranges partition the rows.
   const uint32_t n_seg = std::max<uint32_t>(1, n_genes);
-  int rc = cmb_set_reference(c, n_seg, seg_len.data(), 0, n_seg);
+  auto seg_cut = [&](uint32_t t) { return t == n_contigs ? n_seg : first[t]; };
+  const uint32_t g_begin = whole || tid_begin == 0 ? 0 : seg_cut(tid_begin), g_end = whole ? n_seg : seg_cut(tid_end);
+  int rc = cmb_set_reference(c, n_seg, seg_len.data(), g_begin, g_end);
   if (rc) return rc;
   c->gene_mode = true;
   c->n_ref_contigs = n_contigs;
+  c->gene_tid_begin = whole ? 0 : tid_begin;
+  c->gene_tid_end = whole ? n_contigs : tid_end;
   auto& r = c->ref;
   const size_t n_ctg = std::max<uint32_t>(1, n_contigs);
   if ((rc = r.d_gene_first.ensure(c, (size_t)n_contigs + 1)) || (rc = r.d_gene_start.ensure(c, n_seg)) || (rc = r.d_gene_end.ensure(c, n_seg)) ||
       (rc = r.d_gene_maxlen.ensure(c, n_ctg)) || (rc = r.d_contig_len32.ensure(c, n_ctg)) || (rc = r.d_contig_seen.ensure(c, n_ctg)) ||
-      (rc = r.d_gene_bound.ensure(c, n_seg)))
+      (rc = r.d_gene_bound.ensure(c, std::max<uint32_t>(1, c->n_local))))
     return rc;
   CU_TRY(c, cudaMemcpyAsync(r.d_gene_first, first.data(), 4ull * (n_contigs + 1), cudaMemcpyHostToDevice, c->stream));
   CU_TRY(c, cudaMemcpyAsync(r.d_gene_start, gs.data(), 4ull * n_seg, cudaMemcpyHostToDevice, c->stream));
@@ -733,6 +749,15 @@ int cmb_set_genes(cmb_ctx* c, uint32_t n_contigs, const uint64_t* contig_len, ui
   CU_TRY(c, cudaMemcpyAsync(r.d_contig_len32, clen.data(), 4 * n_ctg, cudaMemcpyHostToDevice, c->stream));
   CU_TRY(c, cudaStreamSynchronize(c->stream));
   return CMB_OK;
+}
+
+int cmb_set_genes(cmb_ctx* c, uint32_t n_contigs, const uint64_t* contig_len, uint32_t n_genes, const cmb_gene* genes) {
+  return set_genes(c, n_contigs, contig_len, n_genes, genes, 0, n_contigs, true);
+}
+
+int cmb_set_genes_range(cmb_ctx* c, uint32_t n_contigs, const uint64_t* contig_len, uint32_t n_genes, const cmb_gene* genes,
+                        uint32_t tid_begin, uint32_t tid_end) {
+  return set_genes(c, n_contigs, contig_len, n_genes, genes, tid_begin, tid_end, false);
 }
 
 int cmb_fetch_gene_extras(cmb_ctx* c, uint8_t* contig_seen, uint64_t* n_kept_primary) {
@@ -899,7 +924,7 @@ int cmb_submit_batch(cmb_ctx* c, uint32_t n_records, uint32_t n_intervals) {
   const uint32_t i = (c->next_batch + c->cfg.n_staging - c->n_acquired) % c->cfg.n_staging;  // oldest acquired batch
   c->n_acquired -= 1;
   if (n_records == 0) return CMB_OK;
-  if (c->n_local == 0) return CMB_OK;
+  if (!k1_active(c)) return CMB_OK;
   const cmb_read_batch& h = c->host_batch[i];
   const cmb_read_batch& d = c->dev_batch[i].ptr;
   CU_TRY(c, cudaSetDevice(c->device));
@@ -931,7 +956,7 @@ int cmb_submit_device_batch(cmb_ctx* c, const cmb_read_batch* dev, uint32_t n_re
   NvtxRange nvtx_fn("cmb_submit_device_batch: K1");
   if (!c || !dev) return fail(c, CMB_E_ARG, "cmb_submit_device_batch: null argument");
   if (!c->in_sample) return fail(c, CMB_E_ARG, "cmb_submit_device_batch: no sample in progress");
-  if (c->n_local == 0) return CMB_OK;
+  if (!k1_active(c)) return CMB_OK;
   CU_TRY(c, cudaSetDevice(c->device));
   // re-submitting the tuples of the last device decode (cmb_last_bgzf_batch) in pair mode: its mate table goes with it
   const bool is_last = c->dec.last_valid && (const void*)dev->tid == c->dec.d_tuple_slab;
@@ -954,7 +979,13 @@ int cmb_end_sample_device(cmb_ctx* c, const cmb_contig_stats** dev_stats) {
     int rc = run_end_of_sample(c);
     if (rc) return rc;
   } else {
-    for (int i = 2; i <= 5; ++i) CU_TRY(c, cudaEventRecord(c->ev[i], c->stream));
+    CU_TRY(c, cudaEventRecord(c->ev[2], c->stream));
+    if (c->block_minmax_used) {  // gene mode: owned contigs without genes still ran K1 (k1_active)
+      k1c_check_sorted<<<1, 1024, 0, c->stream>>>(c->d_block_minmax, c->block_minmax_used, c->d_counters + 0,
+                                                  c->have_xrange ? c->d_block_xrange.p : nullptr, c->d_counters + 6);
+      CU_TRY(c, cudaGetLastError());
+    }
+    for (int i = 3; i <= 5; ++i) CU_TRY(c, cudaEventRecord(c->ev[i], c->stream));
   }
   uint32_t counters[6];
   int rc = collect_errors_and_timing(c, counters);
@@ -1755,7 +1786,7 @@ int BgzfCall::extract() {
     out->n_launches += 5;
   }
   CU_TRY(c, cudaEventRecord(d.ev[4], c->stream));
-  if (c->n_local && !decode_only) {
+  if (k1_active(c) && !decode_only) {
     // records that start before excl_end_block are this rank's exclusive share of the stream (cmb_kept_tid_range)
     uint32_t excl_n = 0xffffffffu;
     if (in->ranged && in->excl_end_block < walk_end) {

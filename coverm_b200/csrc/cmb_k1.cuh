@@ -21,7 +21,9 @@ struct K1Args {
   // reference
   const uint32_t* off_span;  // [n_local+1]
   const uint32_t* len;       // [n_local]
-  uint32_t n_contigs, tid_begin, tid_end;
+  // the contigs [tid_begin, tid_end) this context owns; in gene mode seg_begin is the global number of its first local segment
+  // (gene), as the arena, gene_bound and the bin pool are laid out over the genes [seg_begin, seg_begin + n_local) only
+  uint32_t n_contigs, tid_begin, tid_end, seg_begin;
   // outputs
   int32_t* arena;
   uint32_t* span_bits;  // span occupancy bitmap: the bit of every span an event is added to (K2 loads only those spans)
@@ -39,9 +41,9 @@ struct K1Args {
   const uint32_t* gene_end;
   const uint32_t* gene_maxlen;  // [n_contigs] longest gene of the contig (bounds the backward search for overlaps)
   const uint32_t* contig_len;   // [n_contigs]
-  uint8_t* contig_seen;         // [n_contigs] a kept record mapped here (genes.rs:220-246)
-  unsigned long long* kept_primary;  // primaries among the kept records (ReadsMapped.num_mapped_reads, genes.rs:249-252)
-  uint32_t* gene_bound;         // [n_genes] records that may add events to the gene: bounds its depth (K1b's bin pool layout)
+  uint8_t* contig_seen;         // [n_contigs] a kept record of an owned contig mapped here (genes.rs:220-246)
+  unsigned long long* kept_primary;  // primaries among the kept records of owned contigs (ReadsMapped, genes.rs:249-252)
+  uint32_t* gene_bound;         // [n_local] records that may add events to the gene: bounds its depth (K1b's bin pool layout)
   // pair path: partner of each record (cmb_pairs.cuh, records in file order) or NULL = the host layout (completed pairs
   // only, stored first mate at the even index, its partner right after)
   const int32_t* mate;
@@ -229,8 +231,10 @@ __global__ void __launch_bounds__(K1_THREADS, CMB_K1_MINBLOCKS) k1_filter_accumu
   if (a.gene_first) {
     // ---- per-gene coverage (genes.rs:182-344, 467-552).  A gene's delta array is the contig's, cut to [start, end) with the
     //      running depth at `start` as its first element: exactly what clipping every aligned block to the gene gives.  Reads
-    //      are assigned to the genes that contain their leftmost position.
-    if (keep) {
+    //      are assigned to the genes that contain their leftmost position.  Under a contig shard (cmb_set_genes_range) only
+    //      records of the owned contigs count: all of their genes are local segments, rows keep the global gene number.
+    //      keep implies 0 <= tid < n_contigs, so one unsigned compare tests the range.
+    if (keep && (uint32_t)tid - a.tid_begin < a.tid_end - a.tid_begin) {
       const bool primary = !secondary && !supplementary;
       a.contig_seen[tid] = 1;
       if (primary) atomicAdd(a.kept_primary, 1ull);
@@ -259,7 +263,8 @@ __global__ void __launch_bounds__(K1_THREADS, CMB_K1_MINBLOCKS) k1_filter_accumu
         for (uint32_t g = lo; g < g1; ++g) {
           const uint32_t gsx = a.gene_start[g], gex = a.gene_end[g];
           if ((uint64_t)gsx >= max(ref_end, (uint64_t)(uint32_t)pos + 1)) break;  // genes are sorted by start
-          atomicAdd(a.gene_bound + g, 1u);  // every gene the record may add events to: bounds the gene's depth
+          const uint32_t lg = g - a.seg_begin;
+          atomicAdd(a.gene_bound + lg, 1u);  // every gene the record may add events to: bounds the gene's depth
           if ((uint32_t)pos >= gsx && (uint32_t)pos < gex) {  // read_starts.partition_point range (genes.rs:518-523)
             cmb_contig_stats* row = a.rows + g;
             atomicAdd((unsigned long long*)&row->n_records, 1ull);
@@ -274,7 +279,7 @@ __global__ void __launch_bounds__(K1_THREADS, CMB_K1_MINBLOCKS) k1_filter_accumu
             const uint64_t e = (uint64_t)(uint32_t)s + (uint32_t)a.iv_len[k];
             if (e <= gsx || (uint32_t)s >= gex) continue;  // no overlap
             const uint32_t cs = max((uint32_t)s, gsx) - gsx;
-            add_events(g, cs, e - gsx);  // e - gsx >= gene length: the block runs past the gene, no -1
+            add_events(lg, cs, e - gsx);  // e - gsx >= gene length: the block runs past the gene, no -1
           }
         }
       }

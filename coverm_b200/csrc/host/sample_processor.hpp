@@ -10,6 +10,11 @@
 #include "genes.hpp"
 #include "shard_range.hpp"
 
+// Referenced weakly: the host code also links against stand-ins of the device library that predate per-gene sharding (the CPU
+// emulator of the ABI).  With such a library a group run with --gff stops with an error; libcoverm_b200 always defines it.
+extern "C" int cmb_set_genes_range(cmb_ctx* ctx, uint32_t n_contigs, const uint64_t* contig_len, uint32_t n_genes, const cmb_gene* genes,
+                                   uint32_t tid_begin, uint32_t tid_end) __attribute__((weak));
+
 namespace cmbh {
 
 // NVTX range of a host-side stage (cmb_nvtx_push / cmb_nvtx_pop of the device library; no-ops without a profiler)
@@ -159,6 +164,7 @@ class DeviceSession {
       mine.n_primary = res.num_detected_primary_alignments;
       mine.counts_global = sh.counts_global ? 1 : 0;
       mine.n_pairs = sh.n_pairs;
+      mine.kept_primary = res.kept_primary;
       int32_t lo = INT32_MAX, hi = INT32_MIN;
       if (!sh.counts_global) cmb_kept_tid_range(ctx_, &lo, &hi);
       mine.min_tid = lo;
@@ -185,20 +191,23 @@ class DeviceSession {
       if (s.kind == 2) throw ExitError(s.code, s.message);
     }
     check_rank_order(all);
-    // ---- the gather of the path: every rank ends up with the complete per-contig table (+ histogram pairs)
+    // ---- the gather of the path: every rank ends up with the complete per-contig (gene mode: per-gene) table + histogram pairs
     const uint32_t n_ref = (uint32_t)res.hdr->names.size();
     std::vector<uint64_t> pair_base((size_t)group_n_ + 1, 0);
     for (int r = 0; r < group_n_; ++r) pair_base[(size_t)r + 1] = pair_base[(size_t)r] + all[(size_t)r].n_pairs;
     const bool csr = params.want & CMB_WANT_HIST_CSR;
     res.pairs.clear();
     if (csr) res.pairs.resize(pair_base[(size_t)group_n_]);
-    ensure_rows(n_ref);
-    if (group_nccl_) {
-      const int rc = cmb_allgather_stats(ctx_, sh.cuts.data(), csr ? pair_base.data() : nullptr, rows_buf_, csr ? res.pairs.data() : nullptr);
+    ensure_rows(res.genes ? std::max<uint32_t>(1, (uint32_t)res.genes->entries.size()) : n_ref);
+    if (res.genes && res.genes->entries.empty()) {
+      // no gene rows to report (every printed row is a gene's): nothing to gather
+    } else if (group_nccl_) {
+      const int rc = cmb_allgather_stats(ctx_, sh.row_cuts.data(), csr ? pair_base.data() : nullptr, rows_buf_, csr ? res.pairs.data() : nullptr);
       if (rc) throw_device_error(ctx_, rc);
     } else {
       gather_rows_through_host(sh, res, all, pair_base, csr);
     }
+    if (res.genes) gather_contig_seen(sh, res);
     res.rows = rows_buf_;
     fold_counters(all, res);
     res.timing.gather_s = now_s() - t_g0;
@@ -209,7 +218,8 @@ class DeviceSession {
 
  private:
   struct ShardState {
-    std::vector<uint32_t> cuts;
+    std::vector<uint32_t> cuts;      // contig (tid) cuts: rank r owns the records of contigs [cuts[r], cuts[r+1])
+    std::vector<uint32_t> row_cuts;  // the ranks' row ranges: == cuts, or in gene mode the genes of those contigs
     bool counts_global = false;  // this rank read the whole file (host decode): its counters cover every record
     uint64_t n_pairs = 0;
   };
@@ -217,6 +227,7 @@ class DeviceSession {
     int32_t kind;       // 0 fine, 1 Panic, 2 ExitError
     int32_t code;
     uint64_t n_records, n_primary, n_pairs;
+    uint64_t kept_primary;  // gene mode: primaries among the kept records of the rank's own contigs
     int32_t min_tid, max_tid;
     uint32_t counts_global, reserved;
     char message[208];
@@ -234,7 +245,10 @@ class DeviceSession {
     }
   }
   // The whole-file counters: taken from the first rank that had to read the whole file, else summed over the ranks' owned records.
+  // kept_primary is always summed: whichever part of the file a rank read, K1 counted only its own contigs' records.
   static void fold_counters(const std::vector<RankSummary>& all, SampleResult& res) {
+    res.kept_primary = 0;
+    for (const RankSummary& s : all) res.kept_primary += s.kept_primary;
     res.n_records = res.num_detected_primary_alignments = 0;
     for (const RankSummary& s : all) {
       if (s.counts_global) {
@@ -273,10 +287,11 @@ class DeviceSession {
     const int N = group_n_, me = group_rank_;
     size_t max_rows = 0, max_pairs = 0;
     for (int r = 0; r < N; ++r) {
-      max_rows = std::max<size_t>(max_rows, sh.cuts[(size_t)r + 1] - sh.cuts[(size_t)r]);
+      max_rows = std::max<size_t>(max_rows, sh.row_cuts[(size_t)r + 1] - sh.row_cuts[(size_t)r]);
       max_pairs = std::max<size_t>(max_pairs, all[(size_t)r].n_pairs);
     }
-    const uint32_t b = sh.cuts[(size_t)me], e = sh.cuts[(size_t)me + 1];
+    const std::vector<uint32_t>& cuts = sh.row_cuts;
+    const uint32_t b = cuts[(size_t)me], e = cuts[(size_t)me + 1];
     if (max_rows) {
       std::vector<cmb_contig_stats> send(max_rows), recv(max_rows * (size_t)N);
       for (uint32_t t = b; t < e; ++t) {
@@ -285,7 +300,7 @@ class DeviceSession {
       }
       group_allgather(send.data(), recv.data(), max_rows * sizeof(cmb_contig_stats));
       for (int r = 0; r < N; ++r)
-        for (uint32_t t = sh.cuts[(size_t)r]; t < sh.cuts[(size_t)r + 1]; ++t) rows_buf_[t] = recv[(size_t)r * max_rows + (t - sh.cuts[(size_t)r])];
+        for (uint32_t t = cuts[(size_t)r]; t < cuts[(size_t)r + 1]; ++t) rows_buf_[t] = recv[(size_t)r * max_rows + (t - cuts[(size_t)r])];
     }
     if (csr && max_pairs) {
       std::vector<cmb_hist_pair> send(max_pairs), recv(max_pairs * (size_t)N);
@@ -295,6 +310,20 @@ class DeviceSession {
         std::copy(recv.begin() + (ptrdiff_t)((size_t)r * max_pairs), recv.begin() + (ptrdiff_t)((size_t)r * max_pairs + all[(size_t)r].n_pairs),
                   res.pairs.begin() + (ptrdiff_t)pair_base[(size_t)r]);
     }
+  }
+
+  // Gene mode: each rank's contig_seen covers its own contigs only; the ranks' slices, padded to the largest, complete it.
+  void gather_contig_seen(const ShardState& sh, SampleResult& res) {
+    const int N = group_n_, me = group_rank_;
+    size_t max_tids = 0;
+    for (int r = 0; r < N; ++r) max_tids = std::max<size_t>(max_tids, sh.cuts[(size_t)r + 1] - sh.cuts[(size_t)r]);
+    if (!max_tids) return;
+    std::vector<uint8_t> send(max_tids, 0), recv(max_tids * (size_t)N);
+    std::copy(res.contig_seen.begin() + sh.cuts[(size_t)me], res.contig_seen.begin() + sh.cuts[(size_t)me + 1], send.begin());
+    group_allgather(send.data(), recv.data(), max_tids);
+    for (int r = 0; r < N; ++r)
+      std::copy(recv.begin() + (ptrdiff_t)((size_t)r * max_tids), recv.begin() + (ptrdiff_t)((size_t)r * max_tids + sh.cuts[(size_t)r + 1] - sh.cuts[(size_t)r]),
+                res.contig_seen.begin() + sh.cuts[(size_t)r]);
   }
 
   // cmb_set_params; whether the parameters filter read pairs
@@ -393,29 +422,48 @@ class DeviceSession {
     void reference() {
       sb = std::min<uint32_t>(s.shard_begin_, n_ref);
       se = std::min<uint32_t>(s.shard_end_, n_ref);
-      if (shard) {
+      if (shard && !s.gene_defs_) {
         shard->cuts = tid_cuts_by_length(res.hdr->lens, s.group_n_);
+        shard->row_cuts = shard->cuts;
         sb = shard->cuts[(size_t)s.group_rank_];
         se = shard->cuts[(size_t)s.group_rank_ + 1];
       }
-      res.timing.tid_begin = sb;
-      res.timing.tid_end = se;
       n_rows = n_ref;
       int rc;
       if (s.gene_defs_) {
-        if (shard) throw ExitError(1, "--gff is not available together with --gpus (per-gene coverage runs on one GPU)");
-        if (!s.gene_cache_ || res.hdr->lens != s.ref_lens_ || res.hdr->names != s.gene_cache_names_) {
+        const bool resolve = !s.gene_cache_ || res.hdr->lens != s.ref_lens_ || res.hdr->names != s.gene_cache_names_;
+        if (resolve) {
           s.gene_cache_ = std::make_shared<ResolvedGenes>(resolve_genes_against_header(*s.gene_defs_, *res.hdr, s.gene_namer_));
           s.gene_cache_names_ = res.hdr->names;
-          const auto& entries = s.gene_cache_->entries;
+        }
+        const auto& entries = s.gene_cache_->entries;
+        n_rows = std::max<uint32_t>(1, (uint32_t)entries.size());
+        if (shard) {  // contigs cut by their genes' padded bases; each rank owns the genes of its contigs
+          std::vector<uint32_t> seg_tid(entries.size());
+          std::vector<uint64_t> seg_len(entries.size());
+          for (size_t g = 0; g < entries.size(); ++g) {
+            seg_tid[g] = entries[g].tid;
+            seg_len[g] = entries[g].end - entries[g].start;
+          }
+          shard->cuts = tid_cuts_by_length(padded_gene_bases(n_ref, seg_tid, seg_len), s.group_n_);
+          shard->row_cuts = gene_row_cuts(shard->cuts, s.gene_cache_->first_of_tid, n_rows);
+          sb = shard->cuts[(size_t)s.group_rank_];
+          se = shard->cuts[(size_t)s.group_rank_ + 1];
+        }
+        // the device's genes depend on the header and, in a group, on this rank's contig range
+        if (resolve || (shard != nullptr) != s.gene_ranged_ || (shard && (sb != s.gene_sb_ || se != s.gene_se_))) {
+          if (shard && !cmb_set_genes_range) throw ExitError(1, "this device library has no cmb_set_genes_range: --gff needs it over several ranks");
           std::vector<cmb_gene> genes(entries.size());
           for (size_t g = 0; g < genes.size(); ++g) genes[g] = cmb_gene{entries[g].tid, entries[g].start, entries[g].end};
-          rc = cmb_set_genes(s.ctx_, n_ref, res.hdr->lens.data(), (uint32_t)genes.size(), genes.data());
+          rc = shard ? cmb_set_genes_range(s.ctx_, n_ref, res.hdr->lens.data(), (uint32_t)genes.size(), genes.data(), sb, se)
+                     : cmb_set_genes(s.ctx_, n_ref, res.hdr->lens.data(), (uint32_t)genes.size(), genes.data());
           if (rc) throw_device_error(s.ctx_, rc);
           s.ref_lens_ = res.hdr->lens;
+          s.gene_ranged_ = shard != nullptr;
+          s.gene_sb_ = sb;
+          s.gene_se_ = se;
         }
         res.genes = s.gene_cache_;
-        n_rows = std::max<uint32_t>(1, (uint32_t)s.gene_cache_->entries.size());
       } else if (res.hdr->lens != s.ref_lens_ || sb != s.ref_sb_ || se != s.ref_se_) {
         s.ref_sb_ = sb;
         s.ref_se_ = se;
@@ -423,6 +471,8 @@ class DeviceSession {
         if (rc) throw_device_error(s.ctx_, rc);
         s.ref_lens_ = res.hdr->lens;
       }
+      res.timing.tid_begin = sb;
+      res.timing.tid_end = se;
       rc = cmb_begin_sample(s.ctx_);
       if (rc) throw_device_error(s.ctx_, rc);
     }
@@ -697,6 +747,8 @@ class DeviceSession {
   const GenomeNamer* gene_namer_ = nullptr;
   std::shared_ptr<ResolvedGenes> gene_cache_;
   std::vector<std::string> gene_cache_names_;
+  bool gene_ranged_ = false;  // the device holds the genes of the contigs [gene_sb_, gene_se_) (cmb_set_genes_range), else all
+  uint32_t gene_sb_ = 0, gene_se_ = 0;
   // group (multi-GPU contig sharding)
   int group_rank_ = 0, group_n_ = 1;
   bool group_nccl_ = false, every_rank_prints_ = false;

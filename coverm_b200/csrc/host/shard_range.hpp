@@ -35,6 +35,30 @@ inline std::vector<uint32_t> tid_cuts_by_length(const std::vector<uint64_t>& len
   return cut;
 }
 
+// Per-gene coverage (--gff): a contig's share of the work is its genes' arena, every gene padded to whole 32-base spans (the
+// device lays a rank's arena out over the genes of its contigs, cmb_set_genes_range).  seg_tid / seg_len: contig and length of
+// each gene.  Cutting these weights with tid_cuts_by_length keeps the cuts on contig boundaries: a contig's genes never split
+// across ranks, and the block-range search by tid is the one of contig mode.
+inline std::vector<uint64_t> padded_gene_bases(size_t n_ref, const std::vector<uint32_t>& seg_tid, const std::vector<uint64_t>& seg_len) {
+  constexpr uint64_t SPAN = 32;
+  std::vector<uint64_t> w(n_ref, 0);
+  for (size_t g = 0; g < seg_tid.size(); ++g) w[seg_tid[g]] += std::max<uint64_t>(1, (seg_len[g] + SPAN - 1) / SPAN) * SPAN;
+  return w;
+}
+
+// The row cuts of gene mode: rank r's rows are the genes of its contigs, [first_of_tid[cut[r]], first_of_tid[cut[r+1]]), and
+// the rank whose range ends with the last contig also holds the placeholder row of an empty gene set (n_rows = max(1, genes)).
+// The same rule as cmb_set_genes_range's, so these are the cuts cmb_allgather_stats checks against each rank's context.
+inline std::vector<uint32_t> gene_row_cuts(const std::vector<uint32_t>& tid_cuts, const std::vector<uint32_t>& first_of_tid, uint32_t n_rows) {
+  const uint32_t n_ref = (uint32_t)first_of_tid.size() - 1;
+  std::vector<uint32_t> rc(tid_cuts.size());
+  for (size_t r = 0; r < tid_cuts.size(); ++r) {
+    const uint32_t t = tid_cuts[r];
+    rc[r] = t == 0 && r == 0 ? 0 : t == n_ref ? n_rows : first_of_tid[t];
+  }
+  return rc;
+}
+
 struct BlockRange {
   uint32_t walk_begin = 0, walk_end = 0;  // records starting in blocks [walk_begin, walk_end) are this rank's to decode
   uint64_t records_at = 0;                // uncompressed offset of the first record that starts in walk_begin

@@ -196,6 +196,15 @@ typedef struct cmb_gene {
   uint32_t end;
 } cmb_gene;
 int cmb_set_genes(cmb_ctx* ctx, uint32_t n_contigs, const uint64_t* contig_len, uint32_t n_genes, const cmb_gene* genes);
+/* Per-gene coverage over a contig shard (multi-GPU): like cmb_set_genes, but this context counts only the records of the
+ * contigs [tid_begin, tid_end), and its arena holds only their genes, [gene_first[tid_begin], gene_first[tid_end]) with
+ * gene_first[t] = genes on contigs before t (the range that ends at n_contigs also holds the placeholder row of an empty gene
+ * set).  Rows keep their global gene numbers; rows outside the range stay zero.  contig_seen and *n_kept_primary
+ * (cmb_fetch_gene_extras) cover the owned contigs only, so the ranks' values OR / add up to the whole sample's.  Consecutive
+ * contig ranges give consecutive gene ranges: their bounds are the `tid_cuts` of cmb_allgather_stats in gene mode.
+ * cmb_set_genes is the same call over [0, n_contigs). */
+int cmb_set_genes_range(cmb_ctx* ctx, uint32_t n_contigs, const uint64_t* contig_len, uint32_t n_genes, const cmb_gene* genes,
+                        uint32_t tid_begin, uint32_t tid_end);
 /* After cmb_end_sample in gene mode: contig_seen[tid] = 1 when a record that passed every filter mapped to contig tid (its
  * genes are reported through the estimators, the others as zero-coverage entries, genes.rs:434-465); *n_kept_primary =
  * primary alignments among those records (ReadsMapped.num_mapped_reads, genes.rs:249-252). */
