@@ -1,12 +1,17 @@
 // libcoverm_b200 — device side: hand-written sm_90a kernels + the C ABI of include/coverm_b200.h.
 //
 // Data layout in HBM (one cmb_ctx = one GPU = one contig shard):
-//   arena        i32[arena_elems]   all contigs' `ups_and_downs` (contig.rs:144-145) back to back; every contig
+//   arena        i32[arena_elems]   all segments' `ups_and_downs` (contig.rs:144-145) back to back; every segment
 //                                   starts on a 32-element span boundary (SPAN), the arena is a whole number of
-//                                   8192-element chunks (CHUNK).  4 B per reference base.
+//                                   8192-element chunks (CHUNK).  4 B per reference base.  Gene mode adds its events
+//                                   here; contig mode only uses its coordinates (element g of the arena).
 //   span_bits    u32[arena_elems/1024]  one bit per 32-element span: set by K1 for every event it adds, read (and, when
-//                                   cleaning as it goes, cleared) by K2, which loads only the spans named there.
+//                                   cleaning as it goes, cleared) by K2, which works only on the spans named there.
 //                                   Zero exactly when the arena is (zeroed together; K2 cleans both).
+//   events       u64[2 * intervals of the sample]  contig mode, K1: interval k's start / end as (g << 1) | sign
+//   word_count   u32[arena_elems/1024]  contig mode, K1: events per bitmap word; K1e counts them back down to zero
+//   word_off     u32[arena_elems/1024 + 1]  contig mode, K1b: exclusive scan of word_count
+//   buckets      u16[events + 8]    contig mode, K1e: (g % 1024) | sign << 10 of every event, by word (word_off)
 //   off_span     u32[n_local+1]     padded contig offsets in span units; len u32[n_local]
 //   chunk_first  u32[n_chunks+1]    contig containing the first span of each chunk
 //   tail_sum     i32[n_chunks]      K1: sum of the deltas of the contig that continues past the chunk end
@@ -19,16 +24,20 @@
 // Kernels (all HBM-bound integer work, no tensor cores):
 //   K1  k1_filter_accumulate  one thread per record: FlagFilter + ReferenceSortedBamFilter predicates
 //                             (lib.rs:59-79, filter.rs:243-336), per-contig read counters (contig.rs:157-211),
-//                             +1/-1 delta REDs into the arena (contig.rs:166-202), chunk tail sums.
-//   K1b k1b_local/apply       segmented scan of the per-chunk tail sums -> carry_in (so K2 needs no look-back), and the
-//                             exclusive scan of the contigs' bin counts -> bin_base, in the same two launches.
+//                             +1/-1 delta events (contig.rs:166-202): plain stores to the event list (contig mode) or REDs
+//                             into the arena (gene mode); span bits, per-word event counts, chunk tail sums.
+//   K1b k1b_local/apply       segmented scan of the per-chunk tail sums -> carry_in (so K2 needs no look-back), the
+//                             exclusive scans of the contigs' bin counts -> bin_base and of the word counts -> word_off, in
+//                             the same two launches.
+//   K1e k1e_bucket_events     contig mode: the event list bucketed by bitmap word, 2 B per event.
 //   K2  k2_scan_reduce        persistent warps, a warp per chunk, work only for the spans that hold events (slots, 32 per
 //                             round): 32-row TMA boxes (cp.async.bulk.tensor, 128B swizzle) + mbarrier for chunks with many
-//                             non-empty spans, cp.async of just the non-empty 128-B rows for the others; warp-shuffle
+//                             non-empty spans, cp.async of just the non-empty 128-B rows for the others (gene mode); in
+//                             contig mode each round's rows are built in shared memory from its word buckets; warp-shuffle
 //                             segmented scan of the slot totals, the event-free stretches between slots closed as one run
 //                             each, then every O(L) reduction of EST:366-502 in one pass: sum/covered over the end-trimmed window,
 //                             covered over the full contig, window depth histogram as REDs into the contig's bins;
-//                             optionally re-zeroes the arena as it goes.
+//                             optionally re-zeroes the arena (gene mode) and the span bitmap as it goes.
 //   K3  k3_finalize           per contig: walk its bins, trimmed-mean walk (EST:598-642) and the variance sums
 //                             (EST:790-805) in integers; optional CSR histogram output.
 //   KD* kd_inflate ...        device-side BAM decode behind cmb_submit_bgzf (cmb_decode.cuh): BGZF inflate, record chain,
@@ -181,6 +190,7 @@ struct cmb_ctx {
   struct Reference {  // the buffers that live as long as one reference (cmb_set_reference / cmb_set_genes)
     Buf<int32_t> d_arena;
     Buf<uint32_t> d_span_bits;
+    Buf<uint32_t> d_word_count, d_word_off, d_word_block_sum;  // contig mode: events per bitmap word, their scan (K1b)
     Buf<uint32_t> d_off_span, d_len, d_chunk_first;
     Buf<int32_t> d_tail_sum, d_carry_in;
     Buf<int2> d_block_agg;
@@ -196,7 +206,10 @@ struct cmb_ctx {
   } ref;
   Buf<uint32_t> d_counters;  // 16 words: [0] error flags, [4..5] pair_count (u64),
                              // [6..7] kept tid range of the exclusive records (K1Args::kept_range), [8..9] gene mode
-                             // kept primaries (u64), [10..11] K2 spans loaded / chunks loaded whole
+                             // kept primaries (u64), [10..12] K2 spans loaded / chunks loaded whole / bucket entries read
+  // contig mode: the sample's event list (K1, one entry pair per interval) and its events bucketed by word (K1e); grow-only
+  Buf<ulonglong2> d_events;
+  Buf<uint16_t> d_buckets;
   uint32_t kept_range[2] = {0, 0};  // host copy after cmb_end_sample*
   // multi-GPU (cmb_comm_*): one NCCL communicator per ctx, collectives on the ctx stream
   ncclComm_t comm = nullptr;
@@ -365,6 +378,7 @@ bool k1_active(const cmb_ctx* c) { return c->n_local || (c->gene_mode && c->gene
 int launch_k1(cmb_ctx* c, const cmb_read_batch& b, uint32_t n_records, uint32_t n_intervals, uint32_t excl_n = 0xffffffffu,
               const int32_t* mate = nullptr) {
   if (n_records == 0) return CMB_OK;
+  int rc_ = CMB_OK;
   const uint32_t blocks = (n_records + K1_THREADS - 1) / K1_THREADS;
   if (c->block_minmax_used + blocks > c->d_block_minmax.cap) {
     // grow (rare): allocate larger arrays and copy what is there
@@ -373,6 +387,12 @@ int launch_k1(cmb_ctx* c, const cmb_read_batch& b, uint32_t n_records, uint32_t 
     if (int rc = c->d_block_xrange.grow_keep(c, c->block_minmax_used, ncap, c->stream)) return rc;
   }
   const auto& r = c->ref;
+  if (!c->gene_mode) {  // the event list holds the sample's intervals so far: grow it, keeping the earlier batches' entries
+    const uint64_t need = c->n_intervals + n_intervals;
+    if (2 * need > 0xffffffffull)  // word_off and the buckets count events in u32
+      return fail(c, CMB_E_CAPACITY, "more than 2^31 - 1 aligned blocks in one sample; split the input across more GPUs");
+    if (c->d_events.cap < need && (rc_ = c->d_events.grow_keep(c, c->n_intervals, with_slack(need), c->stream))) return rc_;
+  }
   K1Args a{};
   a.tid = b.tid; a.pos = b.pos; a.flag = b.flag; a.mapq = b.mapq; a.nm_state = b.nm_state; a.nm = b.nm;
   a.l_seq = b.l_seq; a.aligned = b.aligned; a.del = b.del; a.ins = b.ins; a.iv_begin = b.iv_begin;
@@ -388,6 +408,9 @@ int launch_k1(cmb_ctx* c, const cmb_read_batch& b, uint32_t n_records, uint32_t 
     a.gene_bound = r.d_gene_bound;
   }
   a.arena = r.d_arena; a.span_bits = r.d_span_bits; a.tail_sum = r.d_tail_sum; a.rows = r.d_rows;
+  if (!c->gene_mode) {
+    a.events = c->d_events; a.iv_base = c->n_intervals; a.n_iv = n_intervals; a.word_count = r.d_word_count;
+  }
   a.block_minmax = c->d_block_minmax + c->block_minmax_used;
   a.error_flags = c->d_counters + 0;
   a.block_xrange = c->comm_size > 1 || excl_n != 0xffffffffu ? c->d_block_xrange + c->block_minmax_used : nullptr;
@@ -415,27 +438,28 @@ int launch_k1(cmb_ctx* c, const cmb_read_batch& b, uint32_t n_records, uint32_t 
   return CMB_OK;
 }
 
-// CTAs of k2_scan_reduce<HIST, CLEAN> that fit on one SM (K2 is persistent: it launches that many per SM)
-template <bool HIST, bool CLEAN>
+// CTAs of k2_scan_reduce<HIST, CLEAN, BUCKETS> that fit on one SM (K2 is persistent: it launches that many per SM)
+template <bool HIST, bool CLEAN, bool BUCKETS>
 int k2_blocks_per_sm(cmb_ctx* c, int* occ) {
-  auto kern = k2_scan_reduce<HIST, CLEAN>;
-  CU_TRY(c, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)K2_SMEM_BYTES));
+  auto kern = k2_scan_reduce<HIST, CLEAN, BUCKETS>;
+  constexpr uint32_t smem = k2_smem_bytes<BUCKETS>();
+  CU_TRY(c, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   *occ = 0;
-  CU_TRY(c, cudaOccupancyMaxActiveBlocksPerMultiprocessor(occ, kern, (int)K2_THREADS, K2_SMEM_BYTES));
+  CU_TRY(c, cudaOccupancyMaxActiveBlocksPerMultiprocessor(occ, kern, (int)K2_THREADS, smem));
   if (*occ < 1) return fail(c, CMB_E_CUDA, "k2_scan_reduce does not fit on an SM");
   return CMB_OK;
 }
 
-template <bool HIST, bool CLEAN>
+template <bool HIST, bool CLEAN, bool BUCKETS>
 int launch_k2_variant(cmb_ctx* c, const K2Args& a) {
   int occ = 0;
-  if (int rc = k2_blocks_per_sm<HIST, CLEAN>(c, &occ)) return rc;
+  if (int rc = k2_blocks_per_sm<HIST, CLEAN, BUCKETS>(c, &occ)) return rc;
   // a warp per chunk: no more CTAs than it takes to give every chunk its own warp
   const uint32_t grid = std::min<uint32_t>((c->n_chunks + K2_WARPS - 1) / K2_WARPS, (uint32_t)(occ * c->sm_count));
   if (getenv("CMB_PIPELINE_STATS"))
-    fprintf(stderr, "#k2_grid\tgrid=%u\tblocks_per_sm=%d\tsms=%d\thist=%d\tclean=%d\twarps=%u\n", grid, occ, c->sm_count, (int)HIST,
-            (int)CLEAN, grid * K2_WARPS);
-  k2_scan_reduce<HIST, CLEAN><<<grid, K2_THREADS, K2_SMEM_BYTES, c->stream>>>(c->tmap, a);
+    fprintf(stderr, "#k2_grid\tgrid=%u\tblocks_per_sm=%d\tsms=%d\thist=%d\tclean=%d\tbuckets=%d\twarps=%u\n", grid, occ, c->sm_count,
+            (int)HIST, (int)CLEAN, (int)BUCKETS, grid * K2_WARPS);
+  k2_scan_reduce<HIST, CLEAN, BUCKETS><<<grid, K2_THREADS, k2_smem_bytes<BUCKETS>(), c->stream>>>(c->tmap, a);
   CU_TRY(c, cudaGetLastError());
   return CMB_OK;
 }
@@ -467,11 +491,24 @@ int run_end_of_sample(cmb_ctx* c) {
     g.len = r.d_len; g.rows = r.d_rows + c->tid_begin; g.gene_bound = c->gene_mode ? r.d_gene_bound.p : nullptr;
     g.n_seg = c->n_local; g.excl = excl; g.bin_base = r.d_bin_base; g.block_sum = r.d_bin_block_sum;
     g.n_blocks = hist ? c->n_local / K1B_BLOCK + 1 : 0;  // n_local + 1 entries
-    const uint32_t blocks = (c->n_chunks + K1B_BLOCK - 1) / K1B_BLOCK + g.n_blocks;
-    k1b_local<<<blocks, K1B_THREADS, 0, c->stream>>>(r.d_tail_sum, r.d_chunk_first, r.d_off_span, c->n_chunks, r.d_carry_in, r.d_block_agg, g);
+    K1bWords wd{};
+    wd.count = r.d_word_count; wd.off = r.d_word_off; wd.block_sum = r.d_word_block_sum; wd.n_words = c->n_chunks * K2_WARPS;
+    wd.n_blocks = c->gene_mode ? 0 : wd.n_words / K1B_BLOCK + 1;  // n_words + 1 entries
+    const uint32_t blocks = (c->n_chunks + K1B_BLOCK - 1) / K1B_BLOCK + g.n_blocks + wd.n_blocks;
+    k1b_local<<<blocks, K1B_THREADS, 0, c->stream>>>(r.d_tail_sum, r.d_chunk_first, r.d_off_span, c->n_chunks, r.d_carry_in, r.d_block_agg, g, wd);
     CU_TRY(c, cudaGetLastError());
-    k1b_apply<<<blocks, K1B_THREADS, 0, c->stream>>>(r.d_tail_sum, r.d_block_agg, c->n_chunks, r.d_carry_in, g);
+    k1b_apply<<<blocks, K1B_THREADS, 0, c->stream>>>(r.d_tail_sum, r.d_block_agg, c->n_chunks, r.d_carry_in, g, wd);
     CU_TRY(c, cudaGetLastError());
+  }
+  if (!c->gene_mode) {  // K1e: the event list by bitmap word (K2 reads 8 entries past the last event at most)
+    const uint64_t n_events = 2 * c->n_intervals;
+    if (int rc = c->d_buckets.ensure(c, n_events + 8, with_slack(n_events + 8))) return rc;
+    if (c->n_intervals) {
+      const uint64_t blocks = (c->n_intervals + K1E_THREADS - 1) / K1E_THREADS;
+      k1e_bucket_events<<<(uint32_t)blocks, K1E_THREADS, 0, c->stream>>>(c->d_events, c->n_intervals, r.d_word_off, r.d_word_count, c->d_buckets);
+      CU_TRY(c, cudaGetLastError());
+      c->timing.k1_launches += 1;
+    }
   }
   if (hist && !small_hist()) {
     // Contig mode: a contig's bins are its read count + 1, and the records submitted bound the read counts together.  Gene
@@ -487,12 +524,19 @@ int run_end_of_sample(cmb_ctx* c) {
   a.off_span = r.d_off_span; a.len = r.d_len; a.chunk_first = r.d_chunk_first; a.carry_in = r.d_carry_in;
   a.rows = r.d_rows; a.tid_begin = c->tid_begin; a.n_local = c->n_local; a.n_chunks = c->n_chunks; a.excl = excl;
   a.arena = r.d_arena; a.span_bits = r.d_span_bits; a.load_stats = c->d_counters + 10;
+  a.word_off = r.d_word_off; a.buckets = c->d_buckets;
   a.bin_base = r.d_bin_base; a.bins = r.d_bins; a.pool_cap = r.d_bins.cap; a.bin_hi = r.d_bin_hi;
   a.error_flags = c->d_counters + 0;
   CU_TRY(c, cudaEventRecord(c->ev[3], c->stream));
   int rc;
-  if (hist) rc = c->clean_as_you_go ? launch_k2_variant<true, true>(c, a) : launch_k2_variant<true, false>(c, a);
-  else rc = c->clean_as_you_go ? launch_k2_variant<false, true>(c, a) : launch_k2_variant<false, false>(c, a);
+  const bool clean = c->clean_as_you_go;
+  if (!c->gene_mode) {  // contig mode: rows from the word buckets
+    if (hist) rc = clean ? launch_k2_variant<true, true, true>(c, a) : launch_k2_variant<true, false, true>(c, a);
+    else rc = clean ? launch_k2_variant<false, true, true>(c, a) : launch_k2_variant<false, false, true>(c, a);
+  } else {  // gene mode: rows from the arena
+    if (hist) rc = clean ? launch_k2_variant<true, true, false>(c, a) : launch_k2_variant<true, false, false>(c, a);
+    else rc = clean ? launch_k2_variant<false, true, false>(c, a) : launch_k2_variant<false, false, false>(c, a);
+  }
   if (rc) return rc;
   c->timing.k2_launches = 1;
   c->arena_dirty = !c->clean_as_you_go;
@@ -516,7 +560,7 @@ int run_end_of_sample(cmb_ctx* c) {
 }
 
 int collect_errors_and_timing(cmb_ctx* c, uint32_t* counters_out) {
-  uint32_t h[12];
+  uint32_t h[13];
   CU_TRY(c, cudaMemcpyAsync(h, c->d_counters, sizeof h, cudaMemcpyDeviceToHost, c->stream));
   CU_TRY(c, cudaEventRecord(c->ev[6], c->stream));
   CU_TRY(c, cudaStreamSynchronize(c->stream));
@@ -526,6 +570,11 @@ int collect_errors_and_timing(cmb_ctx* c, uint32_t* counters_out) {
   if (c->n_local && getenv("CMB_PIPELINE_STATS"))  // what K2 fetched: 128 B per span loaded + 32 B of bitmap per chunk
     fprintf(stderr, "#k2_load\tspans_loaded=%u\tspans=%llu\tdense_chunks=%u\tchunks=%u\n", h[10],
             (unsigned long long)c->n_chunks * CHUNK_SPANS, h[11], c->n_chunks);
+  if (c->n_local && !c->gene_mode && getenv("CMB_PIPELINE_STATS")) {  // contig mode: the bucket entries K2 read (2 B each)
+    uint32_t events = 0;  // word_off[n_words]: the events of the sample
+    CU_TRY(c, cudaMemcpy(&events, c->ref.d_word_off + (size_t)c->n_chunks * K2_WARPS, 4, cudaMemcpyDeviceToHost));
+    fprintf(stderr, "#k2_events\tentries_read=%u\tevents=%u\n", h[12], events);
+  }
   float ms = 0;
   cudaEventElapsedTime(&ms, c->ev[0], c->ev[1]); c->timing.ms_zero = ms;
   cudaEventElapsedTime(&ms, c->ev[3], c->ev[4]); c->timing.ms_scan = ms;
@@ -810,7 +859,10 @@ int cmb_set_reference(cmb_ctx* c, uint32_t n_contigs, const uint64_t* contig_len
   int rc;
   if (c->n_local == 0)  // empty shard: nothing to allocate beyond the rows
     return r.d_rows.ensure(c, std::max<size_t>(1, n_contigs));
-  if ((rc = r.d_arena.ensure(c, c->arena_elems)) || (rc = r.d_span_bits.ensure(c, c->arena_elems / BITMAP_ELEMS_PER_WORD)) ||
+  const size_t n_words = c->arena_elems / BITMAP_ELEMS_PER_WORD;
+  if ((rc = r.d_arena.ensure(c, c->arena_elems)) || (rc = r.d_span_bits.ensure(c, n_words)) ||
+      (rc = r.d_word_count.ensure(c, n_words)) || (rc = r.d_word_off.ensure(c, n_words + 1)) ||
+      (rc = r.d_word_block_sum.ensure(c, n_words / K1B_BLOCK + 1)) ||
       (rc = r.d_off_span.ensure(c, (size_t)c->n_local + 1)) || (rc = r.d_len.ensure(c, c->n_local)) ||
       (rc = r.d_chunk_first.ensure(c, (size_t)c->n_chunks + 1)) || (rc = r.d_tail_sum.ensure(c, c->n_chunks)) ||
       (rc = r.d_carry_in.ensure(c, c->n_chunks)) || (rc = r.d_block_agg.ensure(c, (size_t)c->n_chunks / K1B_BLOCK + 1)) ||
@@ -873,9 +925,10 @@ int cmb_begin_sample(cmb_ctx* c) {
   c->n_records = c->n_intervals = 0;
   CU_TRY(c, cudaEventRecord(c->ev[0], c->stream));
   if (c->n_local) {
-    if (c->arena_dirty) {
-      CU_TRY(c, cudaMemsetAsync(c->ref.d_arena, 0, c->arena_elems * 4, c->stream));
+    if (c->arena_dirty) {  // contig mode adds no event into the arena
+      if (c->gene_mode) CU_TRY(c, cudaMemsetAsync(c->ref.d_arena, 0, c->arena_elems * 4, c->stream));
       CU_TRY(c, cudaMemsetAsync(c->ref.d_span_bits, 0, c->arena_elems / BITMAP_ELEMS_PER_WORD * 4, c->stream));
+      CU_TRY(c, cudaMemsetAsync(c->ref.d_word_count, 0, c->arena_elems / BITMAP_ELEMS_PER_WORD * 4, c->stream));
     }
     CU_TRY(c, cudaMemsetAsync(c->ref.d_tail_sum, 0, 4ull * c->n_chunks, c->stream));
     if (c->pool_dirty) {

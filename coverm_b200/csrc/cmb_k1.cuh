@@ -25,8 +25,15 @@ struct K1Args {
   // (gene), as the arena, gene_bound and the bin pool are laid out over the genes [seg_begin, seg_begin + n_local) only
   uint32_t n_contigs, tid_begin, tid_end, seg_begin;
   // outputs
-  int32_t* arena;
-  uint32_t* span_bits;  // span occupancy bitmap: the bit of every span an event is added to (K2 loads only those spans)
+  int32_t* arena;       // gene mode: the events are added here
+  // contig mode: the sample's event list, entry 2k / 2k + 1 = interval k's start / end as (arena element << 1) | sign (1 for
+  // the -1 at the end), K1_NO_EVENT where there is none; interval k counts from the sample's first (iv_base is the batch's
+  // first, n_iv its interval slots).  K1e buckets the entries by bitmap word, in the order word_count (+1 per event) gives.
+  ulonglong2* events;
+  uint64_t iv_base;
+  uint32_t n_iv;
+  uint32_t* word_count;
+  uint32_t* span_bits;  // span occupancy bitmap: the bit of every span an event is added to (K2 works only on those spans)
   int32_t* tail_sum;
   cmb_contig_stats* rows;
   int2* block_minmax;  // per block {min kept tid, max kept tid} for the cross-block sortedness check
@@ -51,6 +58,8 @@ struct K1Args {
   cmb_params p;
   uint8_t filter_single, filter_pairs;
 };
+
+constexpr unsigned long long K1_NO_EVENT = ~0ull;
 
 #ifndef CMB_K1_MINBLOCKS
 #define CMB_K1_MINBLOCKS 6
@@ -195,27 +204,33 @@ __global__ void __launch_bounds__(K1_THREADS, CMB_K1_MINBLOCKS) k1_filter_accumu
   }
 
   // +1 at `s` and -1 at `e` (when e lies inside the segment) of segment `lc`, the bits of their spans, plus the chunk tail
-  // sums K1b scans
+  // sums K1b scans.  Gene mode adds the events into the arena; contig mode returns them as event list entries.
   // Records are sorted, so neighbouring lanes mostly mark the same bitmap word: one RED per distinct word of the warp.  Plain
-  // per-lane REDs took K1 from 6.7 to 14.2 ms on `bench.py --config ns` (H100 80GB HBM3, 400 W); aggregated: 7.0 ms.
+  // per-lane REDs took K1 from 6.7 to 14.2 ms on `bench.py --config ns` (H100 80GB HBM3, 400 W); aggregated: 7.0 ms.  The
+  // same group adds its event count to the word's count (contig mode).
   auto mark_span = [&](uint64_t g) {
     const uint32_t w = (uint32_t)(g / BITMAP_ELEMS_PER_WORD);
     const uint32_t peers = __match_any_sync(__activemask(), w);
     const uint32_t bits = __reduce_or_sync(peers, 1u << ((uint32_t)(g / SPAN) % BITMAP_SPANS_PER_WORD));
-    if (lane == (uint32_t)__ffs(peers) - 1) atomicOr(a.span_bits + w, bits);
+    if (lane == (uint32_t)__ffs(peers) - 1) {
+      atomicOr(a.span_bits + w, bits);
+      if (a.word_count) atomicAdd(a.word_count + w, (uint32_t)__popc(peers));
+    }
   };
-  auto add_events_in = [&](uint32_t L, uint32_t off0, uint32_t off1, uint32_t s, uint64_t e) {
+  auto add_events_in = [&](uint32_t L, uint32_t off0, uint32_t off1, uint32_t s, uint64_t e) -> ulonglong2 {
     const uint64_t base = (uint64_t)off0 * SPAN;
     const uint64_t end_padded = (uint64_t)off1 * SPAN;  // first element of the next segment
     const uint64_t gs = base + s;
     const bool has_end = e < L;  // "True unless the read hits the contig end"
-    atomicAdd(a.arena + gs, 1);
+    ulonglong2 out = make_ulonglong2(gs << 1, K1_NO_EVENT);
+    if (!a.events) atomicAdd(a.arena + gs, 1);
     mark_span(gs);
     const uint64_t ks = gs / CHUNK;
     const bool cont_s = end_padded > (ks + 1) * (uint64_t)CHUNK;  // this segment continues past chunk ks
     if (has_end) {
       const uint64_t ge = base + e;
-      atomicAdd(a.arena + ge, -1);
+      if (!a.events) atomicAdd(a.arena + ge, -1);
+      out.y = ge << 1 | 1u;
       mark_span(ge);
       const uint64_t ke = ge / CHUNK;
       if (ke != ks) {
@@ -225,6 +240,7 @@ __global__ void __launch_bounds__(K1_THREADS, CMB_K1_MINBLOCKS) k1_filter_accumu
     } else if (cont_s) {
       atomicAdd(a.tail_sum + ks, 1);
     }
+    return out;
   };
   auto add_events = [&](uint32_t lc, uint32_t s, uint64_t e) { add_events_in(a.len[lc], a.off_span[lc], a.off_span[lc + 1], s, e); };
 
@@ -335,29 +351,44 @@ __global__ void __launch_bounds__(K1_THREADS, CMB_K1_MINBLOCKS) k1_filter_accumu
     }
   }
 
-  // ---- delta events (contig.rs:171-186)
-  if (mine) {
+  // ---- delta events (contig.rs:171-186) into the event list: plain coalesced stores, one 16-B entry pair per interval slot.
+  //      Every slot of the batch is written: K1_NO_EVENT for the slots of records that add no event (filtered out, another
+  //      shard's contig), for CMB_IV_PAD and for an interval out of bounds.  Threads 0 and n - 1 also fill the slots before
+  //      the first record's and after the last record's, which belong to no record.
+  if (valid) {
+    const ulonglong2 none = make_ulonglong2(K1_NO_EVENT, K1_NO_EVENT);
+    ulonglong2* ev = a.events + a.iv_base;
+    if (i == 0)
+      for (uint32_t k = 0; k < min(ivb, a.n_iv); ++k) __stcs(ev + k, none);
+    if (i + 1 == a.n)
+      for (uint32_t k = ive; k < a.n_iv; ++k) __stcs(ev + k, none);
     const uint32_t lc = (uint32_t)tid - a.tid_begin;
     (void)lc;
 #if CMB_K1_PREFETCH
     const uint32_t L = pre_L, off0 = pre_off0, off1 = pre_off1;
 #else
-    const uint32_t L = a.len[lc], off0 = a.off_span[lc], off1 = a.off_span[lc + 1];
+    uint32_t L = 0, off0 = 0, off1 = 0;
+    if (mine) L = a.len[lc], off0 = a.off_span[lc], off1 = a.off_span[lc + 1];
 #endif
-    for (uint32_t k = ivb; k < ive; ++k) {
+    for (uint32_t k = ivb; k < min(ive, a.n_iv); ++k) {
+      ulonglong2 out = none;
+      if (mine) {
 #if CMB_K1_PREFETCH
-      const int32_t s = k == ivb ? pre_s : a.iv_start[k];
-      const uint32_t n = (uint32_t)(k == ivb ? pre_n : a.iv_len[k]);
+        const int32_t s = k == ivb ? pre_s : a.iv_start[k];
+        const uint32_t n = (uint32_t)(k == ivb ? pre_n : a.iv_len[k]);
 #else
-      const int32_t s = a.iv_start[k];
-      const uint32_t n = (uint32_t)a.iv_len[k];
+        const int32_t s = a.iv_start[k];
+        const uint32_t n = (uint32_t)a.iv_len[k];
 #endif
-      if (s == INT_MIN) continue;  // CMB_IV_PAD: unused slot of the interval pool
-      if (s < 0 || (uint32_t)s >= L) {  // `ups_and_downs[cursor] += 1` would panic
-        err |= ERR_BOUNDS;
-        continue;
+        if (s == INT_MIN) {
+          // CMB_IV_PAD: unused slot of the interval pool
+        } else if (s < 0 || (uint32_t)s >= L) {  // `ups_and_downs[cursor] += 1` would panic
+          err |= ERR_BOUNDS;
+        } else {
+          out = add_events_in(L, off0, off1, (uint32_t)s, (uint64_t)(uint32_t)s + n);
+        }
       }
-      add_events_in(L, off0, off1, (uint32_t)s, (uint64_t)(uint32_t)s + n);
+      __stcs(ev + k, out);
     }
   }
   err = __reduce_or_sync(FULL, err);
@@ -403,5 +434,35 @@ __global__ void __launch_bounds__(1024) k1c_check_sorted(const int2* block_minma
     if (mm.x != INT_MAX && mm.x < before) bad = true;
   }
   if (bad) atomicOr(error_flags, ERR_UNSORTED);
+}
+
+// ------------------------------------------------------------------------------------------------ K1e
+// Contig mode: the sample's event list bucketed by bitmap word (1024 arena elements), one thread per interval slot.  An event
+// at element g goes to buckets[word_off[w] + r] of its word w = g / 1024 as the u16 code (g % 1024) | sign << 10.  The slots
+// r of a word are handed out by counting word_count[w] down from K1's count, one RED per distinct word of a warp (records are
+// sorted, so a warp's events fall in a few words), which leaves every count at zero for the next sample.  Order inside a
+// bucket is arbitrary: K2 only adds the deltas up.
+constexpr uint32_t K1E_THREADS = 256;
+__global__ void __launch_bounds__(K1E_THREADS) k1e_bucket_events(const ulonglong2* events, uint64_t n_iv, const uint32_t* word_off,
+                                                                uint32_t* word_count, uint16_t* buckets) {
+  const uint64_t k = (uint64_t)blockIdx.x * K1E_THREADS + threadIdx.x;
+  const uint32_t lane = threadIdx.x & 31;
+  const ulonglong2 e = k < n_iv ? __ldcs(events + k) : make_ulonglong2(K1_NO_EVENT, K1_NO_EVENT);
+  auto place = [&](unsigned long long x) {
+    const bool has = x != K1_NO_EVENT;
+    const uint32_t active = __ballot_sync(FULL, has);
+    if (!has) return;
+    const uint64_t g = x >> 1;
+    const uint32_t w = (uint32_t)(g / BITMAP_ELEMS_PER_WORD);
+    const uint32_t off = __ldg(word_off + w);
+    const uint32_t peers = __match_any_sync(active, w), n = __popc(peers), head = __ffs(peers) - 1;
+    uint32_t top = 0;
+    if (lane == head) top = atomicSub(word_count + w, n);
+    top = __shfl_sync(peers, top, head);
+    const uint32_t r = top - n + __popc(peers & ((1u << lane) - 1));
+    buckets[off + r] =(uint16_t)((uint32_t)(g % BITMAP_ELEMS_PER_WORD) | (uint32_t)(x & 1) << 10);
+  };
+  place(e.x);
+  place(e.y);
 }
 

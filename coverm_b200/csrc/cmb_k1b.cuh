@@ -28,6 +28,64 @@ struct K1bBins {
   uint32_t n_blocks;              // 0 = no histogram wanted
 };
 
+// Contig mode: the exclusive scan of K1's per-bitmap-word event counts, word_off[w] = events of the words before w (the
+// first of w's bucket, K1e), word_off[n_words] = events of the sample.  The host keeps a sample under 2^32 events.
+struct K1bWords {
+  const uint32_t* count;  // [n_words]
+  uint32_t* off;          // [n_words + 1]
+  uint32_t* block_sum;    // [n_blocks]: events of each block of K1B_BLOCK words
+  uint32_t n_words, n_blocks;  // n_blocks = 0: gene mode, no scan
+};
+
+// Word block `b` of k1b_local: local exclusive scan of its K1B_BLOCK counts (entry n_words gets the total) and its sum.
+__device__ __forceinline__ void k1b_words_local(const K1bWords& g, uint32_t b) {
+  __shared__ uint32_t s_w[K1B_THREADS / 32];
+  const uint32_t t = threadIdx.x, lane = t & 31, warp = t >> 5;
+  const uint32_t i0 = b * K1B_BLOCK + t * K1B_PER;
+  uint32_t n[K1B_PER], sum = 0;
+#pragma unroll
+  for (uint32_t i = 0; i < K1B_PER; ++i) {
+    n[i] = i0 + i < g.n_words ? g.count[i0 + i] : 0u;
+    sum += n[i];
+  }
+  uint32_t incl = sum;
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) {
+    const uint32_t o = __shfl_up_sync(FULL, incl, d);
+    if ((int)lane >= d) incl += o;
+  }
+  if (lane == 31) s_w[warp] = incl;
+  __syncthreads();
+  uint32_t x = incl - sum;
+  for (uint32_t w = 0; w < warp; ++w) x += s_w[w];
+  if (t == K1B_THREADS - 1) g.block_sum[b] = x + sum;
+#pragma unroll
+  for (uint32_t i = 0; i < K1B_PER; ++i) {
+    if (i0 + i <= g.n_words) g.off[i0 + i] = x;
+    x += n[i];
+  }
+}
+
+// Word block `b` of k1b_apply: adds the events of the blocks before it.
+__device__ __forceinline__ void k1b_words_apply(const K1bWords& g, uint32_t b) {
+  __shared__ uint32_t s_w[K1B_THREADS / 32];
+  const uint32_t t = threadIdx.x;
+  uint32_t acc = 0;
+  for (uint32_t j = t; j < b; j += K1B_THREADS) acc += g.block_sum[j];
+  acc = __reduce_add_sync(FULL, acc);
+  if ((t & 31) == 0) s_w[t >> 5] = acc;
+  __syncthreads();
+  uint32_t before = 0;
+#pragma unroll
+  for (uint32_t w = 0; w < K1B_THREADS / 32; ++w) before += s_w[w];
+  if (before == 0) return;
+#pragma unroll
+  for (uint32_t i = 0; i < K1B_PER; ++i) {
+    const uint32_t s = b * K1B_BLOCK + t * K1B_PER + i;
+    if (s <= g.n_words) g.off[s] += before;
+  }
+}
+
 struct K1bElem {
   bool reset;
   int add;
@@ -100,10 +158,16 @@ __device__ __forceinline__ void k1b_bins_apply(const K1bBins& g, uint32_t b) {
   }
 }
 
-// Blocks [0, ceil(n_chunks / K1B_BLOCK)) scan the chunks, the g.n_blocks after them the segments.
+// Blocks [0, ceil(n_chunks / K1B_BLOCK)) scan the chunks, the g.n_blocks after them the segments, the wd.n_blocks after
+// those the bitmap words.
 __global__ void __launch_bounds__(K1B_THREADS) k1b_local(int32_t* tail_sum, const uint32_t* chunk_first, const uint32_t* off_span,
-                                                        uint32_t n_chunks, int32_t* carry_in, int2* block_agg, const K1bBins g) {
-  const uint32_t chunk_blocks = gridDim.x - g.n_blocks;
+                                                        uint32_t n_chunks, int32_t* carry_in, int2* block_agg, const K1bBins g,
+                                                        const K1bWords wd) {
+  const uint32_t chunk_blocks = gridDim.x - g.n_blocks - wd.n_blocks;
+  if (blockIdx.x >= chunk_blocks + g.n_blocks) {
+    k1b_words_local(wd, blockIdx.x - chunk_blocks - g.n_blocks);
+    return;
+  }
   if (blockIdx.x >= chunk_blocks) {
     k1b_bins_local(g, blockIdx.x - chunk_blocks);
     return;
@@ -176,8 +240,12 @@ __global__ void __launch_bounds__(K1B_THREADS) k1b_local(int32_t* tail_sum, cons
 }
 
 __global__ void __launch_bounds__(K1B_THREADS) k1b_apply(const int32_t* needs, const int2* block_agg, uint32_t n_chunks, int32_t* carry_in,
-                                                        const K1bBins g) {
-  const uint32_t chunk_blocks = gridDim.x - g.n_blocks;
+                                                        const K1bBins g, const K1bWords wd) {
+  const uint32_t chunk_blocks = gridDim.x - g.n_blocks - wd.n_blocks;
+  if (blockIdx.x >= chunk_blocks + g.n_blocks) {
+    k1b_words_apply(wd, blockIdx.x - chunk_blocks - g.n_blocks);
+    return;
+  }
   if (blockIdx.x >= chunk_blocks) {
     k1b_bins_apply(g, blockIdx.x - chunk_blocks);
     return;

@@ -1,4 +1,4 @@
-// K2: segmented prefix sum of the delta arena + every O(L) reduction of EST::add_contig, one pass over the spans that hold
+// K2: segmented prefix sum of the delta events + every O(L) reduction of EST::add_contig, one pass over the spans that hold
 // events.
 //
 // Persistent warps: warp g of W (8 per CTA) reduces the 8192-element chunks g, g + W, g + 2W, ...  Which of a chunk's 256
@@ -18,10 +18,17 @@
 // most its read count), so a run's count is one fire-and-forget RED; K3 reads the bins in depth order and re-zeroes them.
 // Depth 0 is not added: K3 derives its count from the window length and covered_window.
 //
-// Loads: each warp has a ring of K2_STAGES buffers of 32 rows x 128 B laid out as a TMA box with the 128-B swizzle writes
-// them.  A dense chunk's rounds are one 32-row TMA box each (completion on the stage's mbarrier); a sparse round copies its
+// Loads (gene mode, from the arena): each warp has a ring of K2_STAGES buffers of 32 rows x 128 B laid out as a TMA box with
+// the 128-B swizzle writes them.  A dense chunk's rounds are one 32-row TMA box each (completion on the stage's mbarrier); a sparse round copies its
 // occupied rows with cp.async into rows 0..n-1, four whole 128-B lines per instruction.  The next round's rows, possibly of
 // the next chunk, are requested before the current round is reduced.
+//
+// Contig mode (BUCKETS) reads no arena: K1 wrote the sample's events to a list and K1e bucketed them by bitmap word
+// (cmb_k1.cuh), so a round's events are the contiguous bucket range of the words its slots lie in.  The fetch stage copies
+// that range into the round's stage of bucket entries with cp.async (16-B units, up to K2_STAGE_CODES entries; a round with
+// more reads the rest straight from global memory), and right before the reduction the warp adds each entry into the one row
+// buffer in shared memory, at its slot's row (cmb_k2_slots.cuh, k2_round_events), with a shared-memory atomic.  The
+// reduction reads the rows exactly as it reads an arena round, then re-zeroes the units that held an event.
 #pragma once
 #include "cmb_k2_slots.cuh"
 
@@ -32,9 +39,11 @@ struct K2Args {
   const int32_t* carry_in;
   cmb_contig_stats* rows;
   uint32_t tid_begin, n_local, n_chunks, excl;
-  int32_t* arena;
+  int32_t* arena;               // gene mode
+  const uint32_t* word_off;     // contig mode: [n_chunks * 8 + 1] first bucket entry of each bitmap word (K1b)
+  const uint16_t* buckets;      // contig mode: the events bucketed by word (K1e), 8 entries of padding at the end
   uint32_t* span_bits;   // [n_chunks * 8] span occupancy bitmap (K1); bit b of word w of a chunk = its span 32 w + b
-  uint32_t* load_stats;  // [0] += spans loaded, [1] += chunks loaded whole (CMB_PIPELINE_STATS)
+  uint32_t* load_stats;  // [0] += spans loaded, [1] += chunks loaded whole, [2] += bucket entries read (CMB_PIPELINE_STATS)
   const uint64_t* bin_base;  // [n_local + 1] first bin of each contig (K1b); bin_base[n_local] = bins needed
   uint32_t* bins;            // the bin pool: pool_cap u32 counts, zero outside a sample
   uint64_t pool_cap;
@@ -42,7 +51,8 @@ struct K2Args {
   uint32_t* error_flags;
 };
 
-// A chunk with at least this many non-empty spans (of 256) is loaded whole, 32 rows per TMA box; sparser chunks row by row.
+// A chunk with at least this many non-empty spans (of 256) is reduced whole, all 256 spans as slots (gene mode: loaded 32 rows
+// per TMA box); sparser chunks only their occupied spans.
 // On an H100 80GB HBM3 at 400 W, K2 time moved by under 2 % for thresholds from 96 to 257 (never whole) on both `bench.py
 // --config 2` and `--config ns` (DESIGN.md §4, K2): row copies are not what limits K2 there.  160 sends chunks above ~60 %
 // occupancy down the TMA path.
@@ -56,23 +66,32 @@ static_assert(K2_CHUNK_SPANS == CHUNK_SPANS && K2_WARPS == 8, "a chunk is 8 bitm
 constexpr uint32_t K2_ROUND = 32;                     // slots per round, one per lane
 constexpr uint32_t K2_BUF_BYTES = K2_ROUND * 128;     // one round's rows: 4 KB, whole 1024-B swizzle atoms
 constexpr uint32_t K2_BOX_ROWS = K2_ROUND;            // rows of the TMA box (cmb_set_reference encodes it)
-constexpr uint32_t K2_SMEM_STAGE_BYTES = K2_WARPS * K2_STAGES * K2_BUF_BYTES;
-constexpr uint32_t K2_SMEM_MISC = K2_WARPS * K2_STAGES * 8 /*an mbarrier per (warp, stage)*/ + K2_WARPS * 64 /*bitmap words*/;
-constexpr uint32_t K2_SMEM_BYTES = K2_SMEM_STAGE_BYTES + K2_SMEM_MISC;
+constexpr uint32_t K2_STAGE_CODES = 1024;             // bucket entries one stage holds (contig mode): 2 KB
+constexpr uint32_t K2_STAGE_BYTES = K2_STAGE_CODES * 2;
+// a warp's buffers: a ring of K2_STAGES round buffers (arena), or one round buffer and K2_STAGES stages of bucket entries
+template <bool BUCKETS>
+__host__ __device__ constexpr uint32_t k2_warp_bytes() { return BUCKETS ? K2_BUF_BYTES + K2_STAGES * K2_STAGE_BYTES : K2_STAGES * K2_BUF_BYTES; }
+constexpr uint32_t K2_SMEM_MISC = K2_WARPS * K2_STAGES * 8 /*an mbarrier per (warp, stage)*/ +
+                                  K2_WARPS * 128 /*bitmap words of two chunks, bucket offsets of one*/;
+template <bool BUCKETS>
+__host__ __device__ constexpr uint32_t k2_smem_bytes() { return K2_WARPS * k2_warp_bytes<BUCKETS>() + K2_SMEM_MISC; }
+static_assert(k2_warp_bytes<true>() % 1024 == 0 && k2_warp_bytes<false>() % 1024 == 0, "round buffers are whole swizzle atoms");
 
 __device__ __forceinline__ uint32_t k2_rounds(uint32_t pop, bool dense) { return dense ? CHUNK_SPANS / K2_ROUND : (pop + K2_ROUND - 1) / K2_ROUND; }
 
-template <bool HIST, bool CLEAN>
+template <bool HIST, bool CLEAN, bool BUCKETS>
 __global__ void __launch_bounds__(K2_THREADS, CMB_K2_MINBLOCKS) k2_scan_reduce(const __grid_constant__ CUtensorMap tmap, const K2Args a) {
   extern __shared__ __align__(1024) uint8_t smem[];  // the buffers need the 1024 B swizzle-atom alignment
   const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  uint8_t* ring = smem + warp * K2_STAGES * K2_BUF_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + K2_SMEM_STAGE_BYTES) + warp * K2_STAGES;
-  // the 8 bitmap words of the chunk being fetched and of the one being reduced (in shared memory rather than registers: K2
-  // runs at the 80-register cap)
-  uint32_t* words = reinterpret_cast<uint32_t*>(smem + K2_SMEM_STAGE_BYTES + K2_WARPS * K2_STAGES * 8) + warp * 16;
+  constexpr uint32_t RING = K2_WARPS * k2_warp_bytes<BUCKETS>();
+  uint8_t* ring = smem + warp * k2_warp_bytes<BUCKETS>();
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + RING) + warp * K2_STAGES;
+  // the 8 bitmap words of the chunk being fetched and of the one being reduced, and (BUCKETS) the 9 bucket offsets of the
+  // latter's words (in shared memory rather than registers: K2 runs at the 80-register cap)
+  uint32_t* words = reinterpret_cast<uint32_t*>(smem + RING + K2_WARPS * K2_STAGES * 8) + warp * 32;
   uint32_t(&fw)[8] = *reinterpret_cast<uint32_t(*)[8]>(words);
   uint32_t(&w)[8] = *reinterpret_cast<uint32_t(*)[8]>(words + 8);
+  uint32_t* wo = words + 16;
 
   // The pool is sized before the launch from a bound of bin_base[n_local]; when it is still too small (cmb_grow_buffers
   // then grows it to exactly that) no bin is added and K3 reads none.
@@ -82,10 +101,14 @@ __global__ void __launch_bounds__(K2_THREADS, CMB_K2_MINBLOCKS) k2_scan_reduce(c
   const uint32_t W = gridDim.x * K2_WARPS, g = blockIdx.x * K2_WARPS + warp;
   // word `lane` (lanes 0..7) of chunk ck's span bitmap
   auto load_word = [&](uint32_t ck) -> uint32_t { return ck < a.n_chunks && lane < K2_WARPS ? a.span_bits[ck * K2_WARPS + lane] : 0u; };
-  // lanes 0..7 put their words of a chunk into `to` for the whole warp; returns the chunk's popcount
-  auto spread = [&](uint32_t word, uint32_t* to) -> uint32_t {
+  // BUCKETS: the first bucket entry of word `lane` (lanes 0..8, 8 = the next chunk's first) of chunk ck
+  auto load_off = [&](uint32_t ck) -> uint32_t { return BUCKETS && ck < a.n_chunks && lane <= K2_WARPS ? __ldg(a.word_off + ck * K2_WARPS + lane) : 0u; };
+  // lanes 0..7 put their words of a chunk into `to` for the whole warp (and lanes 0..8 their bucket offsets into `to_off`);
+  // returns the chunk's popcount
+  auto spread = [&](uint32_t word, uint32_t* to, uint32_t off = 0, uint32_t* to_off = nullptr) -> uint32_t {
     __syncwarp();  // every lane is done with the previous chunk's words
     if (lane < K2_WARPS) to[lane] = word;
+    if (to_off && lane <= K2_WARPS) to_off[lane] = off;
     __syncwarp();
     return __reduce_add_sync(FULL, __popc(word));
   };
@@ -94,6 +117,8 @@ __global__ void __launch_bounds__(K2_THREADS, CMB_K2_MINBLOCKS) k2_scan_reduce(c
     for (uint32_t s = 0; s < K2_STAGES; ++s) mbar_init(smem_u32(bars + s), 1);
     fence_barrier_init();
   }
+  if (BUCKETS)  // the round buffer starts at zero; every round leaves it so
+    for (uint32_t u = lane; u < K2_BUF_BYTES / 16; u += 32) reinterpret_cast<int4*>(ring)[u] = make_int4(0, 0, 0, 0);
   __syncwarp();
 
   // ---- the fetch cursor: round fr of chunk fk is the next one whose rows are requested.  It runs K2_STAGES - 1
@@ -101,11 +126,14 @@ __global__ void __launch_bounds__(K2_THREADS, CMB_K2_MINBLOCKS) k2_scan_reduce(c
   uint32_t fk = g, fr = 0, fpop = 0;
   bool fdense = false;
   uint32_t f_word = load_word(fk);      // bitmap word of chunk fk, requested a chunk ahead
-  uint32_t n_loaded = 0, n_dense = 0;   // what this warp fetched (load_stats)
+  uint32_t f_off = load_off(fk), fo = 0;  // BUCKETS: bucket offsets of chunk fk, requested a chunk ahead; of the cursor's chunk
+  uint32_t n_loaded = 0, n_dense = 0, n_events = 0;  // what this warp fetched (load_stats)
   auto f_enter = [&]() {
     for (; fk < a.n_chunks; fk += W) {
       const uint32_t word = f_word;
       f_word = load_word(fk + W);
+      fo = f_off;
+      f_off = load_off(fk + W);
       fpop = spread(word, fw);
       fdense = fpop >= K2_DENSE_SPANS;
       fr = 0;
@@ -122,7 +150,17 @@ __global__ void __launch_bounds__(K2_THREADS, CMB_K2_MINBLOCKS) k2_scan_reduce(c
     if (fk < a.n_chunks) {
       uint8_t* buf = ring + (fi % K2_STAGES) * K2_BUF_BYTES;
       const uint32_t bar = smem_u32(bars + fi % K2_STAGES);
-      if (fdense) {
+      if (BUCKETS) {
+        // the round's bucket entries, 16-B units from the one holding its first entry, as many as the stage holds
+        uint32_t wf, wl;
+        k2_round_words(fw, fdense ? CHUNK_SPANS : fpop, fdense, fr, wf, wl);
+        const uint32_t b0 = __shfl_sync(FULL, fo, wf), b1 = __shfl_sync(FULL, fo, wl + 1);
+        const uint32_t base = b0 & ~7u, units = min((b1 - base + 7) / 8, K2_STAGE_CODES / 8);
+        uint8_t* stg = ring + K2_BUF_BYTES + (fi % K2_STAGES) * K2_STAGE_BYTES;
+        const int4* src = reinterpret_cast<const int4*>(a.buckets + base);
+        for (uint32_t u = lane; u < units; u += 32) cp_async_16(smem_u32(stg + u * 16), src + u);
+        n_events += b1 - b0;
+      } else if (fdense) {
         if (lane == 0) {
           fence_proxy_async_smem();  // the stage's earlier reads and cp.async writes (ordered by __syncwarp) come first
           mbar_arrive_expect_tx(bar, K2_BUF_BYTES);
@@ -173,7 +211,7 @@ __global__ void __launch_bounds__(K2_THREADS, CMB_K2_MINBLOCKS) k2_scan_reduce(c
     top = max(top, (uint32_t)depth);
   };
 
-  uint32_t c_word = load_word(g);  // the next chunk's bitmap word and metadata, requested a chunk ahead
+  uint32_t c_word = load_word(g), c_off = load_off(g);  // the next chunk's bitmap word and metadata, requested a chunk ahead
   uint32_t n_cf = 0, n_cl = 0;
   int n_cin = 0;
   if (g < a.n_chunks) {
@@ -183,15 +221,16 @@ __global__ void __launch_bounds__(K2_THREADS, CMB_K2_MINBLOCKS) k2_scan_reduce(c
   }
   uint32_t i = 0;  // rounds reduced by this warp
   for (uint32_t k = g; k < a.n_chunks; k += W) {
-    const uint32_t word = c_word, cf = n_cf, cl = n_cl;
+    const uint32_t word = c_word, off = c_off, cf = n_cf, cl = n_cl;
     const int cin = n_cin;
     c_word = load_word(k + W);
+    c_off = load_off(k + W);
     if (k + W < a.n_chunks) {
       n_cf = __ldg(a.chunk_first + k + W);
       n_cl = __ldg(a.chunk_first + k + W + 1);
       n_cin = __ldg(a.carry_in + k + W);
     }
-    const uint32_t pop = spread(word, w);
+    const uint32_t pop = spread(word, w, off, BUCKETS ? wo : nullptr);
     const bool dense = pop >= K2_DENSE_SPANS;
     const uint32_t nr = k2_rounds(pop, dense), nslots = dense ? CHUNK_SPANS : pop;
     const uint32_t span0 = k * CHUNK_SPANS;
@@ -223,11 +262,26 @@ __global__ void __launch_bounds__(K2_THREADS, CMB_K2_MINBLOCKS) k2_scan_reduce(c
         }
       }
       const uint32_t st = i % K2_STAGES;
-      mbar_wait(smem_u32(bars + st), (i / K2_STAGES) & 1);
+      if (!BUCKETS) mbar_wait(smem_u32(bars + st), (i / K2_STAGES) & 1);
       cp_async_wait<K2_STAGES - 1>();  // this lane's copies into stage st (only the fill above may still be in flight)
       __syncwarp();                    // ... and those of the other lanes
+      uint8_t* rows = BUCKETS ? ring : ring + st * K2_BUF_BYTES;
+      if (BUCKETS) {
+        // ---- the round's rows from its bucket entries: staged ones from the stage, the rest from global memory
+        // the words of its first and last slot (k2_round_words, from the spans the lanes already hold)
+        const uint32_t wf = __shfl_sync(FULL, s, 0) / 32, wl = __shfl_sync(FULL, s, min(nslots - r * K2_ROUND, K2_ROUND) - 1) / 32;
+        const uint32_t base = wo[wf] & ~7u;
+        const uint16_t* stg = reinterpret_cast<const uint16_t*>(ring + K2_BUF_BYTES + st * K2_STAGE_BYTES);
+        k2_round_events(
+            w, wo, dense, r, wf, wl, lane, 32,
+            [&](uint32_t p) { return p - base < K2_STAGE_CODES ? (uint32_t)stg[p - base] : (uint32_t)__ldg(a.buckets + p); },
+            [&](uint32_t rw, uint32_t e, int d) {
+              atomicAdd(reinterpret_cast<int*>(rows + rw * 128 + (((e >> 2) ^ (rw & 7)) << 4) + ((e & 3) << 2)), d);
+            });
+        __syncwarp();
+      }
       // ---- the slot's 32 deltas (row `lane`): only their sum and the mask of non-zero positions stay in registers
-      const uint8_t* row = ring + st * K2_BUF_BYTES + lane * 128;
+      uint8_t* row = rows + lane * 128;
       int total = 0;
       uint32_t ev = 0;
       if (valid) {
@@ -238,7 +292,7 @@ __global__ void __launch_bounds__(K2_THREADS, CMB_K2_MINBLOCKS) k2_scan_reduce(c
           const uint32_t e4 = (v.x != 0 ? 1u : 0u) | (v.y != 0 ? 2u : 0u) | (v.z != 0 ? 4u : 0u) | (v.w != 0 ? 8u : 0u);
           total += (v.x + v.y) + (v.z + v.w);
           ev |= e4 << (4 * u);
-          if (CLEAN && e4) gsp[u] = make_int4(0, 0, 0, 0);  // re-zero only the 16 B units that hold an event
+          if (!BUCKETS && CLEAN && e4) gsp[u] = make_int4(0, 0, 0, 0);  // re-zero only the 16 B units that hold an event
         }
       }
       // ---- depth entering the slot: segmented (by contig) exclusive scan of the slot totals, seeded from the previous slot
@@ -264,6 +318,10 @@ __global__ void __launch_bounds__(K2_THREADS, CMB_K2_MINBLOCKS) k2_scan_reduce(c
             [&](int d, uint32_t n) {
               if (hist) bin_add(bin0, bin1, d, n, top);
             });
+      if (BUCKETS)  // the row buffer is zero again for the next round
+#pragma unroll
+        for (uint32_t u = 0; u < SPAN / 4; ++u)
+          if (ev >> (4 * u) & 15u) *reinterpret_cast<int4*>(row + ((u ^ (lane & 7)) << 4)) = make_int4(0, 0, 0, 0);
       pc = __shfl_sync(FULL, c, 31);
       pd = __shfl_sync(FULL, out, 31);
       if (r == 0) c_first = __shfl_sync(FULL, c, 0);
@@ -303,5 +361,6 @@ __global__ void __launch_bounds__(K2_THREADS, CMB_K2_MINBLOCKS) k2_scan_reduce(c
   if (lane == 0 && n_loaded) {
     atomicAdd(a.load_stats + 0, n_loaded);
     atomicAdd(a.load_stats + 1, n_dense);
+    if (BUCKETS) atomicAdd(a.load_stats + 2, n_events);
   }
 }

@@ -1,5 +1,6 @@
 // K2's per-slot arithmetic as plain integer code, shared by k2_scan_reduce and tests/native/k2_slots_check.cpp (which
-// compiles it with g++ and walks random arenas in the kernel's order against a per-position prefix sum).
+// compiles it with g++ and walks random arenas in the kernel's order against a per-position prefix sum), and the building of
+// a round's rows from word buckets, shared with tests/native/k2_buckets_check.cpp (against rows cut from a dense arena).
 //
 // A chunk's slots are all 256 of its spans when it is dense, else only its occupied spans, in order.  Slot j covers the
 // positions from its span's start up to the next slot's span (the chunk's end for the last slot): past the span's last
@@ -65,6 +66,42 @@ K2_HD uint32_t k2_slot_span(const uint32_t (&w)[8], uint32_t j, bool dense) {
     }
   }
   return found ? base + k2_nth_bit(word, rem) : K2_CHUNK_SPANS;
+}
+
+// ---- A round's rows from word buckets (contig mode).  K1e puts each event of bitmap word q of a chunk into the word's bucket
+// as the u16 code (element % 1024) | sign << 10 (sign 1: the -1 at a block's end); the bucket of word q is the entries
+// [wo[q], wo[q + 1]).  Row i of round r is slot 32 r + i: span 32 r + i of a dense chunk, else the (32 r + i)-th occupied span.
+
+// The first and last bitmap word (0..7) that round r's slots lie in, of a chunk with nslots slots (nslots > 32 r)
+K2_HD void k2_round_words(const uint32_t (&w)[8], uint32_t nslots, bool dense, uint32_t r, uint32_t& wf, uint32_t& wl) {
+  const uint32_t j1 = r * 32 + 31 < nslots ? r * 32 + 31 : nslots - 1;
+  wf = k2_slot_span(w, r * 32, dense) / 32;
+  wl = k2_slot_span(w, j1, dense) / 32;
+}
+
+// Row of round r for an event of word q with code `code`, `before` the slots of the words before q: its span's slot minus
+// 32 r, 32 or more when the slot is another round's (a word the round shares with its neighbours)
+K2_HD uint32_t k2_bucket_row(const uint32_t (&w)[8], bool dense, uint32_t r, uint32_t q, uint32_t before, uint32_t code) {
+  const uint32_t b = (code & 1023u) / 32u;  // span within word q
+  if (dense) return q * 32 + b - r * 32;
+  return before + k2_popc(w[q] & ((1u << b) - 1u)) - r * 32;  // wraps past 32 for an earlier round's slot
+}
+
+// The events of round r, whose slots lie in words wf..wl: bucket entries p = wo[wf] + p0, + step, ... below wo[wl + 1]
+// (K2: p0 = lane, step = 32).  code(p) reads entry p; add(row, e, delta) is called for each event of the round's slots, e
+// its position in the span.
+template <class Code, class Add>
+K2_HD void k2_round_events(const uint32_t (&w)[8], const uint32_t* wo, bool dense, uint32_t r, uint32_t wf, uint32_t wl,
+                           uint32_t p0, uint32_t step, Code code, Add add) {
+  uint32_t q = wf, before = 0;  // the word of entry p and the slots of the words before it
+  for (uint32_t x = 0; x < wf; ++x) before += k2_popc(w[x]);
+  const uint32_t p1 = wo[wl + 1];
+  for (uint32_t p = wo[wf] + p0; p < p1; p += step) {
+    while (q < wl && wo[q + 1] <= p) before += k2_popc(w[q++]);
+    const uint32_t c = code(p);
+    const uint32_t row = k2_bucket_row(w, dense, r, q, before, c);
+    if (row < 32) add(row, c & 31u, (c >> 10) & 1u ? -1 : 1);
+  }
 }
 
 // A contig's length and its end-trimmed window [w0, w1) (empty when 2E >= L), in contig coordinates.
