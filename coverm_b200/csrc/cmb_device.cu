@@ -1,13 +1,14 @@
 // libcoverm_b200 — device side: hand-written sm_90a kernels + the C ABI of include/coverm_b200.h.
 //
 // Data layout in HBM (one cmb_ctx = one GPU = one contig shard):
-//   arena        i32[arena_elems]   all segments' `ups_and_downs` (contig.rs:144-145) back to back; every segment
-//                                   starts on a 32-element span boundary (SPAN), the arena is a whole number of
-//                                   8192-element chunks (CHUNK).  4 B per reference base.  Gene mode adds its events
-//                                   here; contig mode only uses its coordinates (element g of the arena).
+//   arena        i32[arena_elems]   gene mode only: all segments' `ups_and_downs` (contig.rs:144-145) back to back, 4 B per
+//                                   base.  Both modes lay the segments out in these coordinates (element g of the
+//                                   layout): every segment starts on a 32-element span boundary (SPAN), the layout is a
+//                                   whole number of 8192-element chunks (CHUNK).  Contig mode allocates no arena; its
+//                                   events go to the event list, so its device memory does not grow with the bases.
 //   span_bits    u32[arena_elems/1024]  one bit per 32-element span: set by K1 for every event it adds, read (and, when
 //                                   cleaning as it goes, cleared) by K2, which works only on the spans named there.
-//                                   Zero exactly when the arena is (zeroed together; K2 cleans both).
+//                                   Zero between samples (K2 cleans it, in gene mode together with the arena).
 //   events       u64[2 * intervals of the sample]  contig mode, K1: interval k's start / end as (g << 1) | sign
 //   word_count   u32[arena_elems/1024]  contig mode, K1: events per bitmap word; K1e counts them back down to zero
 //   word_off     u32[arena_elems/1024 + 1]  contig mode, K1b: exclusive scan of word_count
@@ -145,6 +146,7 @@ struct Buf {
   }
   ~Buf() { release(); }
   operator T*() const { return p; }
+  uint64_t bytes() const { return sizeof(T) * (uint64_t)cap; }
   void release() {
     if (p) {
       if (PINNED) cudaFreeHost(p);
@@ -368,7 +370,44 @@ void carve_batch(void* slab, uint32_t nr, uint32_t ni, cmb_read_batch* b) {
 
 void free_reference(cmb_ctx* c) {
   c->ref = {};
+  c->tmap = {};
   c->gene_mode = false;
+}
+
+// Gene mode's delta arena (K1 adds its events there, K2 loads the rows that hold them) and its TMA descriptor: the arena as
+// [rows][32] i32, box = one K2 round (32 rows x 128 B = four 1024-B swizzle atoms), 128B swizzle.  Contig mode has neither.
+int alloc_arena(cmb_ctx* c) {
+  auto& r = c->ref;
+  if (int rc = r.d_arena.ensure(c, c->arena_elems)) return rc;
+  PFN_encodeTiled encode = nullptr;
+  cudaDriverEntryPointQueryResult qres;
+  CU_TRY(c, cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", (void**)&encode, cudaEnableDefault, &qres));
+  if (!encode || qres != cudaDriverEntryPointSuccess) return fail(c, CMB_E_CUDA, "cuTensorMapEncodeTiled not available in this driver");
+  cuuint64_t gdim[2] = {ROW_ELEMS, c->arena_elems / ROW_ELEMS};
+  cuuint64_t gstride[1] = {ROW_ELEMS * 4};
+  cuuint32_t box[2] = {ROW_ELEMS, K2_BOX_ROWS};
+  cuuint32_t estr[2] = {1, 1};
+  CUresult res = encode(&c->tmap, CU_TENSOR_MAP_DATA_TYPE_INT32, 2, r.d_arena.p, gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                        CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (res != CUDA_SUCCESS) return fail(c, CMB_E_CUDA, "cuTensorMapEncodeTiled failed with CUresult %d", (int)res);
+  return CMB_OK;
+}
+
+// CMB_PIPELINE_STATS: the device bytes this context holds for its reference, by part (the sample's event list and buckets,
+// sized by the records, are not included)
+void print_reference_bytes(const cmb_ctx* c) {
+  const auto& r = c->ref;
+  const uint64_t arena = r.d_arena.bytes();
+  const uint64_t bitmap = r.d_span_bits.bytes() + r.d_word_count.bytes() + r.d_word_off.bytes() + r.d_word_block_sum.bytes();
+  const uint64_t chunks = r.d_chunk_first.bytes() + r.d_tail_sum.bytes() + r.d_carry_in.bytes() + r.d_block_agg.bytes();
+  const uint64_t rows = r.d_rows.bytes() + r.d_off_span.bytes() + r.d_len.bytes() + r.d_bin_base.bytes() + r.d_bin_block_sum.bytes() +
+                        r.d_bin_hi.bytes() + r.d_gene_first.bytes() + r.d_gene_start.bytes() + r.d_gene_end.bytes() +
+                        r.d_gene_maxlen.bytes() + r.d_contig_len32.bytes() + r.d_contig_seen.bytes() + r.d_gene_bound.bytes();
+  const uint64_t bins = r.d_bins.bytes(), pairs = r.d_pairs.bytes();
+  fprintf(stderr, "#reference_bytes\tarena=%llu\tbitmap=%llu\tchunks=%llu\trows=%llu\tbins=%llu\tpairs=%llu\ttotal=%llu\tlayout_elems=%llu\n",
+          (unsigned long long)arena, (unsigned long long)bitmap, (unsigned long long)chunks, (unsigned long long)rows,
+          (unsigned long long)bins, (unsigned long long)pairs, (unsigned long long)(arena + bitmap + chunks + rows + bins + pairs),
+          (unsigned long long)c->arena_elems);
 }
 
 // Whether K1 has work: a context with no local segment has none, except in gene mode, where owned contigs without genes still
@@ -519,6 +558,9 @@ int run_end_of_sample(cmb_ctx* c) {
       CU_TRY(c, cudaStreamSynchronize(c->stream));
     }
     if (int rc = ensure_pool(c, need, with_slack(need))) return rc;
+    // CSR pairs: K3 writes at most one per bin, plus a depth-0 pair per contig
+    if (csr)
+      if (int rc = r.d_pairs.ensure(c, need + c->n_local, with_slack(need + c->n_local))) return rc;
   }
   K2Args a{};
   a.off_span = r.d_off_span; a.len = r.d_len; a.chunk_first = r.d_chunk_first; a.carry_in = r.d_carry_in;
@@ -570,6 +612,7 @@ int collect_errors_and_timing(cmb_ctx* c, uint32_t* counters_out) {
   if (c->n_local && getenv("CMB_PIPELINE_STATS"))  // what K2 fetched: 128 B per span loaded + 32 B of bitmap per chunk
     fprintf(stderr, "#k2_load\tspans_loaded=%u\tspans=%llu\tdense_chunks=%u\tchunks=%u\n", h[10],
             (unsigned long long)c->n_chunks * CHUNK_SPANS, h[11], c->n_chunks);
+  if (getenv("CMB_PIPELINE_STATS")) print_reference_bytes(c);
   if (c->n_local && !c->gene_mode && getenv("CMB_PIPELINE_STATS")) {  // contig mode: the bucket entries K2 read (2 B each)
     uint32_t events = 0;  // word_off[n_words]: the events of the sample
     CU_TRY(c, cudaMemcpy(&events, c->ref.d_word_off + (size_t)c->n_chunks * K2_WARPS, 4, cudaMemcpyDeviceToHost));
@@ -781,6 +824,10 @@ static int set_genes(cmb_ctx* c, uint32_t n_contigs, const uint64_t* contig_len,
   const uint32_t g_begin = whole || tid_begin == 0 ? 0 : seg_cut(tid_begin), g_end = whole ? n_seg : seg_cut(tid_end);
   int rc = cmb_set_reference(c, n_seg, seg_len.data(), g_begin, g_end);
   if (rc) return rc;
+  if (c->n_local && (rc = alloc_arena(c))) {
+    free_reference(c);  // no context in gene mode without its arena
+    return rc;
+  }
   c->gene_mode = true;
   c->n_ref_contigs = n_contigs;
   c->gene_tid_begin = whole ? 0 : tid_begin;
@@ -839,7 +886,9 @@ int cmb_set_reference(cmb_ctx* c, uint32_t n_contigs, const uint64_t* contig_len
     off_span[i] = (uint32_t)spans;
     len[i] = (uint32_t)L;
     spans += std::max<uint64_t>(1, (L + SPAN - 1) / SPAN);
-    if (spans > 0xfffffff0ull) return fail(c, CMB_E_ARG, "cmb_set_reference: shard larger than 2^36 bases; use more shards");
+    if (spans > CMB_MAX_SPANS)
+      return fail(c, CMB_E_ARG, "cmb_set_reference: contigs [%u, %u) need more than %llu 32-base spans (about 2^37 bases), the limit of "
+                  "one context; split them over more GPUs (contig shards)", tid_begin, tid_end, (unsigned long long)CMB_MAX_SPANS);
   }
   off_span[c->n_local] = (uint32_t)spans;
   const uint64_t chunks = std::max<uint64_t>(1, (spans + CHUNK_SPANS - 1) / CHUNK_SPANS);
@@ -859,8 +908,10 @@ int cmb_set_reference(cmb_ctx* c, uint32_t n_contigs, const uint64_t* contig_len
   int rc;
   if (c->n_local == 0)  // empty shard: nothing to allocate beyond the rows
     return r.d_rows.ensure(c, std::max<size_t>(1, n_contigs));
+  // no delta arena: contig mode's events go to the sample's event list (K1) and K2 builds its rows in shared memory; gene
+  // mode allocates the arena after this layout (set_genes)
   const size_t n_words = c->arena_elems / BITMAP_ELEMS_PER_WORD;
-  if ((rc = r.d_arena.ensure(c, c->arena_elems)) || (rc = r.d_span_bits.ensure(c, n_words)) ||
+  if ((rc = r.d_span_bits.ensure(c, n_words)) ||
       (rc = r.d_word_count.ensure(c, n_words)) || (rc = r.d_word_off.ensure(c, n_words + 1)) ||
       (rc = r.d_word_block_sum.ensure(c, n_words / K1B_BLOCK + 1)) ||
       (rc = r.d_off_span.ensure(c, (size_t)c->n_local + 1)) || (rc = r.d_len.ensure(c, c->n_local)) ||
@@ -881,18 +932,6 @@ int cmb_set_reference(cmb_ctx* c, uint32_t n_contigs, const uint64_t* contig_len
   if (small_hist() && (rc = ensure_pool(c, 64, 64))) return rc;  // testing aid: a pool that overflows at once
   c->pool_dirty = false;
   c->arena_dirty = true;
-  // TMA descriptor: the arena as [rows][32] i32, box = one K2 round (32 rows x 128 B = four 1024-B swizzle atoms), 128B swizzle
-  PFN_encodeTiled encode = nullptr;
-  cudaDriverEntryPointQueryResult qres;
-  CU_TRY(c, cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", (void**)&encode, cudaEnableDefault, &qres));
-  if (!encode || qres != cudaDriverEntryPointSuccess) return fail(c, CMB_E_CUDA, "cuTensorMapEncodeTiled not available in this driver");
-  cuuint64_t gdim[2] = {ROW_ELEMS, c->arena_elems / ROW_ELEMS};
-  cuuint64_t gstride[1] = {ROW_ELEMS * 4};
-  cuuint32_t box[2] = {ROW_ELEMS, K2_BOX_ROWS};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult res = encode(&c->tmap, CU_TENSOR_MAP_DATA_TYPE_INT32, 2, r.d_arena.p, gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                        CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (res != CUDA_SUCCESS) return fail(c, CMB_E_CUDA, "cuTensorMapEncodeTiled failed with CUresult %d", (int)res);
   return CMB_OK;
 }
 
@@ -943,11 +982,10 @@ int cmb_begin_sample(cmb_ctx* c) {
   if (c->gene_mode) CU_TRY(c, cudaMemsetAsync(c->ref.d_contig_seen, 0, std::max<size_t>(1, c->n_ref_contigs), c->stream));
   CU_TRY(c, cudaEventRecord(c->ev[1], c->stream));
   c->arena_dirty = true;  // until K2 has cleaned it
-  if ((c->params.want & CMB_WANT_HIST_CSR) && c->n_local) {
-    uint64_t want = std::max<uint64_t>(1u << 20, c->arena_elems / 16);
-    if (small_hist()) want = 64;  // testing aid: start with a pair buffer that overflows at once (cmb_grow_buffers path)
-    if (int rc = c->ref.d_pairs.ensure(c, want)) return rc;
-  }
+  // The pair buffer is sized from the sample's records before K3 (run_end_of_sample); the testing aid starts it with 64 pairs,
+  // which overflow at once (cmb_grow_buffers path)
+  if ((c->params.want & CMB_WANT_HIST_CSR) && c->n_local && small_hist())
+    if (int rc = c->ref.d_pairs.ensure(c, 64)) return rc;
   c->in_sample = true;
   c->ended = false;
   c->n_acquired = 0;

@@ -217,19 +217,19 @@ __global__ void __launch_bounds__(K1_THREADS, CMB_K1_MINBLOCKS) k1_filter_accumu
       if (a.word_count) atomicAdd(a.word_count + w, (uint32_t)__popc(peers));
     }
   };
+  // Returns the events as event list entries; only gene mode (add_gene_events) also adds them into the arena, which contig
+  // mode does not have
   auto add_events_in = [&](uint32_t L, uint32_t off0, uint32_t off1, uint32_t s, uint64_t e) -> ulonglong2 {
     const uint64_t base = (uint64_t)off0 * SPAN;
     const uint64_t end_padded = (uint64_t)off1 * SPAN;  // first element of the next segment
     const uint64_t gs = base + s;
     const bool has_end = e < L;  // "True unless the read hits the contig end"
     ulonglong2 out = make_ulonglong2(gs << 1, K1_NO_EVENT);
-    if (!a.events) atomicAdd(a.arena + gs, 1);
     mark_span(gs);
     const uint64_t ks = gs / CHUNK;
     const bool cont_s = end_padded > (ks + 1) * (uint64_t)CHUNK;  // this segment continues past chunk ks
     if (has_end) {
       const uint64_t ge = base + e;
-      if (!a.events) atomicAdd(a.arena + ge, -1);
       out.y = ge << 1 | 1u;
       mark_span(ge);
       const uint64_t ke = ge / CHUNK;
@@ -242,7 +242,11 @@ __global__ void __launch_bounds__(K1_THREADS, CMB_K1_MINBLOCKS) k1_filter_accumu
     }
     return out;
   };
-  auto add_events = [&](uint32_t lc, uint32_t s, uint64_t e) { add_events_in(a.len[lc], a.off_span[lc], a.off_span[lc + 1], s, e); };
+  auto add_gene_events = [&](uint32_t lc, uint32_t s, uint64_t e) {
+    const ulonglong2 ev = add_events_in(a.len[lc], a.off_span[lc], a.off_span[lc + 1], s, e);
+    atomicAdd(a.arena + (ev.x >> 1), 1);
+    if (ev.y != K1_NO_EVENT) atomicAdd(a.arena + (ev.y >> 1), -1);
+  };
 
   if (a.gene_first) {
     // ---- per-gene coverage (genes.rs:182-344, 467-552).  A gene's delta array is the contig's, cut to [start, end) with the
@@ -295,7 +299,7 @@ __global__ void __launch_bounds__(K1_THREADS, CMB_K1_MINBLOCKS) k1_filter_accumu
             const uint64_t e = (uint64_t)(uint32_t)s + (uint32_t)a.iv_len[k];
             if (e <= gsx || (uint32_t)s >= gex) continue;  // no overlap
             const uint32_t cs = max((uint32_t)s, gsx) - gsx;
-            add_events(lg, cs, e - gsx);  // e - gsx >= gene length: the block runs past the gene, no -1
+            add_gene_events(lg, cs, e - gsx);  // e - gsx >= gene length: the block runs past the gene, no -1
           }
         }
       }

@@ -39,7 +39,7 @@ struct K2Args {
   const int32_t* carry_in;
   cmb_contig_stats* rows;
   uint32_t tid_begin, n_local, n_chunks, excl;
-  int32_t* arena;               // gene mode
+  int32_t* arena;               // gene mode (null in contig mode, whose tensor map is all zero)
   const uint32_t* word_off;     // contig mode: [n_chunks * 8 + 1] first bucket entry of each bitmap word (K1b)
   const uint16_t* buckets;      // contig mode: the events bucketed by word (K1e), 8 entries of padding at the end
   uint32_t* span_bits;   // [n_chunks * 8] span occupancy bitmap (K1); bit b of word w of a chunk = its span 32 w + b
@@ -150,7 +150,7 @@ __global__ void __launch_bounds__(K2_THREADS, CMB_K2_MINBLOCKS) k2_scan_reduce(c
     if (fk < a.n_chunks) {
       uint8_t* buf = ring + (fi % K2_STAGES) * K2_BUF_BYTES;
       const uint32_t bar = smem_u32(bars + fi % K2_STAGES);
-      if (BUCKETS) {
+      if constexpr (BUCKETS) {  // contig mode has no arena and no tensor map: only the gene-mode branches name them
         // the round's bucket entries, 16-B units from the one holding its first entry, as many as the stage holds
         uint32_t wf, wl;
         k2_round_words(fw, fdense ? CHUNK_SPANS : fpop, fdense, fr, wf, wl);
@@ -285,14 +285,14 @@ __global__ void __launch_bounds__(K2_THREADS, CMB_K2_MINBLOCKS) k2_scan_reduce(c
       int total = 0;
       uint32_t ev = 0;
       if (valid) {
-        int4* gsp = reinterpret_cast<int4*>(a.arena + (uint64_t)(span0 + s) * SPAN);
 #pragma unroll
         for (uint32_t u = 0; u < SPAN / 4; ++u) {
           const int4 v = *reinterpret_cast<const int4*>(row + ((u ^ (lane & 7)) << 4));
           const uint32_t e4 = (v.x != 0 ? 1u : 0u) | (v.y != 0 ? 2u : 0u) | (v.z != 0 ? 4u : 0u) | (v.w != 0 ? 8u : 0u);
           total += (v.x + v.y) + (v.z + v.w);
           ev |= e4 << (4 * u);
-          if (!BUCKETS && CLEAN && e4) gsp[u] = make_int4(0, 0, 0, 0);  // re-zero only the 16 B units that hold an event
+          if constexpr (!BUCKETS && CLEAN)  // gene mode: re-zero only the arena's 16 B units that hold an event
+            if (e4) reinterpret_cast<int4*>(a.arena + (uint64_t)(span0 + s) * SPAN)[u] = make_int4(0, 0, 0, 0);
         }
       }
       // ---- depth entering the slot: segmented (by contig) exclusive scan of the slot totals, seeded from the previous slot

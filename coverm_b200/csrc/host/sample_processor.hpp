@@ -418,6 +418,21 @@ class DeviceSession {
       nvtx_header.end();
     }
 
+    // Contig mode: every rank's contigs [cuts[r], cuts[r + 1]) fit one device context.  All ranks of a group check every
+    // rank's range, so they stop together.
+    static void check_layout_fits(const std::vector<uint64_t>& lens, const std::vector<uint32_t>& cuts) {
+      for (size_t r = 0; r + 1 < cuts.size(); ++r) {
+        const uint64_t spans = layout_spans(lens, cuts[r], cuts[r + 1]);
+        if (spans <= CMB_MAX_SPANS) continue;
+        const int n = gpus_for_layout(lens);
+        throw ExitError(1, "the reference contigs [" + std::to_string(cuts[r]) + ", " + std::to_string(cuts[r + 1]) + ") take " +
+                               std::to_string(spans) + " 32-base spans, more than one GPU holds (" + std::to_string(CMB_MAX_SPANS) +
+                               ", about 2^37 bases); " +
+                               (n ? "run with --gpus " + std::to_string(n) + " or more to split them over GPUs by contig"
+                                  : std::string("no split by contig brings every GPU's share under that")));
+      }
+    }
+
     // The device's reference (or genes) and the sample begun.
     void reference() {
       sb = std::min<uint32_t>(s.shard_begin_, n_ref);
@@ -465,6 +480,7 @@ class DeviceSession {
         }
         res.genes = s.gene_cache_;
       } else if (res.hdr->lens != s.ref_lens_ || sb != s.ref_sb_ || se != s.ref_se_) {
+        check_layout_fits(res.hdr->lens, shard ? shard->cuts : std::vector<uint32_t>{sb, se});
         s.ref_sb_ = sb;
         s.ref_se_ = se;
         rc = cmb_set_reference(s.ctx_, n_ref, res.hdr->lens.data(), sb, se);

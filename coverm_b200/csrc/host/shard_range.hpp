@@ -35,6 +35,27 @@ inline std::vector<uint32_t> tid_cuts_by_length(const std::vector<uint64_t>& len
   return cut;
 }
 
+// 32-base spans the contigs [b, e) take in one device context's layout (at least one per contig, cmb_set_reference); a
+// context holds at most CMB_MAX_SPANS of them.
+inline uint64_t layout_spans(const std::vector<uint64_t>& lens, uint32_t b, uint32_t e) {
+  uint64_t s = 0;
+  for (uint32_t t = b; t < e; ++t) s += std::max<uint64_t>(1, (lens[t] + 31) / 32);
+  return s;
+}
+
+// The smallest number of GPUs whose contig cuts (tid_cuts_by_length) keep every rank's contigs within CMB_MAX_SPANS, or 0 when
+// no number up to one GPU per contig does.
+inline int gpus_for_layout(const std::vector<uint64_t>& lens) {
+  const uint64_t total = layout_spans(lens, 0, (uint32_t)lens.size());
+  for (uint64_t n = std::max<uint64_t>(1, (total + CMB_MAX_SPANS - 1) / CMB_MAX_SPANS); n <= std::max<size_t>(1, lens.size()); ++n) {
+    const std::vector<uint32_t> cut = tid_cuts_by_length(lens, (int)n);
+    bool fits = true;
+    for (uint64_t r = 0; r < n && fits; ++r) fits = layout_spans(lens, cut[r], cut[r + 1]) <= CMB_MAX_SPANS;
+    if (fits) return (int)n;
+  }
+  return 0;
+}
+
 // Per-gene coverage (--gff): a contig's share of the work is its genes' arena, every gene padded to whole 32-base spans (the
 // device lays a rank's arena out over the genes of its contigs, cmb_set_genes_range).  seg_tid / seg_len: contig and length of
 // each gene.  Cutting these weights with tid_cuts_by_length keeps the cuts on contig boundaries: a contig's genes never split

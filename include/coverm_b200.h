@@ -162,7 +162,7 @@ typedef struct cmb_sample_timing {
   float ms_scan;      /* K2: segmented scan + reductions + histogram emit */
   float ms_finalize;  /* K3: per-contig histogram merge + trimmed/variance walk */
   float ms_total;     /* begin_sample .. end_sample on the stream      */
-  uint64_t arena_elems;   /* padded i32 elements scanned by K2        */
+  uint64_t arena_elems;   /* padded elements (bases) of the reference layout K2 scans */
   uint64_t n_records;     /* records submitted                         */
   uint64_t n_intervals;   /* intervals submitted                       */
   uint32_t k1_launches, k2_launches, k3_launches, reserved;
@@ -177,7 +177,16 @@ const char* cmb_last_error(const cmb_ctx* ctx); /* ctx may be NULL: last cmb_cre
 
 /* Reference layout: `vec![0; header.target_len(tid)]` for every tid at once
  * (contig.rs:144-145).  [tid_begin, tid_end) is the shard this context owns
- * (multi-GPU contig sharding); records on other tids are ignored. */
+ * (multi-GPU contig sharding); records on other tids are ignored.
+ *
+ * Device memory: no per-base depth array is kept.  Each owned contig takes whole 32-base spans; the layout costs about
+ * 0.0132 B per base (span bitmap and per-word event tables: 12 B per 1024 bases; chunk tables: 12 B per 8192 bases) and about
+ * 164 B per owned contig (result row, offsets, histogram bin bases), plus a 144-B result row for every contig of the header.
+ * A 137 Gbp reference needs about 1.8 GB.  A sample adds about 20 B per aligned block (event list and its buckets), 4.5 B per
+ * record with CMB_WANT_HIST (histogram bins) and 9 B more with CMB_WANT_HIST_CSR (pairs), all grow-only.  One context holds at most CMB_MAX_SPANS spans, about 2^37 bases
+ * (137 Gbp): larger references need several contexts on disjoint contig ranges (several GPUs); a larger shard is CMB_E_ARG,
+ * with nothing allocated. */
+#define CMB_MAX_SPANS 0xfffffff0ull
 int cmb_set_reference(cmb_ctx* ctx, uint32_t n_contigs, const uint64_t* contig_len, uint32_t tid_begin,
                       uint32_t tid_end);
 int cmb_set_params(cmb_ctx* ctx, const cmb_params* params, cmb_filter_mode* mode_out);
@@ -189,7 +198,9 @@ int cmb_set_params(cmb_ctx* ctx, const cmb_params* params, cmb_filter_mode* mode
  * arrays, and the usual scan / reductions run over the genes.  Call INSTEAD of cmb_set_reference; records keep carrying contig
  * tids.  `genes` must be sorted by (tid, start) with start < end <= contig_len[tid].  Result rows (cmb_end_sample): one per
  * gene, in that order, with n_primary = primaries starting in the gene, sum_edit = sum of NM.saturating_sub(indels)
- * (genes.rs:297; sum_indel stays 0), sum_identity_primary, and the window / histogram statistics of the gene's own length. */
+ * (genes.rs:297; sum_indel stays 0), sum_identity_primary, and the window / histogram statistics of the gene's own length.
+ * Device memory: the layout of cmb_set_reference over the genes, plus a delta array of 4 B per gene base (each gene padded
+ * to whole 32-base spans), so the genes of one context must fit its GPU at 4 B per base. */
 typedef struct cmb_gene {
   uint32_t tid;
   uint32_t start;
