@@ -89,6 +89,7 @@ namespace {
 #include "cmb_decode_t1.cuh"
 #include "cmb_pairs.cuh"
 #include "cmb_filter.cuh"
+#include "cmb_shards.cuh"
 
 // rows[i].hist_offset += base for the rows that carry histogram pairs (cmb_allgather_stats: local -> global pair offsets)
 __global__ void __launch_bounds__(256) k_rebase_hist_offsets(cmb_contig_stats* rows, uint32_t n, uint64_t base) {
@@ -279,6 +280,30 @@ struct cmb_ctx {
     cudaEvent_t ev[6]{};
     bool have_events = false;
   } dec;
+  // sharded input (cmb_shard_*; cmb_shards.cuh): per-shard primary stores and the running choice of every pair; grow-only
+  struct Shards {
+    struct Store {
+      Buf<uint8_t> slab;  // carved as a cmb_read_batch over the shard's primaries
+      Buf<uint8_t> info;
+      ShardStore view{};
+      uint64_t n_prim = 0, n_iv = 0;
+    };
+    std::vector<Store> store;
+    std::vector<int32_t> tid_offsets;
+    uint32_t n_shards = 0, added = 0;
+    bool active = false;
+    Buf<uint8_t> d_excluded;
+    bool have_excluded = false;
+    Buf<unsigned long long> d_scan, d_hash0, d_err, d_tid_count, d_src, d_slot_iv;
+    Buf<int32_t> d_as_val;
+    Buf<uint8_t> d_as_state;
+    Buf<PairState> d_state;
+    Buf<ShardStore> d_stores;
+    Buf<int32_t> d_tid_offsets;
+    Buf<uint8_t> d_out_slab;
+    cudaEvent_t ev[4]{};
+    float ms_choose = 0, ms_decode = 0;
+  } sh;
 };
 
 namespace {
@@ -773,6 +798,8 @@ void cmb_destroy(cmb_ctx* c) {
   cudaSetDevice(c->device);
   if (c->stream) cudaStreamSynchronize(c->stream);
   for (auto e : c->batch_done) cudaEventDestroy(e);
+  for (auto e : c->sh.ev)
+    if (e) cudaEventDestroy(e);
   for (auto& e : c->k1_events) {
     cudaEventDestroy(e.first);
     cudaEventDestroy(e.second);
@@ -989,6 +1016,7 @@ int cmb_begin_sample(cmb_ctx* c) {
   c->in_sample = true;
   c->ended = false;
   c->n_acquired = 0;
+  c->sh.active = false;
   return CMB_OK;
 }
 
@@ -2014,3 +2042,244 @@ extern "C" int cmb_filter_fetch(cmb_ctx* c, uint8_t* records, uint64_t n_bytes) 
   return CMB_OK;
 }
 
+
+// ---- sharded input (cmb_shards.cuh) ---------------------------------------------------------------------------------------
+namespace {
+
+// The reference's message for the smallest error key of ks_* (see cmb_shards.cuh), or CMB_OK
+int shard_error(cmb_ctx* c, unsigned long long key) {
+  if (key == ~0ull) return CMB_OK;
+  const uint32_t kind = (uint32_t)(key >> 8) & 0xf, detail = (uint32_t)key & 0xff;
+  const unsigned long long set = key >> 24;
+  switch (kind) {
+    case SHE_UNPAIRED:
+      return fail(c, CMB_E_SHARD_EXIT, "This code can only handle paired-end input (at the moment), sorry. Found an unpaired record before primary %llu", set);
+    case SHE_NAME:
+      return fail(c, CMB_E_SHARD_EXIT, "BAM files do not appear to be properly sorted by read name. The read names of primary alignment %llu differ between the shards", set);
+    case SHE_AS_MISSING:
+      return fail(c, CMB_E_SHARD_PANIC, "Mapping record encountered that does not have an 'AS' auxiliary tag in the SAM/BAM format. This is required for ranking pairs of alignments.");
+    case SHE_AS_TYPE: {
+      const char* name = detail == 'c' ? "I8" : detail == 's' ? "I16" : detail == 'i' ? "I32" : detail == 'I' ? "U32" : detail == 'f' ? "Float"
+                         : detail == 'A' ? "Char" : detail == 'Z' ? "String" : detail == 'H' ? "HexByteArray" : "Array";
+      return fail(c, CMB_E_SHARD_PANIC, "Unexpected data type of AS aux tag, found %s", name);
+    }
+    case SHE_NO_SEPARATOR:
+      return fail(c, CMB_E_SHARD_PANIC, "Contig name does not contain split symbol, so cannot determine which genome it belongs to");
+    case SHE_EXCLUDED:
+      return fail(c, CMB_E_SHARD_EXIT, "CoverM cannot currently deal with reads that only map to excluded genomes");
+    case SHE_NM_TYPE:
+      return fail(c, CMB_E_NM, "Unexpected data type of NM aux tag");
+    case SHE_NM_MISSING:
+      return fail(c, CMB_E_NM, "record with name at primary alignment %llu had no NM tag", set);
+  }
+  return fail(c, CMB_E_CUDA, "sharded input: unknown error key %llx", key);
+}
+
+int shard_event(cmb_ctx* c, int i) {
+  if (!c->sh.ev[i]) CU_TRY(c, cudaEventCreate(&c->sh.ev[i]));
+  return CMB_OK;
+}
+
+// cmb_decode_bgzf's stages inside a sample: the shard's records inflated, located and reduced to tuples in device memory
+int decode_shard(cmb_ctx* c, const cmb_bgzf_input* in, cmb_bgzf_result* out, uint32_t k) {
+  c->dec.last_valid = false;
+  c->dec.filter_planned = false;
+  *out = cmb_bgzf_result{};
+  if (in->n_blocks == 0 || in->ranged) return fail(c, CMB_E_ARG, "cmb_shard_add: shard %u: a whole BGZF file is needed", k);
+  BgzfCall j{c, c->dec, in, out, true, in->n_blocks};
+  int rc = j.prepare();
+  if (!rc && !j.nothing_to_decode && !(rc = j.copy_inflate()) && !(rc = j.declined()) && !(rc = j.chain())) rc = j.extract();
+  if (rc == CMB_E_NOMEM) {
+    cudaGetLastError();
+    return fail(c, CMB_E_DECLINED, "shard %u: not enough device memory to decode it", k);
+  }
+  if (rc == CMB_E_DECLINED) return fail(c, CMB_E_DECLINED, "shard %u: the device decoder declined it (%s); sharded input is decoded on the device only", k, c->err.c_str());
+  if (rc) return rc;
+  if (!j.nothing_to_decode) {
+    CU_TRY(c, cudaEventSynchronize(c->dec.ev[4]));
+    cudaEventElapsedTime(&out->ms_total, c->dec.ev[0], c->dec.ev[4]);
+  }
+  c->dec.last_valid = false;  // the tuples are the shard's, not a sample's: cmb_last_bgzf_batch must not hand them out
+  return CMB_OK;
+}
+
+uint64_t shard_bytes(const cmb_ctx* c) {
+  const auto& s = c->sh;
+  uint64_t b = s.d_scan.bytes() + s.d_hash0.bytes() + s.d_tid_count.bytes() + s.d_src.bytes() + s.d_slot_iv.bytes() + s.d_as_val.bytes() +
+               s.d_as_state.bytes() + s.d_state.bytes() + s.d_out_slab.bytes() + s.d_excluded.bytes();
+  for (const auto& st : s.store) b += st.slab.bytes() + st.info.bytes();
+  return b;
+}
+
+}  // namespace
+
+extern "C" int cmb_shard_begin(cmb_ctx* c, uint32_t n_shards, const uint32_t* tid_offsets, const uint8_t* excluded) {
+  NvtxRange nvtx_fn("cmb_shard_begin");
+  if (!c || !tid_offsets || n_shards == 0) return fail(c, CMB_E_ARG, "cmb_shard_begin: null argument or no shards");
+  if (!c->in_sample) return fail(c, CMB_E_ARG, "cmb_shard_begin: no sample in progress");
+  if (c->mode.filter_pairs || c->params.filtering) return fail(c, CMB_E_ARG, "cmb_shard_begin: sharded input takes no read filter");
+  if (n_shards > 255) return fail(c, CMB_E_ARG, "cmb_shard_begin: at most 255 shards");
+  const uint32_t n_ref = c->gene_mode ? c->n_ref_contigs : c->n_contigs;
+  for (uint32_t k = 0; k < n_shards; ++k)
+    if (tid_offsets[k] > n_ref || (k && tid_offsets[k] < tid_offsets[k - 1])) return fail(c, CMB_E_ARG, "cmb_shard_begin: tid offsets outside the reference");
+  CU_TRY(c, cudaSetDevice(c->device));
+  auto& s = c->sh;
+  s.n_shards = n_shards;
+  s.added = 0;
+  s.tid_offsets.assign(tid_offsets, tid_offsets + n_shards);
+  if (s.store.size() < n_shards) s.store.resize(n_shards);
+  s.have_excluded = excluded != nullptr;
+  if (excluded) {
+    if (int rc = s.d_excluded.ensure(c, std::max<uint32_t>(1, n_ref))) return rc;
+    CU_TRY(c, cudaMemcpyAsync(s.d_excluded, excluded, n_ref, cudaMemcpyHostToDevice, c->stream));
+  }
+  if (int rc = s.d_err.ensure(c, 1)) return rc;
+  CU_TRY(c, cudaMemsetAsync(s.d_err, 0xff, 8, c->stream));
+  for (int i = 0; i < 4; ++i)
+    if (int rc = shard_event(c, i)) return rc;
+  s.ms_choose = s.ms_decode = 0;
+  s.active = true;
+  return CMB_OK;
+}
+
+extern "C" int cmb_shard_add(cmb_ctx* c, const cmb_bgzf_input* in, cmb_bgzf_result* out) {
+  NvtxRange nvtx_fn("cmb_shard_add");
+  if (!c || !in || !out || !in->data || !in->block_coffset || !in->block_clen || !in->block_isize)
+    return fail(c, CMB_E_ARG, "cmb_shard_add: null argument");
+  auto& s = c->sh;
+  if (!c->in_sample || !s.active || s.added >= s.n_shards) return fail(c, CMB_E_ARG, "cmb_shard_add: call cmb_shard_begin first, once per shard");
+  CU_TRY(c, cudaSetDevice(c->device));
+  const uint32_t k = s.added;
+  if (int rc = decode_shard(c, in, out, k)) return rc;
+  s.ms_decode += out->ms_total;
+  auto& d = c->dec;
+  const uint64_t n_rec = d.last_n_rec * (uint64_t)(out->n_records != 0);
+  auto& st = s.store[k];
+  CU_TRY(c, cudaEventRecord(s.ev[0], c->stream));
+  // ---- which records are primaries, and where their tuples and intervals go
+  if (int rc = s.d_scan.ensure(c, n_rec + 1, with_slack(n_rec + 1))) return rc;
+  ShardScanArgs a{};
+  a.data = d.last_infl_base; a.rec_off = d.d_rec_off; a.n_records = n_rec; a.scan = s.d_scan;
+  a.shard = k; a.tid_offset = s.tid_offsets[k]; a.err = s.d_err;
+  unsigned long long packed = 0;
+  if (n_rec) {
+    carve_batch(d.d_tuple_slab, d.last_n_rec, d.last_n_cig, &a.tb);
+    ks_mark<<<(uint32_t)((n_rec + 255) / 256), 256, 0, c->stream>>>(a);
+    kf_scan<<<1, 1024, 0, c->stream>>>(s.d_scan, (uint32_t)n_rec);
+    CU_TRY(c, cudaGetLastError());
+    CU_TRY(c, cudaMemcpyAsync(&packed, s.d_scan + n_rec, 8, cudaMemcpyDeviceToHost, c->stream));
+    CU_TRY(c, cudaStreamSynchronize(c->stream));
+  }
+  st.n_prim = packed >> 32;
+  st.n_iv = (uint32_t)packed;
+  // ---- the shard's store
+  size_t offs[13];
+  const size_t slab = batch_slab_bytes((uint32_t)st.n_prim, (uint32_t)st.n_iv, offs);
+  if (int rc = st.slab.ensure(c, slab, slab + slab / 8)) return rc;
+  if (int rc = st.info.ensure(c, st.n_prim + 1, with_slack(st.n_prim + 1))) return rc;
+  carve_batch(st.slab, (uint32_t)st.n_prim, (uint32_t)st.n_iv, &st.view.b);
+  st.view.info = st.info;
+  const uint32_t iv_total = (uint32_t)st.n_iv;
+  CU_TRY(c, cudaMemcpyAsync(st.view.b.iv_begin + st.n_prim, &iv_total, 4, cudaMemcpyHostToDevice, c->stream));
+  if (int rc = s.d_as_val.ensure(c, st.n_prim + 1, with_slack(st.n_prim + 1))) return rc;
+  if (int rc = s.d_as_state.ensure(c, st.n_prim + 1, with_slack(st.n_prim + 1))) return rc;
+  const uint64_t n0 = s.store[0].n_prim;
+  if (k == 0) {
+    if (int rc = s.d_hash0.ensure(c, n0 + 1, with_slack(n0 + 1))) return rc;
+    if (int rc = s.d_state.ensure(c, n0 / 2 + 1, with_slack(n0 / 2 + 1))) return rc;
+    CU_TRY(c, cudaMemsetAsync(s.d_state, 0xff, sizeof(PairState) * (n0 / 2 + 1), c->stream));
+  }
+  a.st = st.view; a.as_val = s.d_as_val; a.as_state = s.d_as_state; a.hash0 = s.d_hash0; a.n0 = n0;
+  if (n_rec) ks_compact<<<(uint32_t)((n_rec + 255) / 256), 256, 0, c->stream>>>(a);
+  // ---- every pair's running winner
+  ShardPairArgs p{};
+  p.st = st.view; p.as_val = s.d_as_val; p.as_state = s.d_as_state; p.excluded = s.have_excluded ? s.d_excluded.p : nullptr;
+  p.state = s.d_state; p.n_pairs = std::min(st.n_prim, n0) / 2; p.shard = k; p.tid_offset = s.tid_offsets[k]; p.err = s.d_err;
+  if (p.n_pairs) ks_pairs<<<(uint32_t)((p.n_pairs + 255) / 256), 256, 0, c->stream>>>(p);
+  CU_TRY(c, cudaGetLastError());
+  CU_TRY(c, cudaEventRecord(s.ev[1], c->stream));
+  CU_TRY(c, cudaEventSynchronize(s.ev[1]));
+  float ms = 0;
+  cudaEventElapsedTime(&ms, s.ev[0], s.ev[1]);
+  s.ms_choose += ms;
+  s.added += 1;
+  return CMB_OK;
+}
+
+extern "C" int cmb_shard_finish(cmb_ctx* c, cmb_shard_result* out) {
+  NvtxRange nvtx_fn("cmb_shard_finish");
+  if (!c || !out) return fail(c, CMB_E_ARG, "cmb_shard_finish: null argument");
+  auto& s = c->sh;
+  if (!c->in_sample || !s.active || s.added != s.n_shards) return fail(c, CMB_E_ARG, "cmb_shard_finish: every shard must be added first");
+  s.active = false;
+  CU_TRY(c, cudaSetDevice(c->device));
+  *out = cmb_shard_result{};
+  // the reader's own checks (shard_bam_reader.rs:117-121, 187-190) are keyed like the kernels' errors
+  const uint64_t n0 = s.store[0].n_prim;
+  uint64_t n_min = n0;
+  bool equal = true;
+  for (uint32_t k = 0; k < s.n_shards; ++k) {
+    n_min = std::min(n_min, s.store[k].n_prim);
+    equal = equal && s.store[k].n_prim == n0;
+  }
+  const uint64_t n_pairs = n_min / 2;
+  const uint32_t n_ref = c->gene_mode ? c->n_ref_contigs : c->n_contigs;
+  CU_TRY(c, cudaEventRecord(s.ev[2], c->stream));
+  if (int rc = s.d_tid_count.ensure(c, (size_t)n_ref + 1, (size_t)n_ref + 1)) return rc;
+  if (int rc = s.d_stores.ensure(c, s.n_shards)) return rc;
+  if (int rc = s.d_tid_offsets.ensure(c, s.n_shards)) return rc;
+  std::vector<ShardStore> views(s.n_shards);
+  for (uint32_t k = 0; k < s.n_shards; ++k) views[k] = s.store[k].view;
+  CU_TRY(c, cudaMemcpyAsync(s.d_stores, views.data(), sizeof(ShardStore) * s.n_shards, cudaMemcpyHostToDevice, c->stream));
+  CU_TRY(c, cudaMemcpyAsync(s.d_tid_offsets, s.tid_offsets.data(), 4ull * s.n_shards, cudaMemcpyHostToDevice, c->stream));
+  CU_TRY(c, cudaMemsetAsync(s.d_tid_count, 0, 8ull * ((size_t)n_ref + 1), c->stream));
+  ShardSortArgs a{};
+  a.stores = s.d_stores; a.tid_offsets = s.d_tid_offsets; a.state = s.d_state; a.n_pairs = n_pairs; a.n_contigs = n_ref;
+  a.tid_count = s.d_tid_count; a.err = s.d_err;
+  const uint32_t grid = (uint32_t)((n_pairs + 255) / 256);
+  if (n_pairs) ks_count<<<grid, 256, 0, c->stream>>>(a);
+  kf_scan<<<1, 1024, 0, c->stream>>>(s.d_tid_count, n_ref);
+  CU_TRY(c, cudaGetLastError());
+  unsigned long long h[2] = {~0ull, 0};
+  CU_TRY(c, cudaMemcpyAsync(&h[0], s.d_err, 8, cudaMemcpyDeviceToHost, c->stream));
+  CU_TRY(c, cudaMemcpyAsync(&h[1], s.d_tid_count + n_ref, 8, cudaMemcpyDeviceToHost, c->stream));
+  CU_TRY(c, cudaStreamSynchronize(c->stream));
+  unsigned long long key = h[0];
+  const unsigned long long phase_end = 0xfff;  // the reader's checks come after every kernel-found error of the same set
+  if (!equal) key = std::min(key, (n_min << 24) | (phase_end << 12) | (3ull << 8));
+  else if (n0 % 2) key = std::min(key, (n0 << 24) | (phase_end << 12) | (4ull << 8));
+  if (key != ~0ull && ((key >> 8) & 0xf) == 3)
+    return fail(c, CMB_E_SHARD_EXIT, "Unexpectedly one BAM file input finished while another had further reads");
+  if (key != ~0ull && ((key >> 8) & 0xf) == 4)
+    return fail(c, CMB_E_SHARD_PANIC, "Unexpectedly was able to read a first read set, but not a second. Hmm.");
+  if (int rc = shard_error(c, key)) return rc;
+  // ---- the winners, sorted by tid, into one device batch
+  const uint64_t n_out = h[1];
+  if (n_out >= 0xffffff00ull) return fail(c, CMB_E_ARG, "cmb_shard_finish: more than 2^32 mapped winners");
+  if (int rc = s.d_src.ensure(c, n_out + 1, with_slack(n_out + 1))) return rc;
+  if (int rc = s.d_slot_iv.ensure(c, n_out + 1, with_slack(n_out + 1))) return rc;
+  a.src = s.d_src; a.slot_iv = s.d_slot_iv; a.n_out = n_out;
+  if (n_pairs) ks_scatter<<<grid, 256, 0, c->stream>>>(a);
+  kf_scan<<<1, 1024, 0, c->stream>>>(s.d_slot_iv, (uint32_t)n_out);
+  unsigned long long n_iv = 0;
+  CU_TRY(c, cudaMemcpyAsync(&n_iv, s.d_slot_iv + n_out, 8, cudaMemcpyDeviceToHost, c->stream));
+  CU_TRY(c, cudaStreamSynchronize(c->stream));
+  size_t offs[13];
+  const size_t slab = batch_slab_bytes((uint32_t)n_out, (uint32_t)n_iv, offs);
+  if (int rc = s.d_out_slab.ensure(c, slab, slab + slab / 8)) return rc;
+  carve_batch(s.d_out_slab, (uint32_t)n_out, (uint32_t)n_iv, &a.out);
+  if (n_out) ks_gather<<<(uint32_t)((n_out + 255) / 256), 256, 0, c->stream>>>(a);
+  CU_TRY(c, cudaGetLastError());
+  CU_TRY(c, cudaEventRecord(s.ev[3], c->stream));
+  out->n_pairs = n_pairs;
+  out->n_records = 2 * n_pairs;
+  out->n_emitted = n_out;
+  out->n_intervals = n_iv;
+  out->store_bytes = shard_bytes(c);
+  out->ms_choose = s.ms_choose;
+  out->ms_decode = s.ms_decode;
+  CU_TRY(c, cudaEventSynchronize(s.ev[3]));
+  cudaEventElapsedTime(&out->ms_sort, s.ev[2], s.ev[3]);
+  if (!n_out) return CMB_OK;
+  return cmb_submit_device_batch(c, &a.out, (uint32_t)n_out, (uint32_t)n_iv);
+}

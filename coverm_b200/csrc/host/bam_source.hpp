@@ -10,6 +10,7 @@
 // Every BAM-format rule of the host lives here, once: opening an input (SAM converted to BAM), the BGZF block index,
 // the header, the record decoder, the walk of an in-memory record stream and the host's mate matching.
 #pragma once
+#include <functional>
 #include <fcntl.h>
 #include <sys/mman.h>
 #include <sys/stat.h>
@@ -84,6 +85,11 @@ struct InputSpec {
   std::string path;              // used for the sample name (file stem) and, when data == nullptr, opened
   const uint8_t* data = nullptr;
   size_t size = 0;
+  // --sharded: one sample made of these read-name-sorted shards (the same read set mapped to each reference shard), and which
+  // of the concatenated reference's contigs belong to excluded genomes (0 no, 1 yes, 2 its genome cannot be told)
+  std::vector<InputSpec> shards;
+  std::function<uint8_t(const std::string&)> excluded;
+  std::string unknown_genome_panic;  // the reference's panic when a candidate's first mate lies on a contig marked 2
 };
 
 // One decoded record, fixed part (everything the device tuple needs) + qname location for mate matching.

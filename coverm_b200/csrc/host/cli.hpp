@@ -3,8 +3,8 @@
 // Mirrors the reference's CLI surface for this path: flag names and defaults from src/cli.rs:1670-2582
 // (genome :1670-2263, contig :2265-2582), FilterParameters (coverm.rs:1648-1704), EstimatorsAndTaker
 // (coverm.rs:1315-1520), parse_percentage (coverm.rs:1296-1312), run_contig / run_genome (coverm.rs:2088-2131,
-// 1539-1628), per-gene coverage with --gff (coverm.rs:488-509, 1554-1590).  Read mapping, sharded BAMs, dereplication and
-// FASTA genome definitions are out of scope.
+// 1539-1628), per-gene coverage with --gff (coverm.rs:488-509, 1554-1590), sharded BAMs (--sharded, coverm.rs:96-239, 565-578).
+// Read mapping, dereplication and FASTA genome definitions are out of scope.
 //
 // Library-level switches (they expose the constructor arguments the reference's unit tests use directly;
 // contig.rs:290-322, genome.rs:940-1086):  --lib-estimators SPEC;SPEC  --lib-streaming  --lib-flags I,S,SEC
@@ -16,6 +16,7 @@
 #include <iostream>
 #include <sstream>
 #include <thread>
+#include <unordered_set>
 
 #include "drivers.hpp"
 #include "filter_command.hpp"
@@ -36,6 +37,8 @@ struct CliOptions {
   std::string output_format = "dense";
   std::optional<std::string> output_file, separator, genome_definition, lib_estimators, lib_flags, gff, gff_feature_type;
   bool single_genome = false, lib_streaming = false, print_reads_mapped = false, timing = false, quiet = false;
+  bool sharded = false;
+  std::optional<std::string> exclude_genomes_from_deshard;
   int threads = 1;
   int device = 0;
   int gpus = 1;  // > 1: every sample is range-partitioned by contig over GPUs device .. device+gpus-1 (one NCCL gather per sample)
@@ -112,6 +115,8 @@ inline CliOptions parse_cli(const std::vector<std::string>& args) {
     else if ((a == "-s" || a == "--separator") && o.sub == "genome") o.separator = value();
     else if (a == "--single-genome" && o.sub == "genome") o.single_genome = true;
     else if (a == "--genome-definition" && o.sub == "genome") o.genome_definition = value();
+    else if (a == "--sharded" && !filter_sub) o.sharded = true;
+    else if (a == "--exclude-genomes-from-deshard" && o.sub == "genome") o.exclude_genomes_from_deshard = value();
     else if (a == "--gff") o.gff = value();
     else if (a == "--gff-feature-type") o.gff_feature_type = value();
     else if (a == "-t" || a == "--threads") o.threads = std::stoi(value());
@@ -129,6 +134,7 @@ inline CliOptions parse_cli(const std::vector<std::string>& args) {
   if (!o.lib_flags && !o.proper_pairs_only &&
       (o.min_read_aligned_length_pair || o.min_read_percent_identity_pair || o.min_read_aligned_percent_pair))
     usage("the following required arguments were not provided: --proper-pairs-only");  // cli.rs `requires`
+  if (o.exclude_genomes_from_deshard && !o.sharded) usage("the following required arguments were not provided: --sharded");  // cli.rs:1698-1701
   if (o.output_format != "sparse" && o.output_format != "dense") usage("invalid value '" + o.output_format + "' for '--output-format'");
   if (o.bam_files.empty()) usage("--bam-files is required: this build implements the BAM-input coverage path only");
   return o;
@@ -305,6 +311,45 @@ inline Plan make_plan(const CliOptions& o) {
   return p;
 }
 
+// The sample's name: the file stem, or the shards' stems joined with '|' (shard_bam_reader.rs:536-551)
+inline std::string sample_name(const InputSpec& in) {
+  if (in.shards.empty()) return file_stem(in.path);
+  std::string name;
+  for (const InputSpec& s : in.shards) name += (name.empty() ? "" : "|") + file_stem(s.path);
+  return name;
+}
+
+// --exclude-genomes-from-deshard (coverm.rs:96-155, genome_exclusion.rs): genome names, one per line (empty lines skipped); a
+// contig is excluded when its genome -- the name up to the separator (-s), or its genome in the definition file -- is listed.
+// --single-genome excludes nothing.
+inline void sharded_exclusion(const CliOptions& o, InputSpec& all) {
+  if (!o.exclude_genomes_from_deshard) return;
+  std::ifstream f(*o.exclude_genomes_from_deshard, std::ios::binary);
+  if (!f) throw Panic("Failed to open file '" + *o.exclude_genomes_from_deshard + "' containing list of excluded genomes");
+  auto names = std::make_shared<std::unordered_set<std::string>>();
+  std::string line;
+  while (std::getline(f, line))
+    if (!line.empty()) names->insert(line);
+  if (names->empty() || o.single_genome) return;
+  if (o.separator) {
+    if (o.separator->size() != 1) usage("invalid value '" + *o.separator + "' for '--separator <separator>': too many characters in string");
+    const char sep = (*o.separator)[0];
+    all.excluded = [names, sep](const std::string& contig) -> uint8_t {
+      const size_t at = contig.find(sep);
+      if (at == std::string::npos) return 2;
+      return names->count(contig.substr(0, at)) ? 1 : 0;
+    };
+    all.unknown_genome_panic = "Contig name " + std::to_string((unsigned)(uint8_t)sep) +
+                               " does not contain split symbol, so cannot determine which genome it belongs to";
+  } else if (o.genome_definition) {
+    auto gc = std::make_shared<GenomesAndContigs>(read_genome_definition_file(*o.genome_definition));
+    all.excluded = [names, gc](const std::string& contig) -> uint8_t {
+      const auto it = gc->contig_to_genome.find(contig);
+      return it != gc->contig_to_genome.end() && names->count(gc->genomes[it->second]) ? 1 : 0;
+    };
+  }
+}
+
 // Runs one CLI invocation on one session (one rank).  `memory_inputs` optionally supplies BAM bytes for paths given with -b
 // (matched by path).
 inline CliResult run_cli_rank(const std::vector<std::string>& args, const std::vector<InputSpec>& memory_inputs, std::ostream& out,
@@ -376,6 +421,15 @@ inline CliResult run_cli_rank(const std::vector<std::string>& args, const std::v
       for (auto& m : memory_inputs)
         if (m.path == path) in = m;
       inputs.push_back(in);
+    }
+    // --sharded makes the BAMs one sample, unless a read filter is given: then the reference ignores it (coverm.rs:168-187, 546-563)
+    if (o.sharded && !plan.params.filtering) {
+      if (o.gpus > 1) throw ExitError(1, "--sharded input runs on one GPU: drop --gpus");
+      InputSpec all;
+      all.path = o.bam_files[0];
+      all.shards = inputs;
+      if (o.sub == "genome") sharded_exclusion(o, all);
+      inputs = {all};
     }
     const bool output_rank = !shared_session || shared_session->is_output_rank();  // multi-GPU: only rank 0 prints
     CoverageTaker taker = plan.taker == Plan::TakerKind::Streaming ? CoverageTaker::streaming(os)
@@ -452,7 +506,7 @@ inline CliResult run_cli_rank(const std::vector<std::string>& args, const std::v
     if (o.timing) err << "#timing_run\tdrivers_s=" << (t_print0 - t_driver0) << "\tprint_s=" << (now_s() - t_print0) << '\n';
     if (o.print_reads_mapped)
       for (size_t i = 0; i < res.reads_mapped.size(); ++i)
-        err << "#reads_mapped\t" << file_stem(o.bam_files[i]) << '\t' << res.reads_mapped[i].num_mapped_reads << '\t'
+        err << "#reads_mapped\t" << sample_name(inputs[i]) << '\t' << res.reads_mapped[i].num_mapped_reads << '\t'
             << res.reads_mapped[i].num_reads << '\n';
     if (o.timing)
       for (size_t i = 0; i < res.timings.size(); ++i) {

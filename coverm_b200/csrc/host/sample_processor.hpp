@@ -15,6 +15,11 @@
 extern "C" int cmb_set_genes_range(cmb_ctx* ctx, uint32_t n_contigs, const uint64_t* contig_len, uint32_t n_genes, const cmb_gene* genes,
                                    uint32_t tid_begin, uint32_t tid_end) __attribute__((weak));
 
+// Referenced weakly for the same reason: the emulator without the sharded-input entry points stops a --sharded run with an error.
+extern "C" int cmb_shard_begin(cmb_ctx* ctx, uint32_t n_shards, const uint32_t* tid_offsets, const uint8_t* excluded) __attribute__((weak));
+extern "C" int cmb_shard_add(cmb_ctx* ctx, const cmb_bgzf_input* in, cmb_bgzf_result* out) __attribute__((weak));
+extern "C" int cmb_shard_finish(cmb_ctx* ctx, cmb_shard_result* out) __attribute__((weak));
+
 namespace cmbh {
 
 // NVTX range of a host-side stage (cmb_nvtx_push / cmb_nvtx_pop of the device library; no-ops without a profiler)
@@ -74,7 +79,8 @@ struct SampleResult {
 
 [[noreturn]] inline void throw_device_error(cmb_ctx* ctx, int rc) {
   const std::string msg = cmb_last_error(ctx);
-  if (rc == CMB_E_UNSORTED || rc == CMB_E_NM || rc == CMB_E_BOUNDS) throw Panic(msg);
+  if (rc == CMB_E_UNSORTED || rc == CMB_E_NM || rc == CMB_E_BOUNDS || rc == CMB_E_SHARD_PANIC) throw Panic(msg);
+  if (rc == CMB_E_SHARD_EXIT) throw ExitError(1, msg);
   throw ExitError(1, "device error " + std::to_string(rc) + ": " + msg);
 }
 
@@ -152,6 +158,10 @@ class DeviceSession {
 
   // One sample.  In a group every rank must call this for the same input (it is collective).
   SampleResult process(const InputSpec& in, const cmb_params& params) {
+    if (!in.shards.empty()) {
+      if (group_n_ > 1) throw ExitError(1, "--sharded input runs on one GPU: drop --gpus");
+      return process_sharded(in, params);
+    }
     if (group_n_ <= 1) return process_local(in, params, nullptr);
     // ---- local phase: this rank's contigs, from this rank's block range.  Nothing may escape before the ranks have
     //      compared notes: a rank that failed still takes part in the exchange, and then every rank fails the same way.
@@ -351,6 +361,102 @@ class DeviceSession {
     }
     if (!c.decoded_on_device && c.pair_mode) c.pair_fallback();
     return c.end_sample();
+  }
+
+  // --sharded (ReadSortedShardedBamReader, shard_bam_reader.rs): the shards' headers concatenated into one reference, every
+  // shard decoded on the device in turn, each pair's best shard chosen there and the winners accumulated as one sample.
+  SampleResult process_sharded(const InputSpec& in, const cmb_params& params) {
+    HostRange nvtx_sample("host: sharded sample");
+    const double t0 = now_s();
+    if (!cmb_shard_begin || !cmb_shard_add || !cmb_shard_finish) throw ExitError(1, "this device library has no cmb_shard_*: --sharded needs it");
+    if (set_params(params)) throw ExitError(1, "--sharded input takes no read-pair filter");
+    SampleResult res;
+    const size_t K = in.shards.size();
+    std::vector<uint32_t> offsets(K);
+    auto hdr = std::make_shared<Header>();
+    for (size_t k = 0; k < K; ++k) {  // the concatenated header (shard_bam_reader.rs:315-336)
+      res.stoit_name += (k ? "|" : "") + file_stem(in.shards[k].path);
+      const BamInput input(in.shards[k]);
+      InflateStream stream(input.data(), input.size(), pool_, 1u << 20);
+      std::vector<uint8_t> buf;
+      const BamHeader h = read_bam_header(stream, buf, in.shards[k].path);
+      offsets[k] = (uint32_t)hdr->names.size();
+      hdr->names.insert(hdr->names.end(), h.header->names.begin(), h.header->names.end());
+      hdr->lens.insert(hdr->lens.end(), h.header->lens.begin(), h.header->lens.end());
+    }
+    res.hdr = hdr;
+    const uint32_t n_ref = (uint32_t)hdr->names.size();
+    uint32_t n_rows = n_ref;
+    int rc;
+    if (gene_defs_) {
+      gene_cache_ = std::make_shared<ResolvedGenes>(resolve_genes_against_header(*gene_defs_, *hdr, gene_namer_));
+      gene_cache_names_ = hdr->names;
+      std::vector<cmb_gene> genes(gene_cache_->entries.size());
+      for (size_t g = 0; g < genes.size(); ++g) genes[g] = cmb_gene{gene_cache_->entries[g].tid, gene_cache_->entries[g].start, gene_cache_->entries[g].end};
+      n_rows = std::max<uint32_t>(1, (uint32_t)genes.size());
+      rc = cmb_set_genes(ctx_, n_ref, hdr->lens.data(), (uint32_t)genes.size(), genes.data());
+      res.genes = gene_cache_;
+    } else {
+      SampleCall::check_layout_fits(hdr->lens, {0, n_ref});
+      rc = cmb_set_reference(ctx_, n_ref, hdr->lens.data(), 0, n_ref);
+    }
+    if (rc) throw_device_error(ctx_, rc);
+    ref_lens_.clear();  // the next ordinary sample sets its own reference
+    gene_cache_names_.clear();
+    if ((rc = cmb_begin_sample(ctx_))) throw_device_error(ctx_, rc);
+    std::vector<uint8_t> excluded;
+    if (in.excluded) {
+      excluded.resize(n_ref);
+      for (uint32_t t = 0; t < n_ref; ++t) excluded[t] = in.excluded(hdr->names[t]);
+    }
+    if ((rc = cmb_shard_begin(ctx_, (uint32_t)K, offsets.data(), in.excluded ? excluded.data() : nullptr))) throw_device_error(ctx_, rc);
+    double decode_s = 0;
+    for (size_t k = 0; k < K; ++k) {
+      const double a = now_s();
+      const BamInput input(in.shards[k]);
+      InflateStream stream(input.data(), input.size(), pool_, 1u << 20);
+      std::vector<uint8_t> buf;
+      const BamHeader h = read_bam_header(stream, buf, in.shards[k].path);
+      const BlockIndex& bx = stream.index();
+      if (!bx.bgzf) throw ExitError(1, "shard " + in.shards[k].path + " is not a BGZF-compressed BAM file: sharded input is decoded on the GPU only");
+      BgzfInput bi(bx, (uint32_t)h.header->names.size(), h.records_at, pool_.size());
+      cmb_bgzf_result br{};
+      rc = cmb_shard_add(ctx_, &bi.in, &br);
+      if (rc == CMB_E_DECLINED) throw ExitError(1, "cannot read shard " + in.shards[k].path + ": " + cmb_last_error(ctx_));
+      if (rc) throw_device_error(ctx_, rc);
+      res.n_records += br.n_records;
+      decode_s += now_s() - a;
+    }
+    cmb_shard_result sr{};
+    if ((rc = cmb_shard_finish(ctx_, &sr))) {
+      const std::string msg = cmb_last_error(ctx_);
+      if (msg.rfind("Contig name does not contain", 0) == 0 && !in.unknown_genome_panic.empty()) throw Panic(in.unknown_genome_panic);
+      throw_device_error(ctx_, rc);
+    }
+    res.num_detected_primary_alignments = sr.n_records;
+    if (getenv("CMB_PIPELINE_STATS"))
+      fprintf(stderr, "#reference_bytes\tshards=%zu\tshard_store=%llu\n#sharded\tpairs=%llu\temitted=%llu\tdecode_ms=%.3f\tchoose_ms=%.3f\tsort_ms=%.3f\n", K,
+              (unsigned long long)sr.store_bytes, (unsigned long long)sr.n_pairs, (unsigned long long)sr.n_emitted, sr.ms_decode, sr.ms_choose, sr.ms_sort);
+    const double t_dec = now_s();
+    ensure_rows(n_rows);
+    res.rows = rows_buf_;
+    uint64_t n_pairs = 0;
+    if ((rc = cmb_end_sample(ctx_, rows_buf_, nullptr, 0, &n_pairs))) throw_device_error(ctx_, rc);
+    if ((params.want & CMB_WANT_HIST_CSR) && n_pairs) {
+      res.pairs.resize(n_pairs);
+      if ((rc = cmb_fetch_pairs(ctx_, res.pairs.data(), n_pairs))) throw_device_error(ctx_, rc);
+    }
+    if (gene_defs_) {
+      res.contig_seen.assign((size_t)n_ref + 1, 0);
+      if ((rc = cmb_fetch_gene_extras(ctx_, res.contig_seen.data(), &res.kept_primary))) throw_device_error(ctx_, rc);
+    }
+    cmb_get_timing(ctx_, &res.timing.device);
+    res.timing.device_decode = true;
+    const double t1 = now_s();
+    res.timing.total_s = t1 - t0;
+    res.timing.decode_s = decode_s;
+    res.timing.end_sample_s = t1 - t_dec;
+    return res;
   }
 
   // One process_local call, handed from stage to stage.

@@ -298,6 +298,42 @@ int cmb_submit_bgzf(cmb_ctx* ctx, const cmb_bgzf_input* in, cmb_bgzf_result* out
  * (stored first mate, second mate) at the second mate's position; cmb_filter_fetch copies them (each with its 4-byte
  * block_size, ready to be written into a BAM stream) to the caller.  CMB_E_NM: the reference would have panicked in nm(). */
 int cmb_decode_bgzf(cmb_ctx* ctx, const cmb_bgzf_input* in, cmb_bgzf_result* out);
+/* ---- Sharded input (`--sharded`; ReadSortedShardedBamReader, src/shard_bam_reader.rs) ----
+ * One read set mapped separately against K reference shards: K read-name-sorted BAMs, every one holding every read pair.
+ * Pair j is primaries 2j and 2j+1 of every shard (shard_bam_reader.rs:55-129); for each pair the shard with the highest summed
+ * AS wins (ties: a deterministic uniform choice, the t-th tied candidate replacing the winner with probability 1/t drawn from a
+ * hash of the pair index and the shard), shards whose first mate lies on an excluded contig are not candidates
+ * (shard_bam_reader.rs:222-262).  The winners' records, their tids shifted into the concatenated layout, are sorted by tid on
+ * the device (counting sort) and accumulated like one reference-sorted sample (cmb_submit_device_batch).  The layout is the
+ * shards' headers concatenated in order (cmb_set_reference / cmb_set_genes as usual).  All three calls sit between
+ * cmb_begin_sample and cmb_end_sample, and need cmb_filter_mode.filter_pairs == 0 and filtering == 0 (with a read filter the
+ * reference ignores --sharded).
+ *   cmb_shard_begin: tid_offsets[k] = targets in shards 0..k-1; excluded = n_contigs bytes, or NULL: 1 = a contig of an excluded
+ *                    genome, 2 = a contig whose genome cannot be told (its name lacks the separator: the reference panics when a
+ *                    candidate's first mate lies there).
+ *   cmb_shard_add:   once per shard, in order: the shard is inflated and decoded on the device (cmb_decode_bgzf's stages), its
+ *                    primaries are kept in a per-shard store (about 41 B per primary + 8 B per CIGAR operation) and the running
+ *                    winner of every pair is updated.  A shard the device decoder declines is CMB_E_DECLINED: there is no host
+ *                    route for shards.
+ *   cmb_shard_finish: checks the shards' lengths, sorts and submits the winners, frees nothing (the stores are grow-only).
+ * Errors carry the reference's message: CMB_E_SHARD_EXIT where it exits with status 1, CMB_E_SHARD_PANIC where it panics, and
+ * CMB_E_NM for an NM tag the reference's clone rejects.  With several errors the one the reference meets first is reported. */
+#define CMB_E_SHARD_EXIT (-9)
+#define CMB_E_SHARD_PANIC (-10)
+typedef struct cmb_shard_result {
+  uint64_t n_pairs;        /* read pairs                                                          */
+  uint64_t n_records;      /* winners' records, 2 per pair: the sample's primaries (ReadsMapped)   */
+  uint64_t n_emitted;      /* mapped winners submitted to K1                                      */
+  uint64_t n_intervals;    /* their interval slots                                                */
+  uint64_t store_bytes;    /* device bytes of the per-shard stores, pair state and sorted batch    */
+  float ms_choose;         /* CUDA events: per-shard compaction + pair updates (summed over shards) */
+  float ms_sort;           /* winners, counting sort, gather                                      */
+  float ms_decode;         /* cmb_decode_bgzf stages, summed over shards                          */
+  uint32_t reserved;
+} cmb_shard_result;
+int cmb_shard_begin(cmb_ctx* ctx, uint32_t n_shards, const uint32_t* tid_offsets, const uint8_t* excluded);
+int cmb_shard_add(cmb_ctx* ctx, const cmb_bgzf_input* in, cmb_bgzf_result* out);
+int cmb_shard_finish(cmb_ctx* ctx, cmb_shard_result* out);
 int cmb_filter_plan(cmb_ctx* ctx, int inverse, uint64_t* n_records, uint64_t* n_bytes);
 int cmb_filter_fetch(cmb_ctx* ctx, uint8_t* records, uint64_t n_bytes);
 
