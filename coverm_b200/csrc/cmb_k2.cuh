@@ -9,8 +9,9 @@
 // so it is closed as one run; positions past the slot's contig's end are padding or contigs without events so far (depth 0).
 // The stretch before the first slot has the chunk's carry-in (K1b) as its depth in the chunk's first contig.
 //
-// Slots go 32 per round, one per lane.  A lane finds its slot's span from the bitmap words (arithmetic only), its contig by
-// bisection, and reads the span's 32 deltas (8 x LDS.128 through the 128-B swizzle), keeping their sum and the mask of
+// Slots go 32 per round, one per lane.  A lane reads its slot's span from the chunk's slot -> span table (built when the warp
+// enters the chunk), its contig from the chunk's contig table (contig mode; by bisection in global memory in gene mode and in
+// chunks with more contigs than the table holds), and reads the span's 32 deltas (8 x LDS.128 through the 128-B swizzle), keeping their sum and the mask of
 // non-zero positions.  The depth entering a slot is a segmented (by contig) warp scan of the slot totals, seeded with the
 // previous round's last slot (the chunk's first contig at its carry-in for round 0); no CTA barrier is involved.  Covered
 // bases, sum of depth and the depth histogram of the end-trimmed window are accumulated per run.  The histogram is a dense
@@ -71,8 +72,26 @@ constexpr uint32_t K2_STAGE_BYTES = K2_STAGE_CODES * 2;
 // a warp's buffers: a ring of K2_STAGES round buffers (arena), or one round buffer and K2_STAGES stages of bucket entries
 template <bool BUCKETS>
 __host__ __device__ constexpr uint32_t k2_warp_bytes() { return BUCKETS ? K2_BUF_BYTES + K2_STAGES * K2_STAGE_BYTES : K2_STAGES * K2_BUF_BYTES; }
+// Contig mode: the contigs of a chunk, [chunk_first[k], chunk_first[k + 1]], when there are at most K2_CHUNK_CONTIGS of them:
+// entry t is contig chunk_first[k] + t.  A contig is at least one span, so a chunk with more has contigs shorter than ~500
+// bases; such chunks, and gene mode (where the table pushed K2 into spills), find their contigs in global memory.
+constexpr uint32_t K2_CHUNK_CONTIGS = 16;
+struct K2ChunkContigs {
+  uint64_t bin[K2_CHUNK_CONTIGS + 1];  // bin_base (HIST only)
+  uint32_t start[K2_CHUNK_CONTIGS];    // off_span
+  uint32_t len[K2_CHUNK_CONTIGS];
+};
+// A warp's per-chunk tables: the contigs of the chunk being reduced, and the slot -> span tables (k2_span_table_lane) of the
+// fetch cursor's chunk [0] and of the one being reduced [1].
+struct K2WarpTables {
+  K2ChunkContigs ct;
+  uint8_t span[2][K2_CHUNK_SPANS];
+  uint8_t pre[2][8];
+};
+static_assert(sizeof(K2WarpTables) % 8 == 0, "the contig tables hold u64 bins");
 constexpr uint32_t K2_SMEM_MISC = K2_WARPS * K2_STAGES * 8 /*an mbarrier per (warp, stage)*/ +
-                                  K2_WARPS * 128 /*bitmap words of two chunks, bucket offsets of one*/;
+                                  K2_WARPS * 128 /*a chunk's bitmap words and bucket offsets*/ +
+                                  K2_WARPS * sizeof(K2WarpTables);
 template <bool BUCKETS>
 __host__ __device__ constexpr uint32_t k2_smem_bytes() { return K2_WARPS * k2_warp_bytes<BUCKETS>() + K2_SMEM_MISC; }
 static_assert(k2_warp_bytes<true>() % 1024 == 0 && k2_warp_bytes<false>() % 1024 == 0, "round buffers are whole swizzle atoms");
@@ -86,12 +105,12 @@ __global__ void __launch_bounds__(K2_THREADS, CMB_K2_MINBLOCKS) k2_scan_reduce(c
   constexpr uint32_t RING = K2_WARPS * k2_warp_bytes<BUCKETS>();
   uint8_t* ring = smem + warp * k2_warp_bytes<BUCKETS>();
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + RING) + warp * K2_STAGES;
-  // the 8 bitmap words of the chunk being fetched and of the one being reduced, and (BUCKETS) the 9 bucket offsets of the
-  // latter's words (in shared memory rather than registers: K2 runs at the 80-register cap)
+  // the 8 bitmap words of the chunk being reduced and (BUCKETS) the 9 bucket offsets of its words (in shared memory rather
+  // than registers: K2 runs at the 80-register cap); the fetch cursor needs only its chunk's slot -> span table
   uint32_t* words = reinterpret_cast<uint32_t*>(smem + RING + K2_WARPS * K2_STAGES * 8) + warp * 32;
-  uint32_t(&fw)[8] = *reinterpret_cast<uint32_t(*)[8]>(words);
   uint32_t(&w)[8] = *reinterpret_cast<uint32_t(*)[8]>(words + 8);
   uint32_t* wo = words + 16;
+  K2WarpTables& tb = reinterpret_cast<K2WarpTables*>(smem + RING + K2_WARPS * K2_STAGES * 8 + K2_WARPS * 128)[warp];
 
   // The pool is sized before the launch from a bound of bin_base[n_local]; when it is still too small (cmb_grow_buffers
   // then grows it to exactly that) no bin is added and K3 reads none.
@@ -103,14 +122,25 @@ __global__ void __launch_bounds__(K2_THREADS, CMB_K2_MINBLOCKS) k2_scan_reduce(c
   auto load_word = [&](uint32_t ck) -> uint32_t { return ck < a.n_chunks && lane < K2_WARPS ? a.span_bits[ck * K2_WARPS + lane] : 0u; };
   // BUCKETS: the first bucket entry of word `lane` (lanes 0..8, 8 = the next chunk's first) of chunk ck
   auto load_off = [&](uint32_t ck) -> uint32_t { return BUCKETS && ck < a.n_chunks && lane <= K2_WARPS ? __ldg(a.word_off + ck * K2_WARPS + lane) : 0u; };
-  // lanes 0..7 put their words of a chunk into `to` for the whole warp (and lanes 0..8 their bucket offsets into `to_off`);
-  // returns the chunk's popcount
-  auto spread = [&](uint32_t word, uint32_t* to, uint32_t off = 0, uint32_t* to_off = nullptr) -> uint32_t {
-    __syncwarp();  // every lane is done with the previous chunk's words
-    if (lane < K2_WARPS) to[lane] = word;
+  // lanes 0..7 put their words of a chunk into `to` for the whole warp (and lanes 0..8 their bucket offsets into `to_off`),
+  // and the warp writes the chunk's slot -> span table t; returns the chunk's popcount
+  auto spread = [&](uint32_t word, uint32_t* to, uint32_t t, uint32_t off = 0, uint32_t* to_off = nullptr) -> uint32_t {
+    __syncwarp();  // every lane is done with the previous chunk's words and table
+    if (to && lane < K2_WARPS) to[lane] = word;
     if (to_off && lane <= K2_WARPS) to_off[lane] = off;
+    const uint32_t pop = __reduce_add_sync(FULL, __popc(word));
+    const uint32_t mw = pop >= K2_DENSE_SPANS && lane < K2_WARPS ? ~0u : word;  // a dense chunk's slots are all its spans
+    uint32_t before = __popc(mw);  // lanes 0..7: slots of the words up to `lane`, then before it
+#pragma unroll
+    for (uint32_t d = 1; d < K2_WARPS; d <<= 1) {
+      const uint32_t o = __shfl_up_sync(FULL, before, d);
+      if (lane >= d) before += o;
+    }
+    before -= __popc(mw);
+    if (lane < K2_WARPS) tb.pre[t][lane] = (uint8_t)before;
+    k2_span_table_lane(__shfl_sync(FULL, mw, lane / 4), __shfl_sync(FULL, before, lane / 4), lane, tb.span[t]);
     __syncwarp();
-    return __reduce_add_sync(FULL, __popc(word));
+    return pop;
   };
 
   if (lane == 0) {
@@ -123,8 +153,7 @@ __global__ void __launch_bounds__(K2_THREADS, CMB_K2_MINBLOCKS) k2_scan_reduce(c
 
   // ---- the fetch cursor: round fr of chunk fk is the next one whose rows are requested.  It runs K2_STAGES - 1
   //      rounds ahead of the reduction, through the same chunks and rounds, skipping the chunks that have none.
-  uint32_t fk = g, fr = 0, fpop = 0;
-  bool fdense = false;
+  uint32_t fk = g, fr = 0, fns = 0;  // fns: the slots of chunk fk (CHUNK_SPANS when dense, so dense = fns >= K2_DENSE_SPANS)
   uint32_t f_word = load_word(fk);      // bitmap word of chunk fk, requested a chunk ahead
   uint32_t f_off = load_off(fk), fo = 0;  // BUCKETS: bucket offsets of chunk fk, requested a chunk ahead; of the cursor's chunk
   uint32_t n_loaded = 0, n_dense = 0, n_events = 0;  // what this warp fetched (load_stats)
@@ -134,12 +163,12 @@ __global__ void __launch_bounds__(K2_THREADS, CMB_K2_MINBLOCKS) k2_scan_reduce(c
       f_word = load_word(fk + W);
       fo = f_off;
       f_off = load_off(fk + W);
-      fpop = spread(word, fw);
-      fdense = fpop >= K2_DENSE_SPANS;
+      const uint32_t pop = spread(word, nullptr, 0);
+      fns = pop >= K2_DENSE_SPANS ? CHUNK_SPANS : pop;
       fr = 0;
-      if (k2_rounds(fpop, fdense)) {
-        n_loaded += fdense ? CHUNK_SPANS : fpop;
-        n_dense += fdense;
+      if (fns) {
+        n_loaded += fns;
+        n_dense += pop >= K2_DENSE_SPANS;
         return;
       }
     }
@@ -153,14 +182,14 @@ __global__ void __launch_bounds__(K2_THREADS, CMB_K2_MINBLOCKS) k2_scan_reduce(c
       if constexpr (BUCKETS) {  // contig mode has no arena and no tensor map: only the gene-mode branches name them
         // the round's bucket entries, 16-B units from the one holding its first entry, as many as the stage holds
         uint32_t wf, wl;
-        k2_round_words(fw, fdense ? CHUNK_SPANS : fpop, fdense, fr, wf, wl);
+        k2_round_words(tb.span[0], fns, fr, wf, wl);
         const uint32_t b0 = __shfl_sync(FULL, fo, wf), b1 = __shfl_sync(FULL, fo, wl + 1);
         const uint32_t base = b0 & ~7u, units = min((b1 - base + 7) / 8, K2_STAGE_CODES / 8);
         uint8_t* stg = ring + K2_BUF_BYTES + (fi % K2_STAGES) * K2_STAGE_BYTES;
         const int4* src = reinterpret_cast<const int4*>(a.buckets + base);
         for (uint32_t u = lane; u < units; u += 32) cp_async_16(smem_u32(stg + u * 16), src + u);
         n_events += b1 - b0;
-      } else if (fdense) {
+      } else if (fns >= K2_DENSE_SPANS) {
         if (lane == 0) {
           fence_proxy_async_smem();  // the stage's earlier reads and cp.async writes (ordered by __syncwarp) come first
           mbar_arrive_expect_tx(bar, K2_BUF_BYTES);
@@ -169,8 +198,8 @@ __global__ void __launch_bounds__(K2_THREADS, CMB_K2_MINBLOCKS) k2_scan_reduce(c
       } else {
         // lanes 8q..8q+7 take the eight 16-byte units of row r0 + q, so every instruction moves four whole 128-byte lines;
         // unit u of row r lands at r * 128 + (u ^ (r & 7)) * 16, where the TMA box would put it
-        const uint32_t n = min(K2_ROUND, fpop - fr * K2_ROUND);
-        const uint32_t sp = k2_slot_span(fw, fr * K2_ROUND + lane, false);
+        const uint32_t n = min(K2_ROUND, fns - fr * K2_ROUND);
+        const uint32_t jf = fr * K2_ROUND + lane, sp = jf < fns ? tb.span[0][jf] : 0u;
         const uint32_t q = lane >> 3, unit = lane & 7;
         const int4* src = reinterpret_cast<const int4*>(a.arena + (uint64_t)fk * CHUNK) + unit;
         for (uint32_t r0 = 0; r0 < n; r0 += 4) {
@@ -180,7 +209,7 @@ __global__ void __launch_bounds__(K2_THREADS, CMB_K2_MINBLOCKS) k2_scan_reduce(c
         }
         if (lane == 0) mbar_arrive(bar);  // keeps the barrier's phase in step with the TMA stages
       }
-      if (++fr == k2_rounds(fpop, fdense)) {
+      if (++fr == (fns + K2_ROUND - 1) / K2_ROUND) {
         fk += W;
         f_enter();
       }
@@ -230,7 +259,22 @@ __global__ void __launch_bounds__(K2_THREADS, CMB_K2_MINBLOCKS) k2_scan_reduce(c
       n_cl = __ldg(a.chunk_first + k + W + 1);
       n_cin = __ldg(a.carry_in + k + W);
     }
-    const uint32_t pop = spread(word, w, off, BUCKETS ? wo : nullptr);
+    // ---- the chunk's contigs cf..cl into the warp's table, entry `lane` (bins: lanes 0..cl - cf + 1), when they fit
+    const bool tabled = BUCKETS && cl - cf < K2_CHUNK_CONTIGS;
+    uint32_t t_start = 0, t_len = 0;
+    uint64_t t_bin = 0;
+    if (tabled && lane <= cl - cf) {
+      t_start = __ldg(a.off_span + cf + lane);
+      t_len = __ldg(a.len + cf + lane);
+    }
+    if (HIST && tabled && lane <= cl - cf + 1) t_bin = __ldg(a.bin_base + cf + lane);
+    const uint32_t pop = spread(word, w, 1, off, BUCKETS ? wo : nullptr);
+    if (tabled && lane <= cl - cf) {
+      tb.ct.start[lane] = t_start;
+      tb.ct.len[lane] = t_len;
+    }
+    if (HIST && tabled && lane <= cl - cf + 1) tb.ct.bin[lane] = t_bin;
+    __syncwarp();
     const bool dense = pop >= K2_DENSE_SPANS;
     const uint32_t nr = k2_rounds(pop, dense), nslots = dense ? CHUNK_SPANS : pop;
     const uint32_t span0 = k * CHUNK_SPANS;
@@ -241,12 +285,25 @@ __global__ void __launch_bounds__(K2_THREADS, CMB_K2_MINBLOCKS) k2_scan_reduce(c
       fill(i + K2_STAGES - 1);
       const uint32_t j = r * K2_ROUND + lane;
       const bool valid = j < nslots;
-      const uint32_t s = k2_slot_span(w, j, dense), sn = k2_slot_span(w, j + 1, dense);
-      // ---- the slot's contig, start, window and bins (no tile data needed: these loads fly while the rows arrive)
+      const uint32_t s = valid ? tb.span[1][j] : CHUNK_SPANS, sn = j + 1 < nslots ? tb.span[1][j + 1] : CHUNK_SPANS;
+      // ---- the slot's contig, start, window and bins: from the chunk's table, else by bisection in global memory (no tile
+      //      data needed: those loads fly while the rows arrive)
       uint32_t c = 0xffffffffu, cstart = 0;
       K2Win win{0u, 0u, 0u};
       uint64_t bin0 = 0, bin1 = 0;
-      if (valid) {
+      if (valid && tabled) {
+        uint32_t t = 0;  // the last entry that starts at or before the slot's span (entry 0 starts before the chunk)
+#pragma unroll
+        for (uint32_t h = K2_CHUNK_CONTIGS / 2; h; h >>= 1)
+          if (t + h <= cl - cf && tb.ct.start[t + h] <= span0 + s) t += h;
+        c = cf + t;
+        cstart = tb.ct.start[t];
+        win = k2_window(tb.ct.len[t], E);
+        if (hist) {
+          bin0 = tb.ct.bin[t];
+          bin1 = tb.ct.bin[t + 1];
+        }
+      } else if (valid) {
         uint32_t lo = cf, hi = cl;
         while (lo < hi) {
           const uint32_t mid = (lo + hi + 1) >> 1;
@@ -273,7 +330,7 @@ __global__ void __launch_bounds__(K2_THREADS, CMB_K2_MINBLOCKS) k2_scan_reduce(c
         const uint32_t base = wo[wf] & ~7u;
         const uint16_t* stg = reinterpret_cast<const uint16_t*>(ring + K2_BUF_BYTES + st * K2_STAGE_BYTES);
         k2_round_events(
-            w, wo, dense, r, wf, wl, lane, 32,
+            w, tb.pre[1], wo, dense, r, wf, wl, lane, 32,
             [&](uint32_t p) { return p - base < K2_STAGE_CODES ? (uint32_t)stg[p - base] : (uint32_t)__ldg(a.buckets + p); },
             [&](uint32_t rw, uint32_t e, int d) {
               atomicAdd(reinterpret_cast<int*>(rows + rw * 128 + (((e >> 2) ^ (rw & 7)) << 4) + ((e & 3) << 2)), d);
@@ -347,13 +404,14 @@ __global__ void __launch_bounds__(K2_THREADS, CMB_K2_MINBLOCKS) k2_scan_reduce(c
     // ---- the chunk's head when no slot took it: from the chunk start to the first slot (the whole chunk if it has none),
     //      at the carry-in, in the chunk's first contig
     if (lane == 0 && cin != 0 && c_first != cf) {
-      const uint32_t cstart = __ldg(a.off_span + cf);
-      const K2Win win = k2_window(__ldg(a.len + cf), E);
-      const uint32_t s0 = k2_slot_span(w, 0, dense);
+      const uint32_t cstart = tabled ? tb.ct.start[0] : __ldg(a.off_span + cf);
+      const K2Win win = k2_window(tabled ? tb.ct.len[0] : __ldg(a.len + cf), E);
+      const uint32_t s0 = nslots ? tb.span[1][0] : CHUNK_SPANS;
       K2Acc acc{0u, 0u, 0ull};
       uint32_t top = 0;
       const uint32_t nw = k2_close_run(acc, win, cin, (span0 - cstart) * SPAN, (span0 + s0 - cstart) * SPAN);
-      if (hist && nw) bin_add(__ldg(a.bin_base + cf), __ldg(a.bin_base + cf + 1), cin, nw, top);
+      if (hist && nw)
+        bin_add(tabled ? tb.ct.bin[0] : __ldg(a.bin_base + cf), tabled ? tb.ct.bin[1] : __ldg(a.bin_base + cf + 1), cin, nw, top);
       flush(cf, acc.cov_full, acc.cov_win, acc.sum_win, top);
     }
     if (CLEAN && word) a.span_bits[k * K2_WARPS + lane] = 0;  // lanes 0..7 (the others hold no word)

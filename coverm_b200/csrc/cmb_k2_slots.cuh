@@ -68,6 +68,19 @@ K2_HD uint32_t k2_slot_span(const uint32_t (&w)[8], uint32_t j, bool dense) {
   return found ? base + k2_nth_bit(word, rem) : K2_CHUNK_SPANS;
 }
 
+// ---- A chunk's slot -> span table, built once when K2 enters the chunk so that its rounds read spans instead of counting
+// bits: span[j] = k2_slot_span(w, j, dense) for j < nslots, and pre[q] = the slots of the words before word q (32 q when
+// dense).  Lane `lane` (0..31) writes the slots of byte lane % 4 of word q = lane / 4: `word` is w[q] (all ones when the
+// chunk is dense) and `before` is pre[q].
+K2_HD void k2_span_table_lane(uint32_t word, uint32_t before, uint32_t lane, uint8_t* span) {
+  const uint32_t q = lane / 4, sh = (lane % 4) * 8;
+  uint32_t m = (word >> sh) & 255u, j = before + k2_popc(word & ((1u << sh) - 1u));
+  while (m) {
+    span[j++] = (uint8_t)(32 * q + sh + k2_low_bit(m));
+    m &= m - 1;
+  }
+}
+
 // ---- A round's rows from word buckets (contig mode).  K1e puts each event of bitmap word q of a chunk into the word's bucket
 // as the u16 code (element % 1024) | sign << 10 (sign 1: the -1 at a block's end); the bucket of word q is the entries
 // [wo[q], wo[q + 1]).  Row i of round r is slot 32 r + i: span 32 r + i of a dense chunk, else the (32 r + i)-th occupied span.
@@ -77,6 +90,12 @@ K2_HD void k2_round_words(const uint32_t (&w)[8], uint32_t nslots, bool dense, u
   const uint32_t j1 = r * 32 + 31 < nslots ? r * 32 + 31 : nslots - 1;
   wf = k2_slot_span(w, r * 32, dense) / 32;
   wl = k2_slot_span(w, j1, dense) / 32;
+}
+// The same from the chunk's slot -> span table
+K2_HD void k2_round_words(const uint8_t* span, uint32_t nslots, uint32_t r, uint32_t& wf, uint32_t& wl) {
+  const uint32_t j1 = r * 32 + 31 < nslots ? r * 32 + 31 : nslots - 1;
+  wf = span[r * 32] / 32u;
+  wl = span[j1] / 32u;
 }
 
 // Row of round r for an event of word q with code `code`, `before` the slots of the words before q: its span's slot minus
@@ -89,19 +108,26 @@ K2_HD uint32_t k2_bucket_row(const uint32_t (&w)[8], bool dense, uint32_t r, uin
 
 // The events of round r, whose slots lie in words wf..wl: bucket entries p = wo[wf] + p0, + step, ... below wo[wl + 1]
 // (K2: p0 = lane, step = 32).  code(p) reads entry p; add(row, e, delta) is called for each event of the round's slots, e
-// its position in the span.
+// its position in the span.  pre[q] is the slots of the words before word q (the chunk's table, k2_span_table_lane).
 template <class Code, class Add>
-K2_HD void k2_round_events(const uint32_t (&w)[8], const uint32_t* wo, bool dense, uint32_t r, uint32_t wf, uint32_t wl,
-                           uint32_t p0, uint32_t step, Code code, Add add) {
-  uint32_t q = wf, before = 0;  // the word of entry p and the slots of the words before it
-  for (uint32_t x = 0; x < wf; ++x) before += k2_popc(w[x]);
+K2_HD void k2_round_events(const uint32_t (&w)[8], const uint8_t* pre, const uint32_t* wo, bool dense, uint32_t r, uint32_t wf,
+                           uint32_t wl, uint32_t p0, uint32_t step, Code code, Add add) {
+  uint32_t q = wf, before = pre[wf];  // the word of entry p and the slots of the words before it
   const uint32_t p1 = wo[wl + 1];
   for (uint32_t p = wo[wf] + p0; p < p1; p += step) {
-    while (q < wl && wo[q + 1] <= p) before += k2_popc(w[q++]);
+    while (q < wl && wo[q + 1] <= p) before = pre[++q];
     const uint32_t c = code(p);
     const uint32_t row = k2_bucket_row(w, dense, r, q, before, c);
     if (row < 32) add(row, c & 31u, (c >> 10) & 1u ? -1 : 1);
   }
+}
+// The same with pre[] counted from the bitmap words
+template <class Code, class Add>
+K2_HD void k2_round_events(const uint32_t (&w)[8], const uint32_t* wo, bool dense, uint32_t r, uint32_t wf, uint32_t wl,
+                           uint32_t p0, uint32_t step, Code code, Add add) {
+  uint8_t pre[8];
+  for (uint32_t q = 0, before = 0; q < 8; before += k2_popc(w[q++])) pre[q] = (uint8_t)before;
+  k2_round_events(w, pre, wo, dense, r, wf, wl, p0, step, code, add);
 }
 
 // A contig's length and its end-trimmed window [w0, w1) (empty when 2E >= L), in contig coordinates.
