@@ -90,6 +90,7 @@ namespace {
 #include "cmb_pairs.cuh"
 #include "cmb_filter.cuh"
 #include "cmb_shards.cuh"
+#include "cmb_shard_slices.hpp"
 
 // rows[i].hist_offset += base for the rows that carry histogram pairs (cmb_allgather_stats: local -> global pair offsets)
 __global__ void __launch_bounds__(256) k_rebase_hist_offsets(cmb_contig_stats* rows, uint32_t n, uint64_t base) {
@@ -282,11 +283,17 @@ struct cmb_ctx {
   } dec;
   // sharded input (cmb_shard_*; cmb_shards.cuh): per-shard primary stores and the running choice of every pair; grow-only
   struct Shards {
-    struct Store {
-      Buf<uint8_t> slab;  // carved as a cmb_read_batch over the shard's primaries
-      Buf<uint8_t> info;
+    struct Store {  // one buffer per column, each grown in place (Buf::grow_keep) as the shard's slices append primaries
+      Buf<int32_t> tid, pos, iv_start, iv_len;
+      Buf<uint32_t> nm, l_seq, aligned, del, ins, iv_begin;
+      Buf<uint16_t> flag;
+      Buf<uint8_t> mapq, nm_state, info;
       ShardStore view{};
       uint64_t n_prim = 0, n_iv = 0;
+      uint64_t bytes() const {
+        return tid.bytes() + pos.bytes() + iv_start.bytes() + iv_len.bytes() + nm.bytes() + l_seq.bytes() + aligned.bytes() + del.bytes() +
+               ins.bytes() + iv_begin.bytes() + flag.bytes() + mapq.bytes() + nm_state.bytes() + info.bytes();
+      }
     };
     std::vector<Store> store;
     std::vector<int32_t> tid_offsets;
@@ -1500,6 +1507,9 @@ struct BgzfCall {
   uint32_t n_copy_threads = 0;
   bool src_pinned = false;
   uint64_t n_rec = 0, n_cig = 0;
+  uint64_t tail_bytes = DEC_TAIL_BYTES;  // ranged: inflated bytes uploaded beyond walk_end
+  bool tail_short = false;               // ranged: a record runs past the tail (a longer tail may decode it)
+  uint64_t exit_off = 0;                 // end of the last record that starts in the range: the next range's records_at
 
   InflateArgs inflate_args(uint32_t b0, uint32_t b1) const;
   int prepare();
@@ -1536,7 +1546,7 @@ int BgzfCall::prepare() {
     if (walk_end == first_block) return CMB_OK;  // an empty share
     data_end = walk_end;
     uint64_t tail = 0;
-    while (data_end < nb && tail < DEC_TAIL_BYTES) tail += in->block_isize[data_end++];
+    while (data_end < nb && tail < tail_bytes) tail += in->block_isize[data_end++];
   }
   nothing_to_decode = false;
   byte_lo = in->block_coffset[first_block];
@@ -1839,9 +1849,12 @@ int BgzfCall::chain() {
     kd_walk<<<(nwb + 127) / 128, 128, 0, c->stream>>>(wa);
     CU_TRY(c, cudaGetLastError());
   }
-  if (walk_end == nb ? h_exit != ustart[nb] : (h_exit == WALK_UNKNOWN || h_exit > total))
+  if (walk_end == nb ? h_exit != ustart[nb] : (h_exit == WALK_UNKNOWN || h_exit > total)) {
+    tail_short = walk_end != nb && data_end < nb;
     return fail(c, CMB_E_DECLINED, walk_end == nb ? "cmb_submit_bgzf: record chain does not end at the end of the stream"
                                                   : "cmb_submit_bgzf: a record runs past the inflated tail of the block range");
+  }
+  exit_off = h_exit;
   kd_scan_items<<<1, 1024, 0, c->stream>>>(d.d_nrec, d.d_ncig, first_block, walk_end, d.d_rec_base, d.d_cig_base, (uint64_t*)(d.d_cnt + 6));
   CU_TRY(c, cudaGetLastError());
   out->n_launches += 1;
@@ -2080,26 +2093,258 @@ int shard_event(cmb_ctx* c, int i) {
   return CMB_OK;
 }
 
-// cmb_decode_bgzf's stages inside a sample: the shard's records inflated, located and reduced to tuples in device memory
+uint64_t shard_bytes(const cmb_ctx* c);
+
+constexpr uint64_t SLICE_TAIL_BYTES = 64u << 10;  // a slice's first tail: one BGZF block; doubled for a longer record
+constexpr int SLICE_HALVINGS = 8;                 // a slice whose buffers fail to allocate is halved this often before giving up
+constexpr uint64_t SLICE_MIN_BYTES = 64u << 20;   // budget floor: below it a failed allocation, not the estimate, shrinks a slice
+
+// CMB_DECODE_MEM_LIMIT_MB (testing aid): behave as if the device had this much room for the sharded sample -- its stores and
+// one slice's compressed and inflated bytes; a fraction of a megabyte slices small files.  0 when unset.
+uint64_t shard_mem_limit() {
+  const char* lim = getenv("CMB_DECODE_MEM_LIMIT_MB");
+  return lim ? (uint64_t)(std::max(0.0, strtod(lim, nullptr)) * 1048576.0) : 0;
+}
+
+// The decode buffers a slice fills (d_scan included); released when a store cannot grow beside them
+uint64_t decode_bytes(const cmb_ctx* c) {
+  const auto& d = c->dec;
+  return d.d_comp.bytes() + d.d_inflated.bytes() + d.d_tuple_slab.bytes() + d.d_rec_off.bytes() + c->sh.d_scan.bytes();
+}
+// The buffers shard_need counts: stores, AS scratch, name hashes, pair state
+uint64_t store_bytes_held(const cmb_ctx* c) {
+  const auto& s = c->sh;
+  uint64_t b = s.d_as_val.bytes() + s.d_as_state.bytes() + s.d_hash0.bytes() + s.d_state.bytes();
+  for (const auto& st : s.store) b += st.bytes();
+  return b;
+}
+void release_decode(cmb_ctx* c) {
+  cudaGetLastError();
+  auto& d = c->dec;
+  d.d_comp.release();
+  d.d_inflated.release();
+  d.d_tuple_slab.release();
+  d.d_rec_off.release();
+  c->sh.d_scan.release();
+}
+
+// Bytes the sharded sample needs beyond its decode buffers when shard k holds n_prim primaries and n_iv interval slots: the
+// stores (37 B per primary, 8 B per interval slot), AS scratch (5 B per primary of the largest shard), shard 0's name hashes
+// and the pair state (8 + 8 B per primary), and the n_out sorted winners with their n_out_iv slots (52 B and 8 B)
+uint64_t shard_need(const cmb_ctx* c, uint32_t k, uint64_t n_prim, uint64_t n_iv, uint64_t n_out = 0, uint64_t n_out_iv = 0) {
+  const auto& s = c->sh;
+  uint64_t b = 37 * n_prim + 8 * n_iv, as = n_prim;
+  for (uint32_t i = 0; i < k; ++i) {
+    b += 37 * s.store[i].n_prim + 8 * s.store[i].n_iv;
+    as = std::max(as, s.store[i].n_prim);
+  }
+  return b + 5 * as + 16 * (k ? s.store[0].n_prim : n_prim) + 52 * n_out + 8 * n_out_iv;
+}
+
+// Bytes the device has for them and a slice: the limit under CMB_DECODE_MEM_LIMIT_MB, else what is free plus the stores and
+// decode buffers the sample holds (the sorted winners' buffers of an earlier sample are not counted: they stay allocated)
+uint64_t shard_room(const cmb_ctx* c) {
+  if (const uint64_t lim = shard_mem_limit()) return lim;
+  size_t free_b = 0, total_b = 0;
+  cudaMemGetInfo(&free_b, &total_b);
+  cudaGetLastError();
+  return free_b + store_bytes_held(c) + decode_bytes(c);
+}
+
+int shard_nomem(cmb_ctx* c, uint64_t need) {
+  return fail(c, CMB_E_NOMEM, "sharded input needs %llu bytes of device memory for its shard stores, pair state, name hashes, AS scratch and "
+              "sorted winners; the device has %llu bytes free for them", (unsigned long long)need, (unsigned long long)shard_room(c));
+}
+
+// `alloc` once, and again after the decode buffers are released; CMB_E_NOMEM with the sample's need when it still fails
+template <class F>
+int shard_alloc(cmb_ctx* c, uint64_t need, F alloc) {
+  if (const uint64_t lim = shard_mem_limit(); lim && need > lim) return shard_nomem(c, need);
+  int rc = alloc();
+  if (rc != CMB_E_NOMEM) return rc;
+  release_decode(c);
+  rc = alloc();
+  if (rc == CMB_E_NOMEM) {
+    cudaGetLastError();
+    return shard_nomem(c, need);
+  }
+  return rc;
+}
+
+// Room for `need` elements keeping the first `used`; `hint` (the shard's expected total) is allocated at once when it fits, so
+// that a sliced shard grows each column about once instead of once per slice
+template <class T>
+int grow_col(cmb_ctx* c, Buf<T>& b, uint64_t used, uint64_t need, uint64_t hint = 0) {
+  if (b.p && b.cap >= need) return CMB_OK;
+  if (hint > need && b.grow_keep(c, used, with_slack(hint), c->stream) == CMB_OK) return CMB_OK;
+  cudaGetLastError();
+  return b.grow_keep(c, used, with_slack(need), c->stream);
+}
+
+// Room in the store for n_prim primaries and n_iv interval slots, keeping what it holds; the view follows the columns
+int store_grow(cmb_ctx* c, cmb_ctx::Shards::Store& st, uint64_t n_prim, uint64_t n_iv, uint64_t hint_prim = 0, uint64_t hint_iv = 0) {
+  const uint64_t r = st.n_prim, v = st.n_iv, h = hint_prim;
+  int rc;
+  if ((rc = grow_col(c, st.tid, r, n_prim, h)) || (rc = grow_col(c, st.pos, r, n_prim, h)) || (rc = grow_col(c, st.nm, r, n_prim, h)) ||
+      (rc = grow_col(c, st.l_seq, r, n_prim, h)) || (rc = grow_col(c, st.aligned, r, n_prim, h)) || (rc = grow_col(c, st.del, r, n_prim, h)) ||
+      (rc = grow_col(c, st.ins, r, n_prim, h)) || (rc = grow_col(c, st.iv_begin, r, n_prim + 1, h + 1)) || (rc = grow_col(c, st.flag, r, n_prim, h)) ||
+      (rc = grow_col(c, st.mapq, r, n_prim, h)) || (rc = grow_col(c, st.nm_state, r, n_prim, h)) || (rc = grow_col(c, st.info, r, n_prim, h)) ||
+      (rc = grow_col(c, st.iv_start, v, n_iv, hint_iv)) || (rc = grow_col(c, st.iv_len, v, n_iv, hint_iv)))
+    return rc;
+  cmb_read_batch& b = st.view.b;
+  b.capacity_records = (uint32_t)std::min<size_t>(st.tid.cap, UINT32_MAX);
+  b.capacity_intervals = (uint32_t)std::min<size_t>(st.iv_start.cap, UINT32_MAX);
+  b.tid = st.tid; b.pos = st.pos; b.nm = st.nm; b.l_seq = st.l_seq; b.aligned = st.aligned; b.del = st.del; b.ins = st.ins;
+  b.iv_begin = st.iv_begin; b.iv_start = st.iv_start; b.iv_len = st.iv_len; b.flag = st.flag; b.mapq = st.mapq; b.nm_state = st.nm_state;
+  st.view.info = st.info;
+  return CMB_OK;
+}
+
+// Shard k's slices (cmb_decode_bgzf's stages over a block range each): every slice's primaries appended to the store, AS
+// scratch and (shard 0) name hashes; `out` sums the slices' results
 int decode_shard(cmb_ctx* c, const cmb_bgzf_input* in, cmb_bgzf_result* out, uint32_t k) {
+  auto& s = c->sh;
+  auto& d = c->dec;
+  auto& st = s.store[k];
   c->dec.last_valid = false;
   c->dec.filter_planned = false;
   *out = cmb_bgzf_result{};
+  st.n_prim = st.n_iv = 0;
   if (in->n_blocks == 0 || in->ranged) return fail(c, CMB_E_ARG, "cmb_shard_add: shard %u: a whole BGZF file is needed", k);
-  BgzfCall j{c, c->dec, in, out, true, in->n_blocks};
-  int rc = j.prepare();
-  if (!rc && !j.nothing_to_decode && !(rc = j.copy_inflate()) && !(rc = j.declined()) && !(rc = j.chain())) rc = j.extract();
-  if (rc == CMB_E_NOMEM) {
-    cudaGetLastError();
-    return fail(c, CMB_E_DECLINED, "shard %u: not enough device memory to decode it", k);
+  const uint32_t nb = in->n_blocks;
+  std::vector<uint64_t> ustart((size_t)nb + 1, 0);
+  for (uint32_t b = 0; b < nb; ++b) ustart[b + 1] = ustart[b] + in->block_isize[b];
+  const ShardBlocks blocks{nb, in->size, in->block_coffset, in->block_clen, ustart.data()};
+  const uint64_t lim = shard_mem_limit();
+  const uint64_t n0 = k ? s.store[0].n_prim : 0, iv0 = k ? s.store[0].n_iv : 0;
+  uint64_t at = in->records_at, tail = SLICE_TAIL_BYTES, max_slice = 0;
+  uint32_t n_slices = 0;
+  float ms_inflate = 0, ms_chain = 0, ms_extract = 0, ms_grow = 0;
+  int halvings = 0;
+  uint32_t cap_end = nb;  // a slice end forced lower by a failed allocation (cleared once a slice decodes)
+  while (at < ustart[nb]) {
+    // ---- the slice: from the block holding `at`, as many blocks as the budget allows
+    const uint32_t b0 = (uint32_t)(std::upper_bound(ustart.begin(), ustart.end(), at) - ustart.begin()) - 1;
+    const uint64_t need_now = shard_need(c, k, st.n_prim, st.n_iv);
+    // What the sample is still expected to need: this shard's rest, the later shards' stores like shard 0's, and the sorted
+    // winners (at most one record per primary of a shard, 60 B each with an interval slot).  Shard 0's first slice has no
+    // estimate: like a whole-shard decode it takes what is free, and a failed allocation halves it.
+    uint64_t expect = 0;
+    if (k) {
+      expect = 37 * (n0 > st.n_prim ? n0 - st.n_prim : 0) + 8 * (iv0 > st.n_iv ? iv0 - st.n_iv : 0) + (s.n_shards - 1 - k) * (37 * n0 + 8 * iv0) +
+               60 * n0;
+    } else if (at > in->records_at) {  // shard 0: scaled by the inflated bytes its slices so far held
+      const double scale = (double)(ustart[nb] - in->records_at) / (double)(at - in->records_at);
+      const double total = need_now * scale, store = (37.0 * st.n_prim + 8.0 * st.n_iv) * scale, winners = 60.0 * st.n_prim * scale;
+      expect = (uint64_t)(total - need_now + store * (s.n_shards - 1) + winners);
+    }
+    const uint64_t room = shard_room(c), held = need_now + expect;
+    uint64_t budget = room > held ? room - held : 0;
+    budget = std::max(budget, lim ? lim / 64 : SLICE_MIN_BYTES);
+    bool over = false;
+    uint32_t b1 = std::min(slice_end(blocks, b0, budget, tail, &over), std::max(cap_end, b0 + 1));
+    // ---- decode it: halved when its buffers do not fit, the tail doubled when a record runs past it
+    cmb_bgzf_input si = *in;
+    si.ranged = 1; si.records_at = at; si.walk_begin_block = b0; si.walk_end_block = b1;
+    si.own_tid_begin = INT_MIN; si.own_tid_end = INT_MAX; si.own_unplaced = 1; si.excl_end_block = b1;
+    cmb_bgzf_result r{};
+    BgzfCall j{c, d, &si, &r, true, nb};
+    j.tail_bytes = tail;
+    int rc = j.prepare();
+    if (!rc && !j.nothing_to_decode && !(rc = j.copy_inflate()) && !(rc = j.declined()) && !(rc = j.chain())) rc = j.extract();
+    if (rc == CMB_E_NOMEM) {
+      release_decode(c);
+      if (b1 - b0 > 1 && halvings < SLICE_HALVINGS) {
+        ++halvings;
+        cap_end = b0 + (b1 - b0) / 2;
+        continue;
+      }
+      return fail(c, CMB_E_NOMEM, "shard %u: not enough device memory to decode blocks %u..%u (%llu bytes); the sharded sample holds %llu bytes", k, b0, b1,
+                  (unsigned long long)slice_bytes(blocks, b0, b1, tail), (unsigned long long)need_now);
+    }
+    if (rc == CMB_E_DECLINED && j.tail_short) {
+      tail *= 2;
+      continue;
+    }
+    if (rc == CMB_E_DECLINED) return fail(c, CMB_E_DECLINED, "shard %u: the device decoder declined it (%s); sharded input is decoded on the device only", k, c->err.c_str());
+    if (rc) return rc;
+    if (j.nothing_to_decode) break;
+    CU_TRY(c, cudaEventSynchronize(d.ev[4]));
+    cudaEventElapsedTime(&r.ms_total, d.ev[0], d.ev[4]);
+    cudaEventElapsedTime(&r.ms_copy_inflate, d.ev[0], d.ev[2]);
+    cudaEventElapsedTime(&r.ms_chain, d.ev[2], d.ev[3]);
+    cudaEventElapsedTime(&r.ms_extract, d.ev[3], d.ev[4]);
+    const uint64_t n_rec = j.n_rec;
+    if (!n_rec || j.exit_off <= at) return fail(c, CMB_E_DECLINED, "shard %u: the slice from block %u decoded no record", k, b0);
+    // ---- which records are primaries, and where their tuples and intervals go
+    CU_TRY(c, cudaEventRecord(s.ev[0], c->stream));
+    if ((rc = s.d_scan.ensure(c, n_rec + 1, with_slack(n_rec + 1))) == CMB_E_NOMEM) {  // part of the slice: halve it like its other buffers
+      release_decode(c);
+      if (b1 - b0 > 1 && halvings < SLICE_HALVINGS) {
+        ++halvings;
+        cap_end = b0 + (b1 - b0) / 2;
+        continue;
+      }
+      return fail(c, CMB_E_NOMEM, "shard %u: not enough device memory to scan the records of blocks %u..%u", k, b0, b1);
+    }
+    if (rc) return rc;
+    ShardScanArgs a{};
+    a.data = d.last_infl_base; a.rec_off = d.d_rec_off; a.n_records = n_rec; a.scan = s.d_scan;
+    a.shard = k; a.tid_offset = s.tid_offsets[k]; a.err = s.d_err;
+    carve_batch(d.d_tuple_slab, (uint32_t)n_rec, (uint32_t)j.n_cig, &a.tb);
+    ks_mark<<<(uint32_t)((n_rec + 255) / 256), 256, 0, c->stream>>>(a);
+    kf_scan<<<1, 1024, 0, c->stream>>>(s.d_scan, (uint32_t)n_rec);
+    CU_TRY(c, cudaGetLastError());
+    unsigned long long packed = 0;
+    CU_TRY(c, cudaMemcpyAsync(&packed, s.d_scan + n_rec, 8, cudaMemcpyDeviceToHost, c->stream));
+    CU_TRY(c, cudaStreamSynchronize(c->stream));
+    const uint64_t n_prim = st.n_prim + (packed >> 32), n_iv = st.n_iv + (uint32_t)packed;
+    if (n_iv >= 0xffffff00ull) return fail(c, CMB_E_ARG, "cmb_shard_add: shard %u: more than 2^32 CIGAR operations in its primaries", k);
+    // ---- room for them in the store, the AS scratch and (shard 0) the name hashes; without the decode buffers the slice is
+    // decoded again
+    // The expected totals: shard 0's, for shard k > 0; for shard 0, its slices so far scaled by the inflated bytes they cover
+    const double scale = (double)(ustart[nb] - in->records_at) / (double)(j.exit_off - in->records_at);
+    const uint64_t hint_prim = k ? n0 : (uint64_t)(n_prim * scale), hint_iv = k ? iv0 : (uint64_t)(n_iv * scale);
+    bool released = false;
+    const auto g0 = std::chrono::steady_clock::now();
+    auto grow = [&]() -> int {
+      int e;
+      if ((e = store_grow(c, st, n_prim, n_iv, hint_prim, hint_iv)) || (e = grow_col(c, s.d_as_val, st.n_prim, n_prim + 1, hint_prim + 1)) ||
+          (e = grow_col(c, s.d_as_state, st.n_prim, n_prim + 1, hint_prim + 1)) ||
+          (k == 0 && (e = grow_col(c, s.d_hash0, st.n_prim, n_prim + 1, hint_prim + 1))))
+        released = released || e == CMB_E_NOMEM;
+      return e;
+    };
+    if ((rc = shard_alloc(c, shard_need(c, k, n_prim, n_iv), grow))) return rc;
+    ms_grow += std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - g0).count();
+    if (released) continue;
+    a.st = st.view; a.prim_base = st.n_prim; a.iv_base = (uint32_t)st.n_iv;
+    a.as_val = s.d_as_val; a.as_state = s.d_as_state; a.hash0 = s.d_hash0; a.n0 = n0;
+    ks_compact<<<(uint32_t)((n_rec + 255) / 256), 256, 0, c->stream>>>(a);
+    CU_TRY(c, cudaGetLastError());
+    CU_TRY(c, cudaEventRecord(s.ev[1], c->stream));
+    CU_TRY(c, cudaEventSynchronize(s.ev[1]));
+    float ms = 0;
+    cudaEventElapsedTime(&ms, s.ev[0], s.ev[1]);
+    s.ms_choose += ms;
+    st.n_prim = n_prim;
+    st.n_iv = n_iv;
+    // ---- the slice's result into the shard's
+    out->n_records += r.n_records; out->n_primary += r.n_primary; out->n_intervals += r.n_intervals;
+    out->n_blocks_host += r.n_blocks_host; out->chain_repairs += r.chain_repairs; out->n_launches += r.n_launches;
+    out->n_blocks_second_pass += r.n_blocks_second_pass; out->h2d_bytes += r.h2d_bytes;
+    out->ms_copy_enqueue_wall += r.ms_copy_enqueue_wall; out->ms_total += r.ms_total;
+    ms_inflate += r.ms_copy_inflate; ms_chain += r.ms_chain; ms_extract += r.ms_extract;
+    max_slice = std::max(max_slice, (j.byte_hi - j.byte_lo) + (j.total - j.u_lo));
+    ++n_slices;
+    at = j.exit_off;
+    cap_end = nb;
+    halvings = 0;
   }
-  if (rc == CMB_E_DECLINED) return fail(c, CMB_E_DECLINED, "shard %u: the device decoder declined it (%s); sharded input is decoded on the device only", k, c->err.c_str());
-  if (rc) return rc;
-  if (!j.nothing_to_decode) {
-    CU_TRY(c, cudaEventSynchronize(c->dec.ev[4]));
-    cudaEventElapsedTime(&out->ms_total, c->dec.ev[0], c->dec.ev[4]);
-  }
-  c->dec.last_valid = false;  // the tuples are the shard's, not a sample's: cmb_last_bgzf_batch must not hand them out
+  if (getenv("CMB_PIPELINE_STATS"))
+    fprintf(stderr, "#shard_slices\tshard=%u\tslices=%u\tmax_slice_bytes=%llu\tcopy_inflate_ms=%.1f\tchain_ms=%.1f\textract_ms=%.1f\tgrow_ms=%.1f\n", k,
+            n_slices, (unsigned long long)max_slice, ms_inflate, ms_chain, ms_extract, ms_grow);
+  c->dec.last_valid = false;  // the tuples are a slice's, not a sample's: cmb_last_bgzf_batch must not hand them out
   return CMB_OK;
 }
 
@@ -2107,7 +2352,7 @@ uint64_t shard_bytes(const cmb_ctx* c) {
   const auto& s = c->sh;
   uint64_t b = s.d_scan.bytes() + s.d_hash0.bytes() + s.d_tid_count.bytes() + s.d_src.bytes() + s.d_slot_iv.bytes() + s.d_as_val.bytes() +
                s.d_as_state.bytes() + s.d_state.bytes() + s.d_out_slab.bytes() + s.d_excluded.bytes();
-  for (const auto& st : s.store) b += st.slab.bytes() + st.info.bytes();
+  for (const auto& st : s.store) b += st.bytes();
   return b;
 }
 
@@ -2152,46 +2397,20 @@ extern "C" int cmb_shard_add(cmb_ctx* c, const cmb_bgzf_input* in, cmb_bgzf_resu
   const uint32_t k = s.added;
   if (int rc = decode_shard(c, in, out, k)) return rc;
   s.ms_decode += out->ms_total;
-  auto& d = c->dec;
-  const uint64_t n_rec = d.last_n_rec * (uint64_t)(out->n_records != 0);
   auto& st = s.store[k];
   CU_TRY(c, cudaEventRecord(s.ev[0], c->stream));
-  // ---- which records are primaries, and where their tuples and intervals go
-  if (int rc = s.d_scan.ensure(c, n_rec + 1, with_slack(n_rec + 1))) return rc;
-  ShardScanArgs a{};
-  a.data = d.last_infl_base; a.rec_off = d.d_rec_off; a.n_records = n_rec; a.scan = s.d_scan;
-  a.shard = k; a.tid_offset = s.tid_offsets[k]; a.err = s.d_err;
-  unsigned long long packed = 0;
-  if (n_rec) {
-    carve_batch(d.d_tuple_slab, d.last_n_rec, d.last_n_cig, &a.tb);
-    ks_mark<<<(uint32_t)((n_rec + 255) / 256), 256, 0, c->stream>>>(a);
-    kf_scan<<<1, 1024, 0, c->stream>>>(s.d_scan, (uint32_t)n_rec);
-    CU_TRY(c, cudaGetLastError());
-    CU_TRY(c, cudaMemcpyAsync(&packed, s.d_scan + n_rec, 8, cudaMemcpyDeviceToHost, c->stream));
-    CU_TRY(c, cudaStreamSynchronize(c->stream));
-  }
-  st.n_prim = packed >> 32;
-  st.n_iv = (uint32_t)packed;
-  // ---- the shard's store
-  size_t offs[13];
-  const size_t slab = batch_slab_bytes((uint32_t)st.n_prim, (uint32_t)st.n_iv, offs);
-  if (int rc = st.slab.ensure(c, slab, slab + slab / 8)) return rc;
-  if (int rc = st.info.ensure(c, st.n_prim + 1, with_slack(st.n_prim + 1))) return rc;
-  carve_batch(st.slab, (uint32_t)st.n_prim, (uint32_t)st.n_iv, &st.view.b);
-  st.view.info = st.info;
+  // ---- the store's closing interval offset; shard 0 sizes every pair's running winner
+  const uint64_t n0 = s.store[0].n_prim;
+  if (int rc = shard_alloc(c, shard_need(c, k, st.n_prim, st.n_iv), [&] {
+        int e = store_grow(c, st, st.n_prim, st.n_iv);
+        if (!e && k == 0) e = s.d_state.ensure(c, n0 / 2 + 1, with_slack(n0 / 2 + 1));
+        return e;
+      }))
+    return rc;
   const uint32_t iv_total = (uint32_t)st.n_iv;
   CU_TRY(c, cudaMemcpyAsync(st.view.b.iv_begin + st.n_prim, &iv_total, 4, cudaMemcpyHostToDevice, c->stream));
-  if (int rc = s.d_as_val.ensure(c, st.n_prim + 1, with_slack(st.n_prim + 1))) return rc;
-  if (int rc = s.d_as_state.ensure(c, st.n_prim + 1, with_slack(st.n_prim + 1))) return rc;
-  const uint64_t n0 = s.store[0].n_prim;
-  if (k == 0) {
-    if (int rc = s.d_hash0.ensure(c, n0 + 1, with_slack(n0 + 1))) return rc;
-    if (int rc = s.d_state.ensure(c, n0 / 2 + 1, with_slack(n0 / 2 + 1))) return rc;
-    CU_TRY(c, cudaMemsetAsync(s.d_state, 0xff, sizeof(PairState) * (n0 / 2 + 1), c->stream));
-  }
-  a.st = st.view; a.as_val = s.d_as_val; a.as_state = s.d_as_state; a.hash0 = s.d_hash0; a.n0 = n0;
-  if (n_rec) ks_compact<<<(uint32_t)((n_rec + 255) / 256), 256, 0, c->stream>>>(a);
-  // ---- every pair's running winner
+  if (k == 0) CU_TRY(c, cudaMemsetAsync(s.d_state, 0xff, sizeof(PairState) * (n0 / 2 + 1), c->stream));
+  // ---- every pair's running winner, over the whole store: a pair whose primaries fell in different slices is whole here
   ShardPairArgs p{};
   p.st = st.view; p.as_val = s.d_as_val; p.as_state = s.d_as_state; p.excluded = s.have_excluded ? s.d_excluded.p : nullptr;
   p.state = s.d_state; p.n_pairs = std::min(st.n_prim, n0) / 2; p.shard = k; p.tid_offset = s.tid_offsets[k]; p.err = s.d_err;
@@ -2256,8 +2475,11 @@ extern "C" int cmb_shard_finish(cmb_ctx* c, cmb_shard_result* out) {
   // ---- the winners, sorted by tid, into one device batch
   const uint64_t n_out = h[1];
   if (n_out >= 0xffffff00ull) return fail(c, CMB_E_ARG, "cmb_shard_finish: more than 2^32 mapped winners");
-  if (int rc = s.d_src.ensure(c, n_out + 1, with_slack(n_out + 1))) return rc;
-  if (int rc = s.d_slot_iv.ensure(c, n_out + 1, with_slack(n_out + 1))) return rc;
+  if (int rc = shard_alloc(c, shard_need(c, s.n_shards, 0, 0, n_out), [&] {
+        int e = s.d_src.ensure(c, n_out + 1, with_slack(n_out + 1));
+        return e ? e : s.d_slot_iv.ensure(c, n_out + 1, with_slack(n_out + 1));
+      }))
+    return rc;
   a.src = s.d_src; a.slot_iv = s.d_slot_iv; a.n_out = n_out;
   if (n_pairs) ks_scatter<<<grid, 256, 0, c->stream>>>(a);
   kf_scan<<<1, 1024, 0, c->stream>>>(s.d_slot_iv, (uint32_t)n_out);
@@ -2266,7 +2488,8 @@ extern "C" int cmb_shard_finish(cmb_ctx* c, cmb_shard_result* out) {
   CU_TRY(c, cudaStreamSynchronize(c->stream));
   size_t offs[13];
   const size_t slab = batch_slab_bytes((uint32_t)n_out, (uint32_t)n_iv, offs);
-  if (int rc = s.d_out_slab.ensure(c, slab, slab + slab / 8)) return rc;
+  if (int rc = shard_alloc(c, shard_need(c, s.n_shards, 0, 0, n_out, n_iv), [&] { return s.d_out_slab.ensure(c, slab, slab + slab / 8); }))
+    return rc;
   carve_batch(s.d_out_slab, (uint32_t)n_out, (uint32_t)n_iv, &a.out);
   if (n_out) ks_gather<<<(uint32_t)((n_out + 255) / 256), 256, 0, c->stream>>>(a);
   CU_TRY(c, cudaGetLastError());

@@ -26,17 +26,21 @@ struct ShardStore {
   uint8_t* info;
 };
 
+// One block slice of a shard (cmb_shard_add): its records are scanned and their primaries appended to the shard's store at
+// prim_base / iv_base, so that every index below (the store's, hash0's, the error keys') counts from the shard's first record.
 struct ShardScanArgs {
   const uint8_t* data;          // biased base of the inflated stream
   const uint64_t* rec_off;
-  cmb_read_batch tb;            // the decoder's tuples of this shard
+  cmb_read_batch tb;            // the decoder's tuples of this slice
   uint64_t n_records;
   unsigned long long* scan;     // [n_records + 1]: packed (primaries << 32 | interval slots), exclusive after kf_scan
   ShardStore st;                // this shard's store (ks_compact)
+  uint64_t prim_base;           // primaries of the shard's earlier slices
+  uint32_t iv_base;             // their interval slots
   int32_t* as_val;              // [primaries] this shard's AS values (ks_pairs reads them)
   uint8_t* as_state;
   unsigned long long* hash0;    // shard 0's name hashes; written by shard 0, compared by the others
-  uint64_t n0;                  // primaries of shard 0
+  uint64_t n0;                  // primaries of shard 0 (complete before shard 1's first slice)
   uint32_t shard;
   int32_t tid_offset;
   unsigned long long* err;
@@ -62,8 +66,8 @@ __global__ void __launch_bounds__(256) ks_compact(const ShardScanArgs a) {
   const uint64_t i = (uint64_t)blockIdx.x * 256 + threadIdx.x;
   if (i >= a.n_records) return;
   const unsigned long long s = a.scan[i];
-  const uint64_t j = s >> 32;
-  const uint32_t ivo = (uint32_t)s;
+  const uint64_t j = a.prim_base + (s >> 32);
+  const uint32_t ivo = a.iv_base + (uint32_t)s;
   const uint32_t flag = a.tb.flag[i];
   // "This code can only handle paired-end input" (shard_bam_reader.rs:79-87): met while reading set j of this shard
   if (!(flag & 0x1)) atomicMin(a.err, sh_key(j, a.shard, SHE_UNPAIRED, 0));

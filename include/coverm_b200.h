@@ -311,10 +311,12 @@ int cmb_decode_bgzf(cmb_ctx* ctx, const cmb_bgzf_input* in, cmb_bgzf_result* out
  *   cmb_shard_begin: tid_offsets[k] = targets in shards 0..k-1; excluded = n_contigs bytes, or NULL: 1 = a contig of an excluded
  *                    genome, 2 = a contig whose genome cannot be told (its name lacks the separator: the reference panics when a
  *                    candidate's first mate lies there).
- *   cmb_shard_add:   once per shard, in order: the shard is inflated and decoded on the device (cmb_decode_bgzf's stages), its
- *                    primaries are kept in a per-shard store (about 41 B per primary + 8 B per CIGAR operation) and the running
- *                    winner of every pair is updated.  A shard the device decoder declines is CMB_E_DECLINED: there is no host
- *                    route for shards.
+ *   cmb_shard_add:   once per shard, in order, with the whole shard file and block table: the shard is inflated and decoded
+ *                    on the device (cmb_decode_bgzf's stages) in consecutive block slices sized to the free device memory, each
+ *                    slice's primaries appended to a per-shard store (about 41 B per primary + 8 B per CIGAR operation), then
+ *                    the running winner of every pair is updated.  `out` sums the slices.  A shard the device decoder declines is
+ *                    CMB_E_DECLINED: there is no host route for shards.  CMB_E_NOMEM: the stores, pair state, name hashes, AS
+ *                    scratch and sorted winners alone do not fit (the message names the bytes needed and free).
  *   cmb_shard_finish: checks the shards' lengths, sorts and submits the winners, frees nothing (the stores are grow-only).
  * Errors carry the reference's message: CMB_E_SHARD_EXIT where it exits with status 1, CMB_E_SHARD_PANIC where it panics, and
  * CMB_E_NM for an NM tag the reference's clone rejects.  With several errors the one the reference meets first is reported. */
