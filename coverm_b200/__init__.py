@@ -107,7 +107,8 @@ DEVICE_SYMBOLS = ["cmb_abi_version", "cmb_create", "cmb_destroy", "cmb_last_erro
                   "cmb_set_genes_range", "cmb_fetch_gene_extras", "cmb_grow_buffers", "cmb_last_bgzf_batch", "cmb_end_sample", "cmb_comm_unique_id",
                   "cmb_comm_init", "cmb_comm_init_local", "cmb_comm_destroy", "cmb_comm_allgather", "cmb_allgather_stats", "cmb_kept_tid_range", "cmb_fetch_pairs", "cmb_end_sample_device",
                   "cmb_get_timing", "cmb_stream", "cmb_host_alloc", "cmb_host_free", "cmb_nvtx_push", "cmb_nvtx_pop",
-                  "cmb_shard_begin", "cmb_shard_add", "cmb_shard_finish"]
+                  "cmb_shard_begin", "cmb_shard_add", "cmb_shard_finish", "cmb_shard_begin_range", "cmb_shard_score",
+                  "cmb_shard_exchange", "cmb_shard_export", "cmb_shard_import", "cmb_shard_choose", "cmb_shard_finish_group"]
 class Tuples(C.Structure):
     _fields_ = [("n_contigs", C.c_uint32), ("contig_len", C.POINTER(C.c_uint64)), ("n_records", C.c_uint64),
                 ("n_intervals", C.c_uint64), ("tid", C.POINTER(C.c_int32)), ("pos", C.POINTER(C.c_int32)),

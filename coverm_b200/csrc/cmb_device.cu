@@ -288,17 +288,29 @@ struct cmb_ctx {
       Buf<uint32_t> nm, l_seq, aligned, del, ins, iv_begin;
       Buf<uint16_t> flag;
       Buf<uint8_t> mapq, nm_state, info;
+      Buf<unsigned long long> names;  // group runs, shards k > 0: name hashes for ks_names
+      Buf<int32_t> as_val;            // group runs: the shard's AS values and states, kept until cmb_shard_score
+      Buf<uint8_t> as_state;
       ShardStore view{};
       uint64_t n_prim = 0, n_iv = 0;
       uint64_t bytes() const {
         return tid.bytes() + pos.bytes() + iv_start.bytes() + iv_len.bytes() + nm.bytes() + l_seq.bytes() + aligned.bytes() + del.bytes() +
-               ins.bytes() + iv_begin.bytes() + flag.bytes() + mapq.bytes() + nm_state.bytes() + info.bytes();
+               ins.bytes() + iv_begin.bytes() + flag.bytes() + mapq.bytes() + nm_state.bytes() + info.bytes() + names.bytes() +
+               as_val.bytes() + as_state.bytes();
       }
     };
     std::vector<Store> store;
     std::vector<int32_t> tid_offsets;
     uint32_t n_shards = 0, added = 0;
     bool active = false;
+    // group runs (cmb_shard_begin_range): this context decodes shards [first, last); the others' scores arrive in d_score
+    uint32_t first = 0, last = 0;
+    bool group = false;
+    Buf<int32_t> d_score;            // [n_shards][n_pairs] score table (ks_score, exchanged, ks_choose)
+    std::vector<uint64_t> n_prim;    // every shard's primaries (cmb_shard_score)
+    uint64_t n_pairs = 0, n_out = 0;
+    unsigned long long len_key = ~0ull;  // the reader's length checks, keyed like the kernels' errors
+    int stage = 0;                   // 1 scored, 2 chosen
     Buf<uint8_t> d_excluded;
     bool have_excluded = false;
     Buf<unsigned long long> d_scan, d_hash0, d_err, d_tid_count, d_src, d_slot_iv;
@@ -2133,12 +2145,15 @@ void release_decode(cmb_ctx* c) {
 // and the pair state (8 + 8 B per primary), and the n_out sorted winners with their n_out_iv slots (52 B and 8 B)
 uint64_t shard_need(const cmb_ctx* c, uint32_t k, uint64_t n_prim, uint64_t n_iv, uint64_t n_out = 0, uint64_t n_out_iv = 0) {
   const auto& s = c->sh;
-  uint64_t b = 37 * n_prim + 8 * n_iv, as = n_prim;
-  for (uint32_t i = 0; i < k; ++i) {
-    b += 37 * s.store[i].n_prim + 8 * s.store[i].n_iv;
-    as = std::max(as, s.store[i].n_prim);
+  // a group rank holds the stores of its own shards [first, k] only, each with its AS columns (5 B per primary) and, after
+  // shard 0, its name hashes (8 B)
+  auto per_prim = [&](uint32_t i) -> uint64_t { return s.group ? (i ? 50 : 42) : 37; };
+  uint64_t b = per_prim(k) * n_prim + 8 * n_iv, as = s.group ? 0 : n_prim;
+  for (uint32_t i = s.first; i < k; ++i) {
+    b += per_prim(i) * s.store[i].n_prim + 8 * s.store[i].n_iv;
+    if (!s.group) as = std::max(as, s.store[i].n_prim);
   }
-  return b + 5 * as + 16 * (k ? s.store[0].n_prim : n_prim) + 52 * n_out + 8 * n_out_iv;
+  return b + 5 * as + 16 * (k > s.first ? s.store[s.first].n_prim : n_prim) + 52 * n_out + 8 * n_out_iv;
 }
 
 // Bytes the device has for them and a slice: the limit under CMB_DECODE_MEM_LIMIT_MB, else what is free plus the stores and
@@ -2216,7 +2231,9 @@ int decode_shard(cmb_ctx* c, const cmb_bgzf_input* in, cmb_bgzf_result* out, uin
   for (uint32_t b = 0; b < nb; ++b) ustart[b + 1] = ustart[b] + in->block_isize[b];
   const ShardBlocks blocks{nb, in->size, in->block_coffset, in->block_clen, ustart.data()};
   const uint64_t lim = shard_mem_limit();
-  const uint64_t n0 = k ? s.store[0].n_prim : 0, iv0 = k ? s.store[0].n_iv : 0;
+  // shards after this context's first are expected to be sized like it (on one GPU: like shard 0)
+  const bool later = k > s.first;
+  const uint64_t n0 = later ? s.store[s.first].n_prim : 0, iv0 = later ? s.store[s.first].n_iv : 0;
   uint64_t at = in->records_at, tail = SLICE_TAIL_BYTES, max_slice = 0;
   uint32_t n_slices = 0;
   float ms_inflate = 0, ms_chain = 0, ms_extract = 0, ms_grow = 0;
@@ -2230,13 +2247,13 @@ int decode_shard(cmb_ctx* c, const cmb_bgzf_input* in, cmb_bgzf_result* out, uin
     // winners (at most one record per primary of a shard, 60 B each with an interval slot).  Shard 0's first slice has no
     // estimate: like a whole-shard decode it takes what is free, and a failed allocation halves it.
     uint64_t expect = 0;
-    if (k) {
-      expect = 37 * (n0 > st.n_prim ? n0 - st.n_prim : 0) + 8 * (iv0 > st.n_iv ? iv0 - st.n_iv : 0) + (s.n_shards - 1 - k) * (37 * n0 + 8 * iv0) +
+    if (later) {
+      expect = 37 * (n0 > st.n_prim ? n0 - st.n_prim : 0) + 8 * (iv0 > st.n_iv ? iv0 - st.n_iv : 0) + (s.last - 1 - k) * (37 * n0 + 8 * iv0) +
                60 * n0;
-    } else if (at > in->records_at) {  // shard 0: scaled by the inflated bytes its slices so far held
+    } else if (at > in->records_at) {  // the first shard: scaled by the inflated bytes its slices so far held
       const double scale = (double)(ustart[nb] - in->records_at) / (double)(at - in->records_at);
       const double total = need_now * scale, store = (37.0 * st.n_prim + 8.0 * st.n_iv) * scale, winners = 60.0 * st.n_prim * scale;
-      expect = (uint64_t)(total - need_now + store * (s.n_shards - 1) + winners);
+      expect = (uint64_t)(total - need_now + store * (s.last - 1 - k) + winners);
     }
     const uint64_t room = shard_room(c), held = need_now + expect;
     uint64_t budget = room > held ? room - held : 0;
@@ -2304,14 +2321,17 @@ int decode_shard(cmb_ctx* c, const cmb_bgzf_input* in, cmb_bgzf_result* out, uin
     // decoded again
     // The expected totals: shard 0's, for shard k > 0; for shard 0, its slices so far scaled by the inflated bytes they cover
     const double scale = (double)(ustart[nb] - in->records_at) / (double)(j.exit_off - in->records_at);
-    const uint64_t hint_prim = k ? n0 : (uint64_t)(n_prim * scale), hint_iv = k ? iv0 : (uint64_t)(n_iv * scale);
+    const uint64_t hint_prim = later ? n0 : (uint64_t)(n_prim * scale), hint_iv = later ? iv0 : (uint64_t)(n_iv * scale);
     bool released = false;
     const auto g0 = std::chrono::steady_clock::now();
     auto grow = [&]() -> int {
       int e;
-      if ((e = store_grow(c, st, n_prim, n_iv, hint_prim, hint_iv)) || (e = grow_col(c, s.d_as_val, st.n_prim, n_prim + 1, hint_prim + 1)) ||
-          (e = grow_col(c, s.d_as_state, st.n_prim, n_prim + 1, hint_prim + 1)) ||
-          (k == 0 && (e = grow_col(c, s.d_hash0, st.n_prim, n_prim + 1, hint_prim + 1))))
+      auto& as_val = s.group ? st.as_val : s.d_as_val;
+      auto& as_state = s.group ? st.as_state : s.d_as_state;
+      if ((e = store_grow(c, st, n_prim, n_iv, hint_prim, hint_iv)) || (e = grow_col(c, as_val, st.n_prim, n_prim + 1, hint_prim + 1)) ||
+          (e = grow_col(c, as_state, st.n_prim, n_prim + 1, hint_prim + 1)) ||
+          (k == 0 && (e = grow_col(c, s.d_hash0, st.n_prim, n_prim + 1, hint_prim + 1))) ||
+          (k && s.group && (e = grow_col(c, st.names, st.n_prim, n_prim + 1, hint_prim + 1))))
         released = released || e == CMB_E_NOMEM;
       return e;
     };
@@ -2319,7 +2339,8 @@ int decode_shard(cmb_ctx* c, const cmb_bgzf_input* in, cmb_bgzf_result* out, uin
     ms_grow += std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - g0).count();
     if (released) continue;
     a.st = st.view; a.prim_base = st.n_prim; a.iv_base = (uint32_t)st.n_iv;
-    a.as_val = s.d_as_val; a.as_state = s.d_as_state; a.hash0 = s.d_hash0; a.n0 = n0;
+    a.as_val = s.group ? st.as_val.p : s.d_as_val.p; a.as_state = s.group ? st.as_state.p : s.d_as_state.p; a.hash0 = s.d_hash0; a.n0 = k ? s.store[0].n_prim : 0;
+    if (k && s.group) a.names = st.names;
     ks_compact<<<(uint32_t)((n_rec + 255) / 256), 256, 0, c->stream>>>(a);
     CU_TRY(c, cudaGetLastError());
     CU_TRY(c, cudaEventRecord(s.ev[1], c->stream));
@@ -2358,21 +2379,28 @@ uint64_t shard_bytes(const cmb_ctx* c) {
 
 }  // namespace
 
-extern "C" int cmb_shard_begin(cmb_ctx* c, uint32_t n_shards, const uint32_t* tid_offsets, const uint8_t* excluded) {
-  NvtxRange nvtx_fn("cmb_shard_begin");
-  if (!c || !tid_offsets || n_shards == 0) return fail(c, CMB_E_ARG, "cmb_shard_begin: null argument or no shards");
-  if (!c->in_sample) return fail(c, CMB_E_ARG, "cmb_shard_begin: no sample in progress");
-  if (c->mode.filter_pairs || c->params.filtering) return fail(c, CMB_E_ARG, "cmb_shard_begin: sharded input takes no read filter");
-  if (n_shards > 255) return fail(c, CMB_E_ARG, "cmb_shard_begin: at most 255 shards");
+namespace {
+int begin_shards(cmb_ctx* c, const char* fn, uint32_t n_shards, const uint32_t* tid_offsets, const uint8_t* excluded, uint32_t first, uint32_t last,
+                bool group) {
+  if (!c || !tid_offsets || n_shards == 0) return fail(c, CMB_E_ARG, "%s: null argument or no shards", fn);
+  if (!c->in_sample) return fail(c, CMB_E_ARG, "%s: no sample in progress", fn);
+  if (c->mode.filter_pairs || c->params.filtering) return fail(c, CMB_E_ARG, "%s: sharded input takes no read filter", fn);
+  if (n_shards > 255) return fail(c, CMB_E_ARG, "%s: at most 255 shards", fn);
+  if (first > last || last > n_shards) return fail(c, CMB_E_ARG, "%s: shard range [%u, %u) outside the %u shards", fn, first, last, n_shards);
   const uint32_t n_ref = c->gene_mode ? c->n_ref_contigs : c->n_contigs;
   for (uint32_t k = 0; k < n_shards; ++k)
-    if (tid_offsets[k] > n_ref || (k && tid_offsets[k] < tid_offsets[k - 1])) return fail(c, CMB_E_ARG, "cmb_shard_begin: tid offsets outside the reference");
+    if (tid_offsets[k] > n_ref || (k && tid_offsets[k] < tid_offsets[k - 1])) return fail(c, CMB_E_ARG, "%s: tid offsets outside the reference", fn);
   CU_TRY(c, cudaSetDevice(c->device));
   auto& s = c->sh;
   s.n_shards = n_shards;
-  s.added = 0;
+  s.first = first;
+  s.last = last;
+  s.group = group;
+  s.added = first;
+  s.stage = 0;
   s.tid_offsets.assign(tid_offsets, tid_offsets + n_shards);
   if (s.store.size() < n_shards) s.store.resize(n_shards);
+  for (auto& st : s.store) st.n_prim = st.n_iv = 0;
   s.have_excluded = excluded != nullptr;
   if (excluded) {
     if (int rc = s.d_excluded.ensure(c, std::max<uint32_t>(1, n_ref))) return rc;
@@ -2386,13 +2414,25 @@ extern "C" int cmb_shard_begin(cmb_ctx* c, uint32_t n_shards, const uint32_t* ti
   s.active = true;
   return CMB_OK;
 }
+}  // namespace
+
+extern "C" int cmb_shard_begin(cmb_ctx* c, uint32_t n_shards, const uint32_t* tid_offsets, const uint8_t* excluded) {
+  NvtxRange nvtx_fn("cmb_shard_begin");
+  return begin_shards(c, "cmb_shard_begin", n_shards, tid_offsets, excluded, 0, n_shards, false);
+}
+
+extern "C" int cmb_shard_begin_range(cmb_ctx* c, uint32_t n_shards, const uint32_t* tid_offsets, const uint8_t* excluded, uint32_t shard_begin,
+                                     uint32_t shard_end) {
+  NvtxRange nvtx_fn("cmb_shard_begin_range");
+  return begin_shards(c, "cmb_shard_begin_range", n_shards, tid_offsets, excluded, shard_begin, shard_end, true);
+}
 
 extern "C" int cmb_shard_add(cmb_ctx* c, const cmb_bgzf_input* in, cmb_bgzf_result* out) {
   NvtxRange nvtx_fn("cmb_shard_add");
   if (!c || !in || !out || !in->data || !in->block_coffset || !in->block_clen || !in->block_isize)
     return fail(c, CMB_E_ARG, "cmb_shard_add: null argument");
   auto& s = c->sh;
-  if (!c->in_sample || !s.active || s.added >= s.n_shards) return fail(c, CMB_E_ARG, "cmb_shard_add: call cmb_shard_begin first, once per shard");
+  if (!c->in_sample || !s.active || s.added >= s.last) return fail(c, CMB_E_ARG, "cmb_shard_add: call cmb_shard_begin first, once per shard");
   CU_TRY(c, cudaSetDevice(c->device));
   const uint32_t k = s.added;
   if (int rc = decode_shard(c, in, out, k)) return rc;
@@ -2403,12 +2443,17 @@ extern "C" int cmb_shard_add(cmb_ctx* c, const cmb_bgzf_input* in, cmb_bgzf_resu
   const uint64_t n0 = s.store[0].n_prim;
   if (int rc = shard_alloc(c, shard_need(c, k, st.n_prim, st.n_iv), [&] {
         int e = store_grow(c, st, st.n_prim, st.n_iv);
-        if (!e && k == 0) e = s.d_state.ensure(c, n0 / 2 + 1, with_slack(n0 / 2 + 1));
+        if (!e && k == 0 && !s.group) e = s.d_state.ensure(c, n0 / 2 + 1, with_slack(n0 / 2 + 1));
         return e;
       }))
     return rc;
   const uint32_t iv_total = (uint32_t)st.n_iv;
   CU_TRY(c, cudaMemcpyAsync(st.view.b.iv_begin + st.n_prim, &iv_total, 4, cudaMemcpyHostToDevice, c->stream));
+  if (s.group) {  // a group run scores every pair once all shards' lengths are known (cmb_shard_score)
+    CU_TRY(c, cudaStreamSynchronize(c->stream));
+    s.added += 1;
+    return CMB_OK;
+  }
   if (k == 0) CU_TRY(c, cudaMemsetAsync(s.d_state, 0xff, sizeof(PairState) * (n0 / 2 + 1), c->stream));
   // ---- every pair's running winner, over the whole store: a pair whose primaries fell in different slices is whole here
   ShardPairArgs p{};
@@ -2425,70 +2470,79 @@ extern "C" int cmb_shard_add(cmb_ctx* c, const cmb_bgzf_input* in, cmb_bgzf_resu
   return CMB_OK;
 }
 
-extern "C" int cmb_shard_finish(cmb_ctx* c, cmb_shard_result* out) {
-  NvtxRange nvtx_fn("cmb_shard_finish");
-  if (!c || !out) return fail(c, CMB_E_ARG, "cmb_shard_finish: null argument");
-  auto& s = c->sh;
-  if (!c->in_sample || !s.active || s.added != s.n_shards) return fail(c, CMB_E_ARG, "cmb_shard_finish: every shard must be added first");
-  s.active = false;
-  CU_TRY(c, cudaSetDevice(c->device));
-  *out = cmb_shard_result{};
-  // the reader's own checks (shard_bam_reader.rs:117-121, 187-190) are keyed like the kernels' errors
-  const uint64_t n0 = s.store[0].n_prim;
+namespace {
+// The reader's own checks (shard_bam_reader.rs:117-121, 187-190), keyed like the kernels' errors: after every kernel-found error
+// of the same set
+unsigned long long shard_length_key(const std::vector<uint64_t>& n_prim) {
+  const uint64_t n0 = n_prim[0];
   uint64_t n_min = n0;
   bool equal = true;
-  for (uint32_t k = 0; k < s.n_shards; ++k) {
-    n_min = std::min(n_min, s.store[k].n_prim);
-    equal = equal && s.store[k].n_prim == n0;
+  for (uint64_t n : n_prim) {
+    n_min = std::min(n_min, n);
+    equal = equal && n == n0;
   }
-  const uint64_t n_pairs = n_min / 2;
+  const unsigned long long phase_end = 0xfff;
+  if (!equal) return (n_min << 24) | (phase_end << 12) | (3ull << 8);
+  if (n0 % 2) return (n0 << 24) | (phase_end << 12) | (4ull << 8);
+  return ~0ull;
+}
+
+// The error of the smallest key, or CMB_OK
+int shard_key_error(cmb_ctx* c, unsigned long long key) {
+  if (key != ~0ull && ((key >> 8) & 0xf) == 3)
+    return fail(c, CMB_E_SHARD_EXIT, "Unexpectedly one BAM file input finished while another had further reads");
+  if (key != ~0ull && ((key >> 8) & 0xf) == 4)
+    return fail(c, CMB_E_SHARD_PANIC, "Unexpectedly was able to read a first read set, but not a second. Hmm.");
+  return shard_error(c, key);
+}
+
+// The store views and tid offsets on the device, the winners counted per tid (ks_count after s.d_state holds the choice); the
+// error key and the mapped winners' count come back to the host
+int shard_count(cmb_ctx* c, ShardSortArgs& a, unsigned long long* key) {
+  auto& s = c->sh;
   const uint32_t n_ref = c->gene_mode ? c->n_ref_contigs : c->n_contigs;
-  CU_TRY(c, cudaEventRecord(s.ev[2], c->stream));
   if (int rc = s.d_tid_count.ensure(c, (size_t)n_ref + 1, (size_t)n_ref + 1)) return rc;
   if (int rc = s.d_stores.ensure(c, s.n_shards)) return rc;
   if (int rc = s.d_tid_offsets.ensure(c, s.n_shards)) return rc;
   std::vector<ShardStore> views(s.n_shards);
-  for (uint32_t k = 0; k < s.n_shards; ++k) views[k] = s.store[k].view;
+  for (uint32_t k = s.first; k < s.last; ++k) views[k] = s.store[k].view;
   CU_TRY(c, cudaMemcpyAsync(s.d_stores, views.data(), sizeof(ShardStore) * s.n_shards, cudaMemcpyHostToDevice, c->stream));
   CU_TRY(c, cudaMemcpyAsync(s.d_tid_offsets, s.tid_offsets.data(), 4ull * s.n_shards, cudaMemcpyHostToDevice, c->stream));
   CU_TRY(c, cudaMemsetAsync(s.d_tid_count, 0, 8ull * ((size_t)n_ref + 1), c->stream));
-  ShardSortArgs a{};
-  a.stores = s.d_stores; a.tid_offsets = s.d_tid_offsets; a.state = s.d_state; a.n_pairs = n_pairs; a.n_contigs = n_ref;
-  a.tid_count = s.d_tid_count; a.err = s.d_err;
-  const uint32_t grid = (uint32_t)((n_pairs + 255) / 256);
-  if (n_pairs) ks_count<<<grid, 256, 0, c->stream>>>(a);
+  a = ShardSortArgs{};
+  a.stores = s.d_stores; a.tid_offsets = s.d_tid_offsets; a.state = s.d_state; a.n_pairs = s.n_pairs; a.n_contigs = n_ref;
+  a.tid_count = s.d_tid_count; a.err = s.d_err; a.own_begin = s.first; a.own_end = s.last;
+  if (s.n_pairs) ks_count<<<(uint32_t)((s.n_pairs + 255) / 256), 256, 0, c->stream>>>(a);
   kf_scan<<<1, 1024, 0, c->stream>>>(s.d_tid_count, n_ref);
   CU_TRY(c, cudaGetLastError());
   unsigned long long h[2] = {~0ull, 0};
   CU_TRY(c, cudaMemcpyAsync(&h[0], s.d_err, 8, cudaMemcpyDeviceToHost, c->stream));
   CU_TRY(c, cudaMemcpyAsync(&h[1], s.d_tid_count + n_ref, 8, cudaMemcpyDeviceToHost, c->stream));
   CU_TRY(c, cudaStreamSynchronize(c->stream));
-  unsigned long long key = h[0];
-  const unsigned long long phase_end = 0xfff;  // the reader's checks come after every kernel-found error of the same set
-  if (!equal) key = std::min(key, (n_min << 24) | (phase_end << 12) | (3ull << 8));
-  else if (n0 % 2) key = std::min(key, (n0 << 24) | (phase_end << 12) | (4ull << 8));
-  if (key != ~0ull && ((key >> 8) & 0xf) == 3)
-    return fail(c, CMB_E_SHARD_EXIT, "Unexpectedly one BAM file input finished while another had further reads");
-  if (key != ~0ull && ((key >> 8) & 0xf) == 4)
-    return fail(c, CMB_E_SHARD_PANIC, "Unexpectedly was able to read a first read set, but not a second. Hmm.");
-  if (int rc = shard_error(c, key)) return rc;
-  // ---- the winners, sorted by tid, into one device batch
-  const uint64_t n_out = h[1];
+  *key = std::min(h[0], s.len_key);
+  s.n_out = h[1];
+  return CMB_OK;
+}
+
+// The counted winners, sorted by tid, into one device batch that is submitted; `out` reports the sample
+int shard_sort_submit(cmb_ctx* c, ShardSortArgs& a, cmb_shard_result* out) {
+  auto& s = c->sh;
+  const uint64_t n_out = s.n_out, n_pairs = s.n_pairs;
   if (n_out >= 0xffffff00ull) return fail(c, CMB_E_ARG, "cmb_shard_finish: more than 2^32 mapped winners");
-  if (int rc = shard_alloc(c, shard_need(c, s.n_shards, 0, 0, n_out), [&] {
+  if (int rc = shard_alloc(c, shard_need(c, s.last, 0, 0, n_out), [&] {
         int e = s.d_src.ensure(c, n_out + 1, with_slack(n_out + 1));
         return e ? e : s.d_slot_iv.ensure(c, n_out + 1, with_slack(n_out + 1));
       }))
     return rc;
   a.src = s.d_src; a.slot_iv = s.d_slot_iv; a.n_out = n_out;
-  if (n_pairs) ks_scatter<<<grid, 256, 0, c->stream>>>(a);
+  if (n_pairs) ks_scatter<<<(uint32_t)((n_pairs + 255) / 256), 256, 0, c->stream>>>(a);
   kf_scan<<<1, 1024, 0, c->stream>>>(s.d_slot_iv, (uint32_t)n_out);
   unsigned long long n_iv = 0;
   CU_TRY(c, cudaMemcpyAsync(&n_iv, s.d_slot_iv + n_out, 8, cudaMemcpyDeviceToHost, c->stream));
   CU_TRY(c, cudaStreamSynchronize(c->stream));
   size_t offs[13];
   const size_t slab = batch_slab_bytes((uint32_t)n_out, (uint32_t)n_iv, offs);
-  if (int rc = shard_alloc(c, shard_need(c, s.n_shards, 0, 0, n_out, n_iv), [&] { return s.d_out_slab.ensure(c, slab, slab + slab / 8); }))
+  if (int rc = shard_alloc(c, shard_need(c, s.last, 0, 0, n_out, n_iv), [&] { return s.d_out_slab.ensure(c, slab, slab + slab / 8); }))
     return rc;
   carve_batch(s.d_out_slab, (uint32_t)n_out, (uint32_t)n_iv, &a.out);
   if (n_out) ks_gather<<<(uint32_t)((n_out + 255) / 256), 256, 0, c->stream>>>(a);
@@ -2505,4 +2559,166 @@ extern "C" int cmb_shard_finish(cmb_ctx* c, cmb_shard_result* out) {
   cudaEventElapsedTime(&out->ms_sort, s.ev[2], s.ev[3]);
   if (!n_out) return CMB_OK;
   return cmb_submit_device_batch(c, &a.out, (uint32_t)n_out, (uint32_t)n_iv);
+}
+}  // namespace
+
+extern "C" int cmb_shard_finish(cmb_ctx* c, cmb_shard_result* out) {
+  NvtxRange nvtx_fn("cmb_shard_finish");
+  if (!c || !out) return fail(c, CMB_E_ARG, "cmb_shard_finish: null argument");
+  auto& s = c->sh;
+  if (!c->in_sample || !s.active || s.group || s.added != s.n_shards) return fail(c, CMB_E_ARG, "cmb_shard_finish: every shard must be added first");
+  s.active = false;
+  CU_TRY(c, cudaSetDevice(c->device));
+  *out = cmb_shard_result{};
+  s.n_prim.resize(s.n_shards);
+  for (uint32_t k = 0; k < s.n_shards; ++k) s.n_prim[k] = s.store[k].n_prim;
+  s.n_pairs = *std::min_element(s.n_prim.begin(), s.n_prim.end()) / 2;
+  s.len_key = shard_length_key(s.n_prim);
+  CU_TRY(c, cudaEventRecord(s.ev[2], c->stream));
+  ShardSortArgs a{};
+  unsigned long long key;
+  if (int rc = shard_count(c, a, &key)) return rc;
+  if (int rc = shard_key_error(c, key)) return rc;
+  // ---- the winners, sorted by tid, into one device batch
+  return shard_sort_submit(c, a, out);
+}
+
+// ---- group runs -------------------------------------------------------------------------------------------------------------
+extern "C" int cmb_shard_score(cmb_ctx* c, const uint64_t* n_primary) {
+  NvtxRange nvtx_fn("cmb_shard_score");
+  if (!c || !n_primary) return fail(c, CMB_E_ARG, "cmb_shard_score: null argument");
+  auto& s = c->sh;
+  if (!c->in_sample || !s.active || !s.group || s.added != s.last || s.stage != 0)
+    return fail(c, CMB_E_ARG, "cmb_shard_score: call cmb_shard_begin_range and add this context's shards first");
+  for (uint32_t k = s.first; k < s.last; ++k)
+    if (n_primary[k] != s.store[k].n_prim)
+      return fail(c, CMB_E_ARG, "cmb_shard_score: shard %u holds %llu primaries, not %llu", k, (unsigned long long)s.store[k].n_prim,
+                  (unsigned long long)n_primary[k]);
+  CU_TRY(c, cudaSetDevice(c->device));
+  s.n_prim.assign(n_primary, n_primary + s.n_shards);
+  const uint64_t n0 = s.n_prim[0];
+  s.n_pairs = *std::min_element(s.n_prim.begin(), s.n_prim.end()) / 2;
+  s.len_key = shard_length_key(s.n_prim);
+  const uint64_t cells = (uint64_t)s.n_shards * s.n_pairs;
+  // the score table, shard 0's name hashes where shard 0 is decoded elsewhere, and the choice
+  if (int rc = shard_alloc(c, shard_need(c, s.last, 0, 0) + 4 * cells + 8 * n0, [&] {
+        int e = s.d_score.ensure(c, std::max<uint64_t>(1, cells), with_slack(std::max<uint64_t>(1, cells)));
+        if (!e && !(s.first == 0 && s.last > 0)) e = s.d_hash0.ensure(c, n0 + 1, with_slack(n0 + 1));
+        if (!e) e = s.d_state.ensure(c, s.n_pairs + 1, with_slack(s.n_pairs + 1));
+        return e;
+      }))
+    return rc;
+  CU_TRY(c, cudaEventRecord(s.ev[0], c->stream));
+  for (uint32_t k = s.first; k < s.last; ++k) {
+    const auto& st = s.store[k];
+    ShardPairArgs p{};
+    p.st = st.view; p.as_val = st.as_val; p.as_state = st.as_state; p.excluded = s.have_excluded ? s.d_excluded.p : nullptr;
+    p.n_pairs = std::min(st.n_prim, n0) / 2; p.shard = k; p.tid_offset = s.tid_offsets[k]; p.err = s.d_err;
+    p.score = s.d_score.p + (uint64_t)k * s.n_pairs; p.n_score = s.n_pairs;
+    if (p.n_pairs) ks_score<<<(uint32_t)((p.n_pairs + 255) / 256), 256, 0, c->stream>>>(p);
+  }
+  CU_TRY(c, cudaGetLastError());
+  CU_TRY(c, cudaEventRecord(s.ev[1], c->stream));
+  CU_TRY(c, cudaEventSynchronize(s.ev[1]));
+  float ms = 0;
+  cudaEventElapsedTime(&ms, s.ev[0], s.ev[1]);
+  s.ms_choose += ms;
+  s.stage = 1;
+  return CMB_OK;
+}
+
+namespace {
+int shard_io(cmb_ctx* c, const char* fn, uint32_t shard, void* scores, void* names, cudaMemcpyKind dir) {
+  if (!c || !scores) return fail(c, CMB_E_ARG, "%s: null argument", fn);
+  auto& s = c->sh;
+  if (!s.active || !s.group || s.stage != 1 || shard >= s.n_shards) return fail(c, CMB_E_ARG, "%s: no scored shard %u (cmb_shard_score first)", fn, shard);
+  CU_TRY(c, cudaSetDevice(c->device));
+  const bool h2d = dir == cudaMemcpyHostToDevice;
+  int32_t* col = s.d_score.p + (uint64_t)shard * s.n_pairs;
+  if (s.n_pairs) CU_TRY(c, cudaMemcpyAsync(h2d ? (void*)col : scores, h2d ? scores : (const void*)col, 4 * s.n_pairs, dir, c->stream));
+  if (shard == 0 && names && s.n_prim[0])
+    CU_TRY(c, cudaMemcpyAsync(h2d ? (void*)s.d_hash0.p : names, h2d ? names : (const void*)s.d_hash0.p, 8 * s.n_prim[0], dir, c->stream));
+  CU_TRY(c, cudaStreamSynchronize(c->stream));
+  return CMB_OK;
+}
+}  // namespace
+
+extern "C" int cmb_shard_export(cmb_ctx* c, uint32_t shard, int32_t* scores, uint64_t* names) {
+  return shard_io(c, "cmb_shard_export", shard, scores, names, cudaMemcpyDeviceToHost);
+}
+
+extern "C" int cmb_shard_import(cmb_ctx* c, uint32_t shard, const int32_t* scores, const uint64_t* names) {
+  return shard_io(c, "cmb_shard_import", shard, const_cast<int32_t*>(scores), const_cast<uint64_t*>(names), cudaMemcpyHostToDevice);
+}
+
+extern "C" int cmb_shard_exchange(cmb_ctx* c, const uint32_t* shard_cuts) {
+  NvtxRange nvtx_fn("cmb_shard_exchange: NCCL broadcasts");
+  if (!c || !shard_cuts) return fail(c, CMB_E_ARG, "cmb_shard_exchange: null argument");
+  if (!c->comm) return fail(c, CMB_E_ARG, "cmb_shard_exchange: no communicator (cmb_comm_init first)");
+  auto& s = c->sh;
+  if (!s.active || !s.group || s.stage != 1) return fail(c, CMB_E_ARG, "cmb_shard_exchange: call cmb_shard_score first");
+  const int N = c->comm_size, me = c->comm_rank;
+  if (shard_cuts[0] != 0 || shard_cuts[N] != s.n_shards || shard_cuts[me] != s.first || shard_cuts[me + 1] != s.last)
+    return fail(c, CMB_E_ARG, "cmb_shard_exchange: shard_cuts do not match this context's shards");
+  for (int r = 0; r < N; ++r)
+    if (shard_cuts[r] > shard_cuts[r + 1]) return fail(c, CMB_E_ARG, "cmb_shard_exchange: shard_cuts must be non-decreasing");
+  CU_TRY(c, cudaSetDevice(c->device));
+  if (c->local_barrier) c->local_barrier->arrive_and_wait();
+  // each owner broadcasts its columns in place (shard k's column sits at k * n_pairs on every rank), the owner of shard 0 its names
+  NCCL_TRY(c, ncclGroupStart());
+  for (int r = 0; r < N; ++r) {
+    const size_t n = (size_t)(shard_cuts[r + 1] - shard_cuts[r]) * s.n_pairs * 4;
+    int32_t* p = s.d_score.p + (uint64_t)shard_cuts[r] * s.n_pairs;
+    if (n) NCCL_TRY(c, ncclBroadcast(p, p, n, ncclChar, r, c->comm, c->stream));
+    if (shard_cuts[r] == 0 && shard_cuts[r + 1] > 0 && s.n_prim[0])
+      NCCL_TRY(c, ncclBroadcast(s.d_hash0.p, s.d_hash0.p, 8 * s.n_prim[0], ncclChar, r, c->comm, c->stream));
+  }
+  NCCL_TRY(c, ncclGroupEnd());
+  CU_TRY(c, cudaStreamSynchronize(c->stream));
+  return CMB_OK;
+}
+
+extern "C" int cmb_shard_choose(cmb_ctx* c, uint64_t* err_key) {
+  NvtxRange nvtx_fn("cmb_shard_choose");
+  if (!c || !err_key) return fail(c, CMB_E_ARG, "cmb_shard_choose: null argument");
+  auto& s = c->sh;
+  if (!c->in_sample || !s.active || !s.group || s.stage != 1) return fail(c, CMB_E_ARG, "cmb_shard_choose: call cmb_shard_score (and exchange the scores) first");
+  CU_TRY(c, cudaSetDevice(c->device));
+  CU_TRY(c, cudaEventRecord(s.ev[0], c->stream));
+  const uint64_t n0 = s.n_prim[0];
+  for (uint32_t k = std::max<uint32_t>(1, s.first); k < s.last; ++k) {
+    const uint64_t n = std::min(s.store[k].n_prim, n0);
+    if (n) ks_names<<<(uint32_t)((n + 255) / 256), 256, 0, c->stream>>>(s.store[k].names.p, s.d_hash0.p, n, k, s.d_err);
+  }
+  if (s.n_pairs) ks_choose<<<(uint32_t)((s.n_pairs + 255) / 256), 256, 0, c->stream>>>(s.d_score.p, s.n_pairs, s.n_shards, s.d_state.p);
+  CU_TRY(c, cudaGetLastError());
+  CU_TRY(c, cudaEventRecord(s.ev[1], c->stream));
+  CU_TRY(c, cudaEventSynchronize(s.ev[1]));
+  float ms = 0;
+  cudaEventElapsedTime(&ms, s.ev[0], s.ev[1]);
+  s.ms_choose += ms;
+  CU_TRY(c, cudaEventRecord(s.ev[2], c->stream));
+  ShardSortArgs a{};
+  unsigned long long key;
+  if (int rc = shard_count(c, a, &key)) return rc;
+  *err_key = key;
+  s.stage = 2;
+  return CMB_OK;
+}
+
+extern "C" int cmb_shard_finish_group(cmb_ctx* c, uint64_t err_key, cmb_shard_result* out) {
+  NvtxRange nvtx_fn("cmb_shard_finish_group");
+  if (!c || !out) return fail(c, CMB_E_ARG, "cmb_shard_finish_group: null argument");
+  auto& s = c->sh;
+  if (!c->in_sample || !s.active || !s.group || s.stage != 2) return fail(c, CMB_E_ARG, "cmb_shard_finish_group: call cmb_shard_choose first");
+  s.active = false;
+  CU_TRY(c, cudaSetDevice(c->device));
+  *out = cmb_shard_result{};
+  if (int rc = shard_key_error(c, err_key)) return rc;
+  // shard_count's view of the device buffers, rebuilt (the choice and the counts are on the device)
+  ShardSortArgs a{};
+  a.stores = s.d_stores; a.tid_offsets = s.d_tid_offsets; a.state = s.d_state; a.n_pairs = s.n_pairs;
+  a.n_contigs = c->gene_mode ? c->n_ref_contigs : c->n_contigs; a.tid_count = s.d_tid_count; a.err = s.d_err;
+  a.own_begin = s.first; a.own_end = s.last;
+  return shard_sort_submit(c, a, out);
 }

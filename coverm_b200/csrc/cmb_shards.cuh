@@ -40,6 +40,7 @@ struct ShardScanArgs {
   int32_t* as_val;              // [primaries] this shard's AS values (ks_pairs reads them)
   uint8_t* as_state;
   unsigned long long* hash0;    // shard 0's name hashes; written by shard 0, compared by the others
+  unsigned long long* names;    // group runs, shards k > 0: this shard's name hashes, compared later by ks_names
   uint64_t n0;                  // primaries of shard 0 (complete before shard 1's first slice)
   uint32_t shard;
   int32_t tid_offset;
@@ -133,6 +134,7 @@ __global__ void __launch_bounds__(256) ks_compact(const ShardScanArgs a) {
   a.as_state[j] = (uint8_t)as_state;
   // the name check of read_a_record_set (shard_bam_reader.rs:88-108): set j of every shard carries one read name
   if (a.shard == 0) a.hash0[j] = h;
+  else if (a.names) a.names[j] = h;
   else if (j < a.n0 && a.hash0[j] != h) atomicMin(a.err, sh_key(j, a.shard, SHE_NAME, 0));
 }
 
@@ -154,6 +156,8 @@ struct ShardPairArgs {
   uint32_t shard;
   int32_t tid_offset;
   unsigned long long* err;
+  int32_t* score;           // ks_score: this shard's column of the score table
+  uint64_t n_score;         // its length: the pairs every shard holds
 };
 
 // the t-th tied candidate (t >= 2) replaces the winner with probability 1/t
@@ -162,46 +166,95 @@ __device__ __forceinline__ bool sh_take_tie(uint64_t pair, uint32_t shard, uint3
   return (uint32_t)(((r >> 32) * (unsigned long long)t) >> 32) == 0;
 }
 
-__global__ void __launch_bounds__(256) ks_pairs(const ShardPairArgs a) {
-  const uint64_t j = (uint64_t)blockIdx.x * 256 + threadIdx.x;
-  if (j >= a.n_pairs) return;
+// Pair j's summed AS in this shard; false when the shard is no candidate for it or its records are in error (the error folded)
+__device__ __forceinline__ bool sh_pair_score(const ShardPairArgs& a, uint64_t j, long long& score) {
   const uint64_t m1 = 2 * j, m2 = m1 + 1;
   const int32_t tid = a.st.b.tid[m1];
   const int32_t local = tid - a.tid_offset;
   // a shard is a candidate unless its first mate is placed on an excluded contig; the second mate is not looked at
   if (local >= 0 && a.excluded && a.excluded[tid] == 2) {  // the contig's name has no genome separator: the reference panics
     atomicMin(a.err, sh_key(m2, SHP_SCORE + a.shard, SHE_NO_SEPARATOR, 0));
-    return;
+    return false;
   }
-  if (local >= 0 && a.excluded && a.excluded[tid]) return;
-  long long score = 0;
+  if (local >= 0 && a.excluded && a.excluded[tid]) return false;
+  score = 0;
   const uint64_t at = m2;  // the choice follows the pair's second set
   if (!(a.st.b.flag[m1] & 0x4)) {
     if (a.as_state[m1] != 1) {
       atomicMin(a.err, sh_key(at, SHP_SCORE + a.shard, a.as_state[m1] ? SHE_AS_TYPE : SHE_AS_MISSING, a.as_state[m1]));
-      return;
+      return false;
     }
     score += a.as_val[m1];
   }
   if (!(a.st.b.flag[m2] & 0x4)) {
     if (a.as_state[m2] != 1) {
       atomicMin(a.err, sh_key(at, SHP_SCORE + a.shard, a.as_state[m2] ? SHE_AS_TYPE : SHE_AS_MISSING, a.as_state[m2]));
-      return;
+      return false;
     }
     score += a.as_val[m2];
   }
-  PairState s = a.state[j];
+  return true;
+}
+
+// The running winner after shard k: first candidate or higher score takes the pair, the t-th tie takes it when sh_take_tie says so
+__device__ __forceinline__ bool sh_update(PairState& s, uint64_t j, uint32_t shard, long long score) {
   if (s.winner == SH_NONE || score > s.best) {
     s.best = score;
-    s.winner = a.shard;
+    s.winner = shard;
     s.ties = 1;
   } else if (score == s.best) {
     s.ties += 1;
-    if (sh_take_tie(j, a.shard, s.ties)) s.winner = a.shard;
+    if (sh_take_tie(j, shard, s.ties)) s.winner = shard;
   } else {
-    return;
+    return false;
   }
-  a.state[j] = s;
+  return true;
+}
+
+__global__ void __launch_bounds__(256) ks_pairs(const ShardPairArgs a) {
+  const uint64_t j = (uint64_t)blockIdx.x * 256 + threadIdx.x;
+  if (j >= a.n_pairs) return;
+  long long score;
+  if (!sh_pair_score(a, j, score)) return;
+  PairState s = a.state[j];
+  if (sh_update(s, j, a.shard, score)) a.state[j] = s;
+}
+
+// ---- group runs (several GPUs, each decoding a run of whole shards): the choice goes through a table of scores instead of the
+// running state, so that the ranks can exchange it.  A column holds one int32 per pair: AS values are of type C or S, so a
+// pair's sum is below 2^17, and the sentinels are negative.
+constexpr int32_t SH_SCORE_NONE = -1;  // the shard is no candidate for the pair
+constexpr int32_t SH_SCORE_ERR = -2;   // the pair's records in this shard are in error (folded into the rank's error key)
+
+// One thread per pair the shard holds with shard 0: its errors folded as ks_pairs folds them, its score into the column
+__global__ void __launch_bounds__(256) ks_score(const ShardPairArgs a) {
+  const uint64_t j = (uint64_t)blockIdx.x * 256 + threadIdx.x;
+  if (j >= a.n_pairs) return;
+  long long score = 0;
+  const uint64_t m1 = 2 * j;
+  const int32_t tid = a.st.b.tid[m1];
+  const bool candidate = sh_pair_score(a, j, score);
+  const bool excluded = tid - a.tid_offset >= 0 && a.excluded && a.excluded[tid] == 1;
+  if (j < a.n_score) a.score[j] = candidate ? (int32_t)score : excluded ? SH_SCORE_NONE : SH_SCORE_ERR;
+}
+
+// The name check of read_a_record_set for a shard decoded away from shard 0: its primary j against shard 0's, once hash0 arrived
+__global__ void __launch_bounds__(256) ks_names(const unsigned long long* names, const unsigned long long* hash0, uint64_t n, uint32_t shard,
+                                                unsigned long long* err) {
+  const uint64_t j = (uint64_t)blockIdx.x * 256 + threadIdx.x;
+  if (j < n && names[j] != hash0[j]) atomicMin(err, sh_key(j, shard, SHE_NAME, 0));
+}
+
+// One thread per pair: the columns walked in shard order with ks_pairs' rule, so every rank reaches the winner one GPU reaches
+__global__ void __launch_bounds__(256) ks_choose(const int32_t* score, uint64_t n_pairs, uint32_t n_shards, PairState* state) {
+  const uint64_t j = (uint64_t)blockIdx.x * 256 + threadIdx.x;
+  if (j >= n_pairs) return;
+  PairState s{0, SH_NONE, 0};
+  for (uint32_t k = 0; k < n_shards; ++k) {
+    const int32_t v = score[(uint64_t)k * n_pairs + j];
+    if (v >= 0) sh_update(s, j, k, v);
+  }
+  state[j] = s;
 }
 
 struct ShardSortArgs {
@@ -216,6 +269,7 @@ struct ShardSortArgs {
   cmb_read_batch out;
   uint64_t n_out;
   unsigned long long* err;
+  uint32_t own_begin, own_end;    // the shards whose winners this context sorts (a group rank's run; else all)
 };
 
 // A winner's record goes to the coverage loop when it is mapped (contig.rs:124 skips the others; they still count as reads)
@@ -231,6 +285,7 @@ __global__ void __launch_bounds__(256) ks_count(const ShardSortArgs a) {
     atomicMin(a.err, sh_key(2 * j + 1, SHP_CHOOSE, SHE_EXCLUDED, 0));
     return;
   }
+  if (w < a.own_begin || w >= a.own_end) return;
   const ShardStore s = a.stores[w];
   for (uint64_t m = 2 * j; m < 2 * j + 2; ++m) {
     const uint32_t info = s.info[m];
@@ -248,7 +303,7 @@ __global__ void __launch_bounds__(256) ks_scatter(const ShardSortArgs a) {
   const uint64_t j = (uint64_t)blockIdx.x * 256 + threadIdx.x;
   if (j >= a.n_pairs) return;
   const uint32_t w = a.state[j].winner;
-  if (w == SH_NONE) return;
+  if (w == SH_NONE || w < a.own_begin || w >= a.own_end) return;
   const ShardStore s = a.stores[w];
   for (uint64_t m = 2 * j; m < 2 * j + 2; ++m) {
     if (!sh_emitted(s, m) || (uint32_t)s.b.tid[m] >= a.n_contigs) continue;

@@ -424,7 +424,6 @@ inline CliResult run_cli_rank(const std::vector<std::string>& args, const std::v
     }
     // --sharded makes the BAMs one sample, unless a read filter is given: then the reference ignores it (coverm.rs:168-187, 546-563)
     if (o.sharded && !plan.params.filtering) {
-      if (o.gpus > 1) throw ExitError(1, "--sharded input runs on one GPU: drop --gpus");
       InputSpec all;
       all.path = o.bam_files[0];
       all.shards = inputs;

@@ -19,6 +19,15 @@ extern "C" int cmb_set_genes_range(cmb_ctx* ctx, uint32_t n_contigs, const uint6
 extern "C" int cmb_shard_begin(cmb_ctx* ctx, uint32_t n_shards, const uint32_t* tid_offsets, const uint8_t* excluded) __attribute__((weak));
 extern "C" int cmb_shard_add(cmb_ctx* ctx, const cmb_bgzf_input* in, cmb_bgzf_result* out) __attribute__((weak));
 extern "C" int cmb_shard_finish(cmb_ctx* ctx, cmb_shard_result* out) __attribute__((weak));
+// ... and so are the entry points of sharded input over a group of ranks: without them a group --sharded run stops on every rank.
+extern "C" int cmb_shard_begin_range(cmb_ctx* ctx, uint32_t n_shards, const uint32_t* tid_offsets, const uint8_t* excluded, uint32_t shard_begin,
+                                     uint32_t shard_end) __attribute__((weak));
+extern "C" int cmb_shard_score(cmb_ctx* ctx, const uint64_t* n_primary) __attribute__((weak));
+extern "C" int cmb_shard_exchange(cmb_ctx* ctx, const uint32_t* shard_cuts) __attribute__((weak));
+extern "C" int cmb_shard_export(cmb_ctx* ctx, uint32_t shard, int32_t* scores, uint64_t* names) __attribute__((weak));
+extern "C" int cmb_shard_import(cmb_ctx* ctx, uint32_t shard, const int32_t* scores, const uint64_t* names) __attribute__((weak));
+extern "C" int cmb_shard_choose(cmb_ctx* ctx, uint64_t* err_key) __attribute__((weak));
+extern "C" int cmb_shard_finish_group(cmb_ctx* ctx, uint64_t err_key, cmb_shard_result* out) __attribute__((weak));
 
 namespace cmbh {
 
@@ -158,18 +167,14 @@ class DeviceSession {
 
   // One sample.  In a group every rank must call this for the same input (it is collective).
   SampleResult process(const InputSpec& in, const cmb_params& params) {
-    if (!in.shards.empty()) {
-      if (group_n_ > 1) throw ExitError(1, "--sharded input runs on one GPU: drop --gpus");
-      return process_sharded(in, params);
-    }
-    if (group_n_ <= 1) return process_local(in, params, nullptr);
-    // ---- local phase: this rank's contigs, from this rank's block range.  Nothing may escape before the ranks have
-    //      compared notes: a rank that failed still takes part in the exchange, and then every rank fails the same way.
+    if (group_n_ <= 1) return in.shards.empty() ? process_local(in, params, nullptr) : process_sharded(in, params);
+    // ---- local phase: this rank's contigs, from this rank's block range (sharded input: from this rank's shards).  Nothing
+    //      may escape before the ranks have compared notes: a rank that failed still takes part in the exchange, and then
+    //      every rank fails the same way.
     ShardState sh;
     SampleResult res;
-    RankSummary mine{};
-    try {
-      res = process_local(in, params, &sh);
+    RankSummary mine = attempt([&](RankSummary& mine) {
+      res = in.shards.empty() ? process_local(in, params, &sh) : process_sharded_group(in, params, sh);
       mine.n_records = res.n_records;
       mine.n_primary = res.num_detected_primary_alignments;
       mine.counts_global = sh.counts_global ? 1 : 0;
@@ -179,19 +184,7 @@ class DeviceSession {
       if (!sh.counts_global) cmb_kept_tid_range(ctx_, &lo, &hi);
       mine.min_tid = lo;
       mine.max_tid = hi;
-    } catch (const Panic& e) {
-      mine.kind = 1;
-      mine.code = 101;
-      snprintf(mine.message, sizeof mine.message, "%s", e.what());
-    } catch (const ExitError& e) {
-      mine.kind = 2;
-      mine.code = e.code;
-      snprintf(mine.message, sizeof mine.message, "%s", e.what());
-    } catch (const std::exception& e) {
-      mine.kind = 1;
-      mine.code = 101;
-      snprintf(mine.message, sizeof mine.message, "%s", e.what());
-    }
+    });
     HostRange nvtx_gather("host: rank summaries + table gather");
     const double t_g0 = now_s();
     std::vector<RankSummary> all((size_t)group_n_);
@@ -242,6 +235,46 @@ class DeviceSession {
     uint32_t counts_global, reserved;
     char message[208];
   };
+
+  // `f` run with its failure, if any, recorded as what this rank tells the others (the fields f filled are kept)
+  template <class F>
+  static RankSummary attempt(F&& f) {
+    RankSummary mine{};
+    try {
+      f(mine);
+    } catch (const Panic& e) {
+      mine.kind = 1;
+      mine.code = 101;
+      snprintf(mine.message, sizeof mine.message, "%s", e.what());
+    } catch (const ExitError& e) {
+      mine.kind = 2;
+      mine.code = e.code;
+      snprintf(mine.message, sizeof mine.message, "%s", e.what());
+    } catch (const std::exception& e) {
+      mine.kind = 1;
+      mine.code = 101;
+      snprintf(mine.message, sizeof mine.message, "%s", e.what());
+    }
+    return mine;
+  }
+
+  // Every rank's summary and `bytes` of payload behind it (all ranks send the same size); the lowest failing rank's error is
+  // thrown on every rank.  Returns the ranks' payloads, rank after rank.
+  std::vector<uint8_t> agree(const RankSummary& mine, const void* payload, size_t bytes) {
+    const size_t each = sizeof(RankSummary) + bytes;
+    std::vector<uint8_t> send(each), recv(each * (size_t)group_n_), out(bytes * (size_t)group_n_);
+    memcpy(send.data(), &mine, sizeof mine);
+    if (bytes) memcpy(send.data() + sizeof mine, payload, bytes);
+    group_allgather(send.data(), recv.data(), each);
+    for (int r = 0; r < group_n_; ++r) {
+      RankSummary s;
+      memcpy(&s, recv.data() + (size_t)r * each, sizeof s);
+      if (s.kind == 1) throw Panic(s.message);
+      if (s.kind == 2) throw ExitError(s.code, s.message);
+      if (bytes) memcpy(out.data() + (size_t)r * bytes, recv.data() + (size_t)r * each + sizeof s, bytes);
+    }
+    return out;
+  }
 
   // The cross-rank half of the sortedness check (contig.rs:129-132): each rank has verified its own (overlapping) stretch of
   // the stream; the kept tids of the ranks' exclusive shares must not decrease from rank to rank either.
@@ -363,6 +396,16 @@ class DeviceSession {
     return c.end_sample();
   }
 
+  // Ends the sample a sharded run began when the run stops on an error, so that the session can take the next sample
+  struct SampleCloser {
+    cmb_ctx* ctx;
+    bool open = false;
+    ~SampleCloser() {
+      uint64_t n_pairs = 0;
+      if (open) cmb_end_sample(ctx, nullptr, nullptr, 0, &n_pairs);
+    }
+  };
+
   // --sharded (ReadSortedShardedBamReader, shard_bam_reader.rs): the shards' headers concatenated into one reference, every
   // shard decoded on the device in turn, each pair's best shard chosen there and the winners accumulated as one sample.
   SampleResult process_sharded(const InputSpec& in, const cmb_params& params) {
@@ -372,11 +415,160 @@ class DeviceSession {
     if (set_params(params)) throw ExitError(1, "--sharded input takes no read-pair filter");
     SampleResult res;
     const size_t K = in.shards.size();
-    std::vector<uint32_t> offsets(K);
+    std::vector<uint32_t> offsets;
+    sharded_header(in, res, offsets, nullptr);
+    const uint32_t n_ref = (uint32_t)res.hdr->names.size();
+    const uint32_t n_rows = sharded_reference(res, nullptr, 0, n_ref);
+    SampleCloser closer{ctx_, true};
+    const std::vector<uint8_t> excluded = sharded_excluded(in, res);
+    int rc;
+    if ((rc = cmb_shard_begin(ctx_, (uint32_t)K, offsets.data(), in.excluded ? excluded.data() : nullptr))) throw_device_error(ctx_, rc);
+    double decode_s = 0;
+    for (size_t k = 0; k < K; ++k) add_shard(in, k, res, decode_s);
+    cmb_shard_result sr{};
+    if ((rc = cmb_shard_finish(ctx_, &sr))) throw_shard_error(in, rc);
+    res.num_detected_primary_alignments = sr.n_records;
+    print_shard_stats(K, sr);
+    const double t_dec = now_s();
+    closer.open = false;
+    sharded_end(res, params, n_ref, n_rows, nullptr);
+    const double t1 = now_s();
+    res.timing.total_s = t1 - t0;
+    res.timing.decode_s = decode_s;
+    res.timing.end_sample_s = t1 - t_dec;
+    return res;
+  }
+
+  // --sharded over the ranks of a group: rank r decodes the whole shards [cuts[r], cuts[r + 1]) (shard_run_cuts over the files'
+  // sizes) and owns their contigs.  A pair's winning records lie on the winning shard's contigs, so only every pair's scores
+  // travel: exchange A the shards' primary counts, exchange B the score columns and shard 0's name hashes, exchange C the
+  // smallest error key.  Every rank then reaches the winners and the error the one-GPU run reaches, sorts and submits the
+  // winners of its own shards, and leaves its rows to the group's gather (process()).
+  SampleResult process_sharded_group(const InputSpec& in, const cmb_params& params, ShardState& sh) {
+    HostRange nvtx_sample("host: sharded sample (group)");
+    const double t0 = now_s();
+    const int N = group_n_, me = group_rank_;
+    const size_t K = in.shards.size();
+    SampleResult res;
+    std::vector<uint32_t> offsets, scut;
+    std::vector<uint64_t> n_prim(K, 0);
+    double decode_s = 0;
+    uint32_t n_ref = 0, n_rows = 0;
+    int rc;
+    SampleCloser closer{ctx_};
+    // ---- this rank's shards, decoded and compacted
+    RankSummary mine = attempt([&](RankSummary&) {
+      if (!cmb_shard_begin_range || !cmb_shard_add || !cmb_shard_score || !cmb_shard_choose || !cmb_shard_finish_group ||
+          (group_nccl_ ? !cmb_shard_exchange : (!cmb_shard_export || !cmb_shard_import)))
+        throw ExitError(1, "this device library has no cmb_shard_begin_range / cmb_shard_score / cmb_shard_choose / cmb_shard_finish_group "
+                           "(and cmb_shard_exchange, or cmb_shard_export / cmb_shard_import): --sharded over several ranks needs them");
+      if (set_params(params)) throw ExitError(1, "--sharded input takes no read-pair filter");
+      std::vector<uint64_t> sizes;
+      sharded_header(in, res, offsets, &sizes);
+      n_ref = (uint32_t)res.hdr->names.size();
+      scut = shard_run_cuts(sizes, N);
+      sh.cuts.assign((size_t)N + 1, n_ref);
+      for (int r = 0; r <= N; ++r)
+        if (scut[(size_t)r] < K) sh.cuts[(size_t)r] = offsets[scut[(size_t)r]];
+      n_rows = sharded_reference(res, &sh, sh.cuts[(size_t)me], sh.cuts[(size_t)me + 1]);
+      closer.open = true;
+      const std::vector<uint8_t> excluded = sharded_excluded(in, res);
+      if ((rc = cmb_shard_begin_range(ctx_, (uint32_t)K, offsets.data(), in.excluded ? excluded.data() : nullptr, scut[(size_t)me], scut[(size_t)me + 1])))
+        throw_device_error(ctx_, rc);
+      for (uint32_t k = scut[(size_t)me]; k < scut[(size_t)me + 1]; ++k) n_prim[k] = add_shard(in, k, res, decode_s);
+    });
+    // ---- exchange A: every shard's primaries (each from its owner; the others send 0)
+    double xs = 0;
+    double a = now_s();
+    const std::vector<uint8_t> counts = agree(mine, n_prim.data(), 8 * K);
+    for (size_t k = 0; k < K; ++k) {
+      n_prim[k] = 0;
+      for (int r = 0; r < N; ++r) {
+        uint64_t v;
+        memcpy(&v, counts.data() + ((size_t)r * K + k) * 8, 8);
+        n_prim[k] += v;
+      }
+    }
+    xs += now_s() - a;
+    const uint64_t n0 = n_prim[0], n_pairs = *std::min_element(n_prim.begin(), n_prim.end()) / 2;
+    agree(attempt([&](RankSummary&) {
+            if ((rc = cmb_shard_score(ctx_, n_prim.data()))) throw_device_error(ctx_, rc);
+          }),
+          nullptr, 0);
+    // ---- exchange B: the score table and shard 0's names on every rank
+    a = now_s();
+    if (group_nccl_) {
+      if ((rc = cmb_shard_exchange(ctx_, scut.data()))) throw ExitError(1, std::string("score exchange over NCCL failed: ") + cmb_last_error(ctx_));
+    } else {
+      exchange_scores_through_host(scut, n_pairs, n0);
+    }
+    xs += now_s() - a;
+    // ---- exchange C: the choice on every rank, and the smallest error key of the group
+    a = now_s();
+    uint64_t key = ~0ull;
+    const std::vector<uint8_t> keys = agree(attempt([&](RankSummary&) {
+                                              if ((rc = cmb_shard_choose(ctx_, &key))) throw_device_error(ctx_, rc);
+                                            }),
+                                            &key, 8);
+    for (int r = 0; r < N; ++r) {
+      uint64_t v;
+      memcpy(&v, keys.data() + (size_t)r * 8, 8);
+      key = std::min(key, v);
+    }
+    xs += now_s() - a;
+    cmb_shard_result sr{};
+    if ((rc = cmb_shard_finish_group(ctx_, key, &sr))) throw_shard_error(in, rc);
+    // the sample's primaries are a global count: rank 0 alone reports them, the group's sum of the ranks' counters is then right
+    res.num_detected_primary_alignments = me == 0 ? sr.n_records : 0;
+    print_shard_stats(K, sr);
+    if (getenv("CMB_PIPELINE_STATS"))
+      fprintf(stderr, "#shard_exchange\tbytes=%llu\tms=%.3f\trank=%d\tshards=%u..%u\tdecode_ms=%.3f\tchoose_ms=%.3f\tsort_ms=%.3f\n",
+              (unsigned long long)(4 * K * n_pairs + 8 * n0), xs * 1e3, me, scut[(size_t)me], scut[(size_t)me + 1], sr.ms_decode, sr.ms_choose, sr.ms_sort);
+    const double t_dec = now_s();
+    closer.open = false;
+    sharded_end(res, params, n_ref, n_rows, &sh);
+    const double t1 = now_s();
+    res.timing.total_s = t1 - t0;
+    res.timing.decode_s = decode_s;
+    res.timing.end_sample_s = t1 - t_dec;
+    return res;
+  }
+
+  // Exchange B without NCCL: each rank's columns (shard 0's owner: its names first) through the caller's all-gather, padded to
+  // the largest share
+  void exchange_scores_through_host(const std::vector<uint32_t>& scut, uint64_t n_pairs, uint64_t n0) {
+    const int N = group_n_, me = group_rank_;
+    auto owns0 = [&](int r) { return scut[(size_t)r] == 0 && scut[(size_t)r + 1] > 0; };
+    auto share = [&](int r) { return (size_t)(scut[(size_t)r + 1] - scut[(size_t)r]) * n_pairs * 4 + (owns0(r) ? 8 * n0 : 0); };
+    size_t max_b = 0;
+    for (int r = 0; r < N; ++r) max_b = std::max(max_b, share(r));
+    if (!max_b) return;
+    std::vector<uint8_t> send(max_b), recv(max_b * (size_t)N);
+    // names (8-byte aligned) at the front, then the columns in shard order
+    auto columns = [&](int r, uint8_t* base, bool out) {
+      uint64_t* names = owns0(r) ? (uint64_t*)base : nullptr;
+      int32_t* col = (int32_t*)(base + (names ? 8 * n0 : 0));
+      for (uint32_t k = scut[(size_t)r]; k < scut[(size_t)r + 1]; ++k, col += n_pairs) {
+        const int rc = out ? cmb_shard_export(ctx_, k, col, k == 0 ? names : nullptr) : cmb_shard_import(ctx_, k, col, k == 0 ? names : nullptr);
+        if (rc) throw_device_error(ctx_, rc);
+      }
+    };
+    columns(me, send.data(), true);
+    group_allgather(send.data(), recv.data(), max_b);
+    for (int r = 0; r < N; ++r)
+      if (r != me) columns(r, recv.data() + (size_t)r * max_b, false);
+  }
+
+  // The shards' headers concatenated (shard_bam_reader.rs:315-336) into res.hdr: offsets[k] = the targets of shards 0 .. k-1;
+  // `sizes` (when given): the shard files' bytes
+  void sharded_header(const InputSpec& in, SampleResult& res, std::vector<uint32_t>& offsets, std::vector<uint64_t>* sizes) {
+    const size_t K = in.shards.size();
+    offsets.assign(K, 0);
     auto hdr = std::make_shared<Header>();
-    for (size_t k = 0; k < K; ++k) {  // the concatenated header (shard_bam_reader.rs:315-336)
+    for (size_t k = 0; k < K; ++k) {
       res.stoit_name += (k ? "|" : "") + file_stem(in.shards[k].path);
       const BamInput input(in.shards[k]);
+      if (sizes) sizes->push_back(input.size());
       InflateStream stream(input.data(), input.size(), pool_, 1u << 20);
       std::vector<uint8_t> buf;
       const BamHeader h = read_bam_header(stream, buf, in.shards[k].path);
@@ -385,66 +577,101 @@ class DeviceSession {
       hdr->lens.insert(hdr->lens.end(), h.header->lens.begin(), h.header->lens.end());
     }
     res.hdr = hdr;
-    const uint32_t n_ref = (uint32_t)hdr->names.size();
+  }
+
+  // The device's reference (or genes) over the contigs [tb, te) -- in a group (`sh`) this rank's, with every rank's ranges in
+  // sh.cuts -- and the sample begun.  Returns the rows of the table.
+  uint32_t sharded_reference(SampleResult& res, ShardState* sh, uint32_t tb, uint32_t te) {
+    const Header& hdr = *res.hdr;
+    const uint32_t n_ref = (uint32_t)hdr.names.size();
     uint32_t n_rows = n_ref;
     int rc;
     if (gene_defs_) {
-      gene_cache_ = std::make_shared<ResolvedGenes>(resolve_genes_against_header(*gene_defs_, *hdr, gene_namer_));
-      gene_cache_names_ = hdr->names;
+      gene_cache_ = std::make_shared<ResolvedGenes>(resolve_genes_against_header(*gene_defs_, hdr, gene_namer_));
       std::vector<cmb_gene> genes(gene_cache_->entries.size());
       for (size_t g = 0; g < genes.size(); ++g) genes[g] = cmb_gene{gene_cache_->entries[g].tid, gene_cache_->entries[g].start, gene_cache_->entries[g].end};
       n_rows = std::max<uint32_t>(1, (uint32_t)genes.size());
-      rc = cmb_set_genes(ctx_, n_ref, hdr->lens.data(), (uint32_t)genes.size(), genes.data());
+      if (sh) {
+        if (!cmb_set_genes_range) throw ExitError(1, "this device library has no cmb_set_genes_range: --gff needs it over several ranks");
+        sh->row_cuts = gene_row_cuts(sh->cuts, gene_cache_->first_of_tid, n_rows);
+        rc = cmb_set_genes_range(ctx_, n_ref, hdr.lens.data(), (uint32_t)genes.size(), genes.data(), tb, te);
+      } else {
+        rc = cmb_set_genes(ctx_, n_ref, hdr.lens.data(), (uint32_t)genes.size(), genes.data());
+      }
       res.genes = gene_cache_;
     } else {
-      SampleCall::check_layout_fits(hdr->lens, {0, n_ref});
-      rc = cmb_set_reference(ctx_, n_ref, hdr->lens.data(), 0, n_ref);
+      SampleCall::check_layout_fits(hdr.lens, sh ? sh->cuts : std::vector<uint32_t>{0, n_ref});
+      if (sh) sh->row_cuts = sh->cuts;
+      rc = cmb_set_reference(ctx_, n_ref, hdr.lens.data(), tb, te);
     }
     if (rc) throw_device_error(ctx_, rc);
     ref_lens_.clear();  // the next ordinary sample sets its own reference
     gene_cache_names_.clear();
+    if (sh) {
+      res.timing.tid_begin = tb;
+      res.timing.tid_end = te;
+    }
     if ((rc = cmb_begin_sample(ctx_))) throw_device_error(ctx_, rc);
+    return n_rows;
+  }
+
+  static std::vector<uint8_t> sharded_excluded(const InputSpec& in, const SampleResult& res) {
     std::vector<uint8_t> excluded;
     if (in.excluded) {
+      const uint32_t n_ref = (uint32_t)res.hdr->names.size();
       excluded.resize(n_ref);
-      for (uint32_t t = 0; t < n_ref; ++t) excluded[t] = in.excluded(hdr->names[t]);
+      for (uint32_t t = 0; t < n_ref; ++t) excluded[t] = in.excluded(res.hdr->names[t]);
     }
-    if ((rc = cmb_shard_begin(ctx_, (uint32_t)K, offsets.data(), in.excluded ? excluded.data() : nullptr))) throw_device_error(ctx_, rc);
-    double decode_s = 0;
-    for (size_t k = 0; k < K; ++k) {
-      const double a = now_s();
-      const BamInput input(in.shards[k]);
-      InflateStream stream(input.data(), input.size(), pool_, 1u << 20);
-      std::vector<uint8_t> buf;
-      const BamHeader h = read_bam_header(stream, buf, in.shards[k].path);
-      const BlockIndex& bx = stream.index();
-      if (!bx.bgzf) throw ExitError(1, "shard " + in.shards[k].path + " is not a BGZF-compressed BAM file: sharded input is decoded on the GPU only");
-      BgzfInput bi(bx, (uint32_t)h.header->names.size(), h.records_at, pool_.size());
-      cmb_bgzf_result br{};
-      rc = cmb_shard_add(ctx_, &bi.in, &br);
-      if (rc == CMB_E_DECLINED) throw ExitError(1, "cannot read shard " + in.shards[k].path + ": " + cmb_last_error(ctx_));
-      if (rc) throw_device_error(ctx_, rc);
-      res.n_records += br.n_records;
-      decode_s += now_s() - a;
-    }
-    cmb_shard_result sr{};
-    if ((rc = cmb_shard_finish(ctx_, &sr))) {
-      const std::string msg = cmb_last_error(ctx_);
-      if (msg.rfind("Contig name does not contain", 0) == 0 && !in.unknown_genome_panic.empty()) throw Panic(in.unknown_genome_panic);
-      throw_device_error(ctx_, rc);
-    }
-    res.num_detected_primary_alignments = sr.n_records;
+    return excluded;
+  }
+
+  // Shard k through cmb_shard_add; returns its primaries
+  uint64_t add_shard(const InputSpec& in, size_t k, SampleResult& res, double& decode_s) {
+    const double a = now_s();
+    const BamInput input(in.shards[k]);
+    InflateStream stream(input.data(), input.size(), pool_, 1u << 20);
+    std::vector<uint8_t> buf;
+    const BamHeader h = read_bam_header(stream, buf, in.shards[k].path);
+    const BlockIndex& bx = stream.index();
+    if (!bx.bgzf) throw ExitError(1, "shard " + in.shards[k].path + " is not a BGZF-compressed BAM file: sharded input is decoded on the GPU only");
+    BgzfInput bi(bx, (uint32_t)h.header->names.size(), h.records_at, pool_.size());
+    cmb_bgzf_result br{};
+    const int rc = cmb_shard_add(ctx_, &bi.in, &br);
+    if (rc == CMB_E_DECLINED) throw ExitError(1, "cannot read shard " + in.shards[k].path + ": " + cmb_last_error(ctx_));
+    if (rc) throw_device_error(ctx_, rc);
+    res.n_records += br.n_records;
+    decode_s += now_s() - a;
+    return br.n_primary;
+  }
+
+  [[noreturn]] void throw_shard_error(const InputSpec& in, int rc) {
+    const std::string msg = cmb_last_error(ctx_);
+    if (msg.rfind("Contig name does not contain", 0) == 0 && !in.unknown_genome_panic.empty()) throw Panic(in.unknown_genome_panic);
+    throw_device_error(ctx_, rc);
+  }
+
+  static void print_shard_stats(size_t K, const cmb_shard_result& sr) {
     if (getenv("CMB_PIPELINE_STATS"))
       fprintf(stderr, "#reference_bytes\tshards=%zu\tshard_store=%llu\n#sharded\tpairs=%llu\temitted=%llu\tdecode_ms=%.3f\tchoose_ms=%.3f\tsort_ms=%.3f\n", K,
               (unsigned long long)sr.store_bytes, (unsigned long long)sr.n_pairs, (unsigned long long)sr.n_emitted, sr.ms_decode, sr.ms_choose, sr.ms_sort);
-    const double t_dec = now_s();
+  }
+
+  // The sample ended: its rows (in a group over NCCL they stay on the device for cmb_allgather_stats), histogram pairs and
+  // gene extras
+  void sharded_end(SampleResult& res, const cmb_params& params, uint32_t n_ref, uint32_t n_rows, ShardState* sh) {
     ensure_rows(n_rows);
     res.rows = rows_buf_;
     uint64_t n_pairs = 0;
-    if ((rc = cmb_end_sample(ctx_, rows_buf_, nullptr, 0, &n_pairs))) throw_device_error(ctx_, rc);
-    if ((params.want & CMB_WANT_HIST_CSR) && n_pairs) {
+    int rc;
+    const bool on_device = sh && group_nccl_;
+    if ((rc = cmb_end_sample(ctx_, on_device ? nullptr : rows_buf_, nullptr, 0, &n_pairs))) throw_device_error(ctx_, rc);
+    if (!on_device && (params.want & CMB_WANT_HIST_CSR) && n_pairs) {
       res.pairs.resize(n_pairs);
       if ((rc = cmb_fetch_pairs(ctx_, res.pairs.data(), n_pairs))) throw_device_error(ctx_, rc);
+    }
+    if (sh) {
+      sh->n_pairs = n_pairs;
+      if (!on_device) local_pairs_ = res.pairs;
     }
     if (gene_defs_) {
       res.contig_seen.assign((size_t)n_ref + 1, 0);
@@ -452,11 +679,6 @@ class DeviceSession {
     }
     cmb_get_timing(ctx_, &res.timing.device);
     res.timing.device_decode = true;
-    const double t1 = now_s();
-    res.timing.total_s = t1 - t0;
-    res.timing.decode_s = decode_s;
-    res.timing.end_sample_s = t1 - t_dec;
-    return res;
   }
 
   // One process_local call, handed from stage to stage.

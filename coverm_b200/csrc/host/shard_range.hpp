@@ -37,6 +37,37 @@ inline std::vector<uint32_t> tid_cuts_by_length(const std::vector<uint64_t>& len
 
 // 32-base spans the contigs [b, e) take in one device context's layout (at least one per contig, cmb_set_reference); a
 // context holds at most CMB_MAX_SPANS of them.
+// Sharded input over a group: rank r decodes the whole shards [cuts[r], cuts[r + 1]).  The runs are contiguous and the cut
+// minimises the largest run's summed size (compressed bytes); the smallest such bound is packed greedily from the first rank,
+// so ranks beyond the shards (n_ranks > shards) own empty runs at the end.
+inline std::vector<uint32_t> shard_run_cuts(const std::vector<uint64_t>& sizes, int n_ranks) {
+  const uint32_t K = (uint32_t)sizes.size();
+  auto pack = [&](uint64_t cap, std::vector<uint32_t>* cuts) {  // ranks used when each takes shards while they fit `cap`
+    int used = 0;
+    for (uint32_t k = 0; k < K; ++used) {
+      if (cuts) cuts->push_back(k);
+      uint64_t sum = 0;
+      do sum += sizes[k++];
+      while (k < K && sum + sizes[k] <= cap);
+    }
+    return used;
+  };
+  uint64_t lo = 0, hi = 0;
+  for (uint64_t x : sizes) {
+    lo = std::max(lo, x);
+    hi += x;
+  }
+  while (lo < hi) {  // the smallest cap that n_ranks runs can hold
+    const uint64_t mid = lo + (hi - lo) / 2;
+    if (pack(mid, nullptr) <= n_ranks) hi = mid;
+    else lo = mid + 1;
+  }
+  std::vector<uint32_t> cuts;
+  pack(lo, &cuts);
+  while ((int)cuts.size() <= n_ranks) cuts.push_back(K);
+  return cuts;
+}
+
 inline uint64_t layout_spans(const std::vector<uint64_t>& lens, uint32_t b, uint32_t e) {
   uint64_t s = 0;
   for (uint32_t t = b; t < e; ++t) s += std::max<uint64_t>(1, (lens[t] + 31) / 32);

@@ -336,6 +336,41 @@ typedef struct cmb_shard_result {
 int cmb_shard_begin(cmb_ctx* ctx, uint32_t n_shards, const uint32_t* tid_offsets, const uint8_t* excluded);
 int cmb_shard_add(cmb_ctx* ctx, const cmb_bgzf_input* in, cmb_bgzf_result* out);
 int cmb_shard_finish(cmb_ctx* ctx, cmb_shard_result* out);
+/* ---- Sharded input over a group of ranks (`--sharded --gpus N`, or N processes in one cmbh_session_set_group group) ----
+ * Rank r decodes a contiguous run of whole shards [shard_begin, shard_end) (the host cuts the shards by compressed size) and
+ * holds only its contigs [tid_offsets[shard_begin], tid_offsets[shard_end]) (cmb_set_reference / cmb_set_genes_range with that
+ * range): a winner's records lie on its shard's contigs, so no record moves between GPUs, only every pair's scores do.  Ranks
+ * beyond the shards own an empty run and still take part in every call and exchange.  The calls, between cmb_begin_sample and
+ * cmb_end_sample, in this order:
+ *   cmb_shard_begin_range: cmb_shard_begin plus this rank's run; then cmb_shard_add once per shard of the run, in order (each
+ *                    shard's store is built as on one GPU; the pair choice waits).
+ *   cmb_shard_score: n_primary[k] = every shard's primaries (cmb_bgzf_result.n_primary of its owner's cmb_shard_add, which the
+ *                    ranks exchange).  Writes one int32 column of the [n_shards][n_pairs] score table per owned shard (n_pairs =
+ *                    the shortest shard's primaries / 2): the pair's summed AS, or a negative sentinel when the shard is no
+ *                    candidate or the pair's records there are in error; the errors are kept like cmb_shard_finish's.
+ *   Exchange, either
+ *     cmb_shard_exchange: over the NCCL communicator (cmb_comm_init*): each owner broadcasts its columns, and the owner of shard 0
+ *                    its 8-byte name hashes of every primary, in place on the device.  shard_cuts[r] = rank r's shard_begin
+ *                    (n_ranks + 1 entries).  Collective.
+ *     or cmb_shard_export / cmb_shard_import: column `shard` (n_pairs int32) to / from the host, and with shard == 0 and names !=
+ *                    NULL shard 0's name hashes (n_primary[0] uint64), for groups whose ranks exchange host buffers.
+ *   cmb_shard_choose: checks the owned shards' read names against shard 0's, picks every pair's winner from the table with
+ *                    cmb_shard_finish's rule (every rank reaches the same winners), counts and checks the owned winners' records,
+ *                    and returns this rank's smallest error key (UINT64_MAX: none).
+ *   cmb_shard_finish_group: err_key = the smallest key over the ranks.  Not UINT64_MAX: returns the error cmb_shard_finish returns
+ *                    for it (the same on every rank).  Else sorts and submits the winners of the owned shards; `out` counts the
+ *                    sample's pairs and primaries (global) and this rank's emitted winners.
+ * Device memory per rank: the owned shards' stores, each with its AS columns (5 B per primary) and, after shard 0, its name
+ * hashes (8 B per primary), the score
+ * table (4 B per pair and shard), shard 0's name hashes (8 B per primary), the choice (16 B per pair) and the owned sorted winners. */
+int cmb_shard_begin_range(cmb_ctx* ctx, uint32_t n_shards, const uint32_t* tid_offsets, const uint8_t* excluded, uint32_t shard_begin,
+                          uint32_t shard_end);
+int cmb_shard_score(cmb_ctx* ctx, const uint64_t* n_primary);
+int cmb_shard_exchange(cmb_ctx* ctx, const uint32_t* shard_cuts);
+int cmb_shard_export(cmb_ctx* ctx, uint32_t shard, int32_t* scores, uint64_t* names);
+int cmb_shard_import(cmb_ctx* ctx, uint32_t shard, const int32_t* scores, const uint64_t* names);
+int cmb_shard_choose(cmb_ctx* ctx, uint64_t* err_key);
+int cmb_shard_finish_group(cmb_ctx* ctx, uint64_t err_key, cmb_shard_result* out);
 int cmb_filter_plan(cmb_ctx* ctx, int inverse, uint64_t* n_records, uint64_t* n_bytes);
 int cmb_filter_fetch(cmb_ctx* ctx, uint8_t* records, uint64_t n_bytes);
 
