@@ -787,3 +787,19 @@ __global__ void __launch_bounds__(256) kd_extract(const ExtractArgs a) {
   err = __reduce_or_sync(FULL, err);
   if (err && (threadIdx.x & 31) == 0) atomicOr(a.flags, err);
 }
+
+// A pair-mode slice of a sliced decode holds records [i0, n) back for the next slice (cmb_decode_slices.hpp): their share of
+// kd_extract's n_primary and n_owned, which the slice's result gives back (same ownership rule as kd_extract)
+__global__ void __launch_bounds__(256) kd_count_held(const int32_t* tid, const uint16_t* flag, uint32_t i0, uint32_t n, int32_t own_lo,
+                                                     int32_t own_hi, uint32_t own_unplaced, unsigned long long* n_primary,
+                                                     unsigned long long* n_owned) {
+  const uint32_t i = i0 + blockIdx.x * 256 + threadIdx.x;
+  bool owned = false, primary = false;
+  if (i < n) {
+    owned = tid[i] < 0 ? own_unplaced != 0 : (tid[i] >= own_lo && tid[i] < own_hi);
+    primary = owned && !(flag[i] & 0x900);
+  }
+  const uint32_t np = __popc(__ballot_sync(FULL, primary)), no = __popc(__ballot_sync(FULL, owned));
+  if ((threadIdx.x & 31) == 0 && np) atomicAdd(n_primary, (unsigned long long)np);
+  if ((threadIdx.x & 31) == 0 && no) atomicAdd(n_owned, (unsigned long long)no);
+}

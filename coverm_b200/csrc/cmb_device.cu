@@ -91,6 +91,7 @@ namespace {
 #include "cmb_filter.cuh"
 #include "cmb_shards.cuh"
 #include "cmb_shard_slices.hpp"
+#include "cmb_decode_slices.hpp"
 
 // rows[i].hist_offset += base for the rows that carry histogram pairs (cmb_allgather_stats: local -> global pair offsets)
 __global__ void __launch_bounds__(256) k_rebase_hist_offsets(cmb_contig_stats* rows, uint32_t n, uint64_t base) {
@@ -253,7 +254,8 @@ struct cmb_ctx {
     Buf<uint32_t> d_tickets;  // [0] block ticket, [1 + w] window w has arrived
     Buf<uint32_t> d_block_window;
     PinnedBuf<uint32_t> h_ones;  // source of the arrival flags
-    Buf<uint32_t> d_cnt;  // 16 words: [0] inflate failures [1] decode error bits [2] chain changed [4..5] n_primary [6..9] totals
+    Buf<uint32_t> d_cnt;  // 20 words: [0] inflate failures [1] decode error bits [2] chain changed [4..5] n_primary [6..9] totals
+                          // [10..11] n_owned; sliced decode: [12..14] pair cut (decode_sliced), [16..19] held-back counts
     Buf<uint64_t> d_rec_off;
     Buf<uint8_t> d_tuple_slab;
     uint32_t last_n_rec = 0, last_n_cig = 0;  // tuples of the last successful cmb_submit_bgzf (cmb_last_bgzf_batch)
@@ -692,8 +694,10 @@ int collect_errors_and_timing(cmb_ctx* c, uint32_t* counters_out) {
 }
 
 // Mate matching over the resident inflated stream (cmb_pairs.cuh); sets d.last_mate.  filter_out: ReferenceSortedBamFilter's
-// (false only for `coverm filter --inverse`).  Declines when the stream needs the host's file-order walk.
-int match_mates(cmb_ctx* c, const uint8_t* infl_base, uint32_t n_rec, bool filter_out, const char* who) {
+// (false only for `coverm filter --inverse`).  Declines when the stream needs the host's file-order walk.  A slice of a sliced
+// decode passes the largest eligible tid of the slices before it (`carry`) and gets its own largest in *largest (device).
+int match_mates(cmb_ctx* c, const uint8_t* infl_base, uint32_t n_rec, bool filter_out, const char* who, uint32_t carry = 0,
+                uint32_t* largest = nullptr) {
   auto& d = c->dec;
   int rc;
   d.last_mate = nullptr;
@@ -721,7 +725,7 @@ int match_mates(cmb_ctx* c, const uint8_t* infl_base, uint32_t n_rec, bool filte
   const uint32_t gr = (n_rec + 255) / 256;
   kd_pair_keys<<<gr, 256, 0, c->stream>>>(pa);
   kd_pair_order<<<(n_chunks + 255) / 256, 256, 0, c->stream>>>(pa);
-  kd_pair_order_fold<<<1, 1024, 0, c->stream>>>(d.d_pair_order, n_chunks, pa.flags);
+  kd_pair_order_fold<<<1, 1024, 0, c->stream>>>(d.d_pair_order, n_chunks, pa.flags, carry, largest);
   kd_pair_insert<<<gr, 256, 0, c->stream>>>(pa);
   kd_pair_resolve<<<(uint32_t)((table + 255) / 256), 256, 0, c->stream>>>(pa);
   CU_TRY(c, cudaGetLastError());
@@ -735,6 +739,8 @@ int match_mates(cmb_ctx* c, const uint8_t* infl_base, uint32_t n_rec, bool filte
   d.last_mate_inverse = !filter_out;
   return CMB_OK;
 }
+
+int reset_sample(cmb_ctx* c);
 
 }  // namespace
 
@@ -1003,6 +1009,18 @@ int cmb_begin_sample(cmb_ctx* c) {
   if (!c->ref.d_rows || !c->have_params) return fail(c, CMB_E_ARG, "cmb_begin_sample: set_reference and set_params first");
   if (c->in_sample) return fail(c, CMB_E_ARG, "cmb_begin_sample: previous sample not ended");
   CU_TRY(c, cudaSetDevice(c->device));
+  if (int rc = reset_sample(c)) return rc;
+  c->in_sample = true;
+  c->ended = false;
+  c->n_acquired = 0;
+  c->sh.active = false;
+  return CMB_OK;
+}
+}  // extern "C"
+
+namespace {
+// The device state of an empty sample: what cmb_begin_sample sets up, and what a declined cmb_submit_bgzf returns to
+int reset_sample(cmb_ctx* c) {
   c->timing = cmb_sample_timing{};
   c->k1_events_used = 0;
   c->block_minmax_used = 0;
@@ -1032,12 +1050,11 @@ int cmb_begin_sample(cmb_ctx* c) {
   // which overflow at once (cmb_grow_buffers path)
   if ((c->params.want & CMB_WANT_HIST_CSR) && c->n_local && small_hist())
     if (int rc = c->ref.d_pairs.ensure(c, 64)) return rc;
-  c->in_sample = true;
-  c->ended = false;
-  c->n_acquired = 0;
-  c->sh.active = false;
   return CMB_OK;
 }
+}  // namespace
+
+extern "C" {
 
 int cmb_acquire_batch(cmb_ctx* c, cmb_read_batch* batch) {
   if (!c || !batch) return fail(c, CMB_E_ARG, "cmb_acquire_batch: null argument");
@@ -1529,6 +1546,7 @@ struct BgzfCall {
   int declined();
   int chain();
   int extract();
+  int excl_n(uint32_t* n);
 };
 
 // The inflate kernels' arguments over blocks [b0, b1) of the call
@@ -1581,7 +1599,7 @@ int BgzfCall::prepare() {
   for (auto* b : {&d.d_clen, &d.d_isize, &d.d_status, &d.d_nrec, &d.d_ncig, &d.d_dirty})
     if ((rc = b->ensure(c, blocks_need, blocks_want))) return rc;
   if ((rc = d.d_t1_scratch.ensure(c, blocks_need * T1_LENS_BYTES, blocks_want * T1_LENS_BYTES))) return rc;
-  if ((rc = d.d_cnt.ensure(c, 16))) return rc;
+  if ((rc = d.d_cnt.ensure(c, 20))) return rc;  // [16..19]: a sliced decode's held-back counts (decode_sliced)
   if (!d.have_events) {
     for (auto& e : d.ev) CU_TRY(c, cudaEventCreate(&e));
     d.have_events = true;
@@ -1931,21 +1949,28 @@ int BgzfCall::extract() {
   }
   CU_TRY(c, cudaEventRecord(d.ev[4], c->stream));
   if (k1_active(c) && !decode_only) {
-    // records that start before excl_end_block are this rank's exclusive share of the stream (cmb_kept_tid_range)
-    uint32_t excl_n = 0xffffffffu;
-    if (in->ranged && in->excl_end_block < walk_end) {
-      if (in->excl_end_block <= first_block) excl_n = 0;
-      else {
-        uint64_t base = 0;
-        CU_TRY(c, cudaMemcpyAsync(&base, d.d_rec_base + in->excl_end_block, 8, cudaMemcpyDeviceToHost, c->stream));
-        CU_TRY(c, cudaStreamSynchronize(c->stream));
-        excl_n = (uint32_t)base;
-      }
-    }
-    d.last_excl_n = excl_n;
-    if ((rc = launch_k1(c, tb, (uint32_t)n_rec, (uint32_t)n_cig, excl_n, d.last_mate))) return rc;
+    uint32_t excl = 0;
+    if ((rc = excl_n(&excl))) return rc;
+    d.last_excl_n = excl;
+    if ((rc = launch_k1(c, tb, (uint32_t)n_rec, (uint32_t)n_cig, excl, d.last_mate))) return rc;
   }
   CU_TRY(c, cudaEventRecord(d.ev[5], c->stream));
+  return CMB_OK;
+}
+
+// K1's excl_n for the call's records: those that start before excl_end_block are this rank's exclusive share of the stream
+// (cmb_kept_tid_range) -- none when the block lies before the range, all when it lies after it
+int BgzfCall::excl_n(uint32_t* n) {
+  *n = 0xffffffffu;
+  if (in->ranged && in->excl_end_block < walk_end) {
+    if (in->excl_end_block <= first_block) *n = 0;
+    else {
+      uint64_t base = 0;
+      CU_TRY(c, cudaMemcpyAsync(&base, d.d_rec_base + in->excl_end_block, 8, cudaMemcpyDeviceToHost, c->stream));
+      CU_TRY(c, cudaStreamSynchronize(c->stream));
+      *n = (uint32_t)base;
+    }
+  }
   return CMB_OK;
 }
 
@@ -1972,14 +1997,15 @@ int submit_bgzf_impl(cmb_ctx* c, const cmb_bgzf_input* in, cmb_bgzf_result* out,
   return CMB_OK;
 }
 
+int decode_sliced(cmb_ctx* c, const cmb_bgzf_input* in, cmb_bgzf_result* out);
+
 int bgzf_entry(cmb_ctx* c, const cmb_bgzf_input* in, cmb_bgzf_result* out, bool decode_only) {
   if (c) {
     c->dec.last_valid = false;
     c->dec.filter_planned = false;
   }
   const auto t_call0 = std::chrono::steady_clock::now();
-  const int rc = submit_bgzf_impl(c, in, out, decode_only);
-  if (out) out->ms_host_wall = (float)std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_call0).count();
+  int rc = submit_bgzf_impl(c, in, out, decode_only);
   if (rc == CMB_E_NOMEM) {
     cudaGetLastError();
     auto& d = c->dec;  // give the big buffers back so that the rest of the sample has room
@@ -1987,14 +2013,17 @@ int bgzf_entry(cmb_ctx* c, const cmb_bgzf_input* in, cmb_bgzf_result* out, bool 
     d.d_inflated.release();
     d.d_tuple_slab.release();
     d.d_rec_off.release();
-    return fail(c, CMB_E_DECLINED, "cmb_submit_bgzf: not enough device memory for device-side decode");
+    // nothing was accumulated: the whole-stream call allocates every buffer before K1
+    rc = decode_only ? fail(c, CMB_E_DECLINED, "cmb_submit_bgzf: not enough device memory for device-side decode") : decode_sliced(c, in, out);
   }
+  if (out) out->ms_host_wall = (float)std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_call0).count();
   return rc;
 }
 }  // namespace
 
-// Device memory for the decode buffers (compressed file + inflated stream + tuples) is requested before anything is
-// accumulated, so running out of it simply declines the sample: the host decoder needs only the staging batches.
+// Device memory for the whole-stream decode buffers (compressed file + inflated stream + tuples) is requested before anything
+// is accumulated; when it runs out, the stream is decoded in block slices (decode_sliced), and a sample that declines there is
+// reset to its empty state first, so that the host decoder can take it over with only the staging batches.
 extern "C" int cmb_last_bgzf_batch(cmb_ctx* c, cmb_read_batch* dev_batch, uint32_t* n_records, uint32_t* n_intervals) {
   if (!c || !dev_batch || !n_records || !n_intervals) return fail(c, CMB_E_ARG, "cmb_last_bgzf_batch: null argument");
   if (!c->dec.last_valid || !c->dec.d_tuple_slab) return fail(c, CMB_E_ARG, "cmb_last_bgzf_batch: no device-decoded sample is resident");
@@ -2112,7 +2141,8 @@ constexpr int SLICE_HALVINGS = 8;                 // a slice whose buffers fail 
 constexpr uint64_t SLICE_MIN_BYTES = 64u << 20;   // budget floor: below it a failed allocation, not the estimate, shrinks a slice
 
 // CMB_DECODE_MEM_LIMIT_MB (testing aid): behave as if the device had this much room for the sharded sample -- its stores and
-// one slice's compressed and inflated bytes; a fraction of a megabyte slices small files.  0 when unset.
+// one slice's compressed and inflated bytes; a fraction of a megabyte slices small files -- or, for an ordinary sliced stream,
+// for the slices' decode buffers and the sample's event list (decode_sliced).  0 when unset.
 uint64_t shard_mem_limit() {
   const char* lim = getenv("CMB_DECODE_MEM_LIMIT_MB");
   return lim ? (uint64_t)(std::max(0.0, strtod(lim, nullptr)) * 1048576.0) : 0;
@@ -2215,8 +2245,96 @@ int store_grow(cmb_ctx* c, cmb_ctx::Shards::Store& st, uint64_t n_prim, uint64_t
   return CMB_OK;
 }
 
-// Shard k's slices (cmb_decode_bgzf's stages over a block range each): every slice's primaries appended to the store, AS
-// scratch and (shard 0) name hashes; `out` sums the slices' results
+// Statistics of one sliced decode
+struct SliceStats {
+  uint32_t n_slices = 0;
+  uint32_t halvings = 0;  // over the whole decode
+  uint64_t max_slice = 0;  // compressed + inflated bytes of the largest slice
+  float ms_inflate = 0, ms_chain = 0, ms_extract = 0;
+};
+constexpr int SLICE_HALVE = 1;  // a slice step's verdict: a buffer of the slice did not fit, halve it
+constexpr int SLICE_AGAIN = 2;  // a slice step's verdict: decode the same slice again (the step released the decode buffers)
+
+// The records of `in` (the whole stream, or its block range when ranged) in consecutive block slices, each a ranged
+// cmb_decode_bgzf call over blocks [b0, b1) that owns every record starting there.  A slice starts at the exact offset where
+// the previous slice's record walk stopped, or where its step cut it.  budget(at): the compressed and inflated bytes the slice
+// from `at` may take (slice_end).  A slice whose buffers fail to allocate, in the call or in its step, is halved up to
+// SLICE_HALVINGS times, after which nomem(blocks, b0, b1, tail) is the error; its tail starts at SLICE_TAIL_BYTES and doubles when a
+// record runs past it.  step(j, r, &next) does the caller's part with the slice's records and may lower `next` (the exit
+// offset): CMB_OK, SLICE_HALVE, SLICE_AGAIN or an error.  `out` sums the slices' results.
+template <class Budget, class Step, class Nomem>
+int decode_in_slices(cmb_ctx* c, const cmb_bgzf_input* in, cmb_bgzf_result* out, SliceStats& ss, Budget budget, Step step, Nomem nomem) {
+  auto& d = c->dec;
+  const uint32_t nb = in->n_blocks;
+  std::vector<uint64_t> ustart((size_t)nb + 1, 0);
+  for (uint32_t b = 0; b < nb; ++b) ustart[b + 1] = ustart[b] + in->block_isize[b];
+  const ShardBlocks blocks{nb, in->size, in->block_coffset, in->block_clen, ustart.data()};
+  const uint32_t walk_end = in->ranged ? std::min(in->walk_end_block, nb) : nb;
+  uint64_t at = in->records_at, tail = SLICE_TAIL_BYTES;
+  uint32_t halvings = 0;
+  uint32_t cap_end = nb;  // a slice end forced lower by a failed allocation (cleared once a slice decodes)
+  while (at < ustart[walk_end]) {
+    // ---- the slice: from the block holding `at`, as many blocks as the budget allows
+    const uint32_t b0 = (uint32_t)(std::upper_bound(ustart.begin(), ustart.end(), at) - ustart.begin()) - 1;
+    bool over = false;
+    const uint32_t b1 = std::min({slice_end(blocks, b0, budget(at), tail, &over), std::max(cap_end, b0 + 1), walk_end});
+    // ---- decode it: halved when its buffers do not fit, the tail doubled when a record runs past it
+    cmb_bgzf_input si = *in;
+    si.ranged = 1; si.records_at = at; si.walk_begin_block = b0; si.walk_end_block = b1;
+    if (!in->ranged) {
+      si.own_tid_begin = INT_MIN; si.own_tid_end = INT_MAX; si.own_unplaced = 1; si.excl_end_block = b1;
+    }
+    cmb_bgzf_result r{};
+    BgzfCall j{c, d, &si, &r, true, nb};
+    j.tail_bytes = tail;
+    int rc = j.prepare();
+    if (!rc && !j.nothing_to_decode && !(rc = j.copy_inflate()) && !(rc = j.declined()) && !(rc = j.chain())) rc = j.extract();
+    if (rc == CMB_E_NOMEM) rc = SLICE_HALVE;
+    uint64_t next = j.exit_off;
+    if (!rc && !j.nothing_to_decode) {
+      CU_TRY(c, cudaEventSynchronize(d.ev[4]));
+      cudaEventElapsedTime(&r.ms_total, d.ev[0], d.ev[4]);
+      cudaEventElapsedTime(&r.ms_copy_inflate, d.ev[0], d.ev[2]);
+      cudaEventElapsedTime(&r.ms_chain, d.ev[2], d.ev[3]);
+      cudaEventElapsedTime(&r.ms_extract, d.ev[3], d.ev[4]);
+      if (!j.n_rec || j.exit_off <= at) return fail(c, CMB_E_DECLINED, "the slice from block %u decoded no record", b0);
+      rc = step(j, r, &next);
+    }
+    if (rc == SLICE_HALVE) {
+      release_decode(c);
+      if (b1 - b0 > 1 && halvings < SLICE_HALVINGS) {
+        ++halvings;
+        ++ss.halvings;
+        cap_end = b0 + (b1 - b0) / 2;
+        continue;
+      }
+      return nomem(blocks, b0, b1, tail);
+    }
+    if (rc == CMB_E_DECLINED && j.tail_short) {
+      tail *= 2;
+      continue;
+    }
+    if (rc == SLICE_AGAIN) continue;
+    if (rc) return rc;
+    if (j.nothing_to_decode) break;
+    // ---- the slice's result into the call's
+    out->n_records += r.n_records; out->n_primary += r.n_primary; out->n_intervals += r.n_intervals;
+    out->n_blocks_host += r.n_blocks_host; out->chain_repairs += r.chain_repairs; out->n_launches += r.n_launches;
+    out->n_blocks_second_pass += r.n_blocks_second_pass; out->h2d_bytes += r.h2d_bytes;
+    out->ms_copy_enqueue_wall += r.ms_copy_enqueue_wall; out->ms_total += r.ms_total;
+    ss.ms_inflate += r.ms_copy_inflate; ss.ms_chain += r.ms_chain; ss.ms_extract += r.ms_extract;
+    ss.max_slice = std::max(ss.max_slice, (j.byte_hi - j.byte_lo) + (j.total - j.u_lo));
+    ++ss.n_slices;
+    at = next;
+    cap_end = nb;
+    halvings = 0;
+  }
+  c->dec.last_valid = false;  // the tuples are a slice's, not the stream's: cmb_last_bgzf_batch must not hand them out
+  return CMB_OK;
+}
+
+// Shard k's slices: every slice's primaries appended to the store, AS scratch and (shard 0) name hashes; `out` sums the
+// slices' results
 int decode_shard(cmb_ctx* c, const cmb_bgzf_input* in, cmb_bgzf_result* out, uint32_t k) {
   auto& s = c->sh;
   auto& d = c->dec;
@@ -2227,21 +2345,14 @@ int decode_shard(cmb_ctx* c, const cmb_bgzf_input* in, cmb_bgzf_result* out, uin
   st.n_prim = st.n_iv = 0;
   if (in->n_blocks == 0 || in->ranged) return fail(c, CMB_E_ARG, "cmb_shard_add: shard %u: a whole BGZF file is needed", k);
   const uint32_t nb = in->n_blocks;
-  std::vector<uint64_t> ustart((size_t)nb + 1, 0);
-  for (uint32_t b = 0; b < nb; ++b) ustart[b + 1] = ustart[b] + in->block_isize[b];
-  const ShardBlocks blocks{nb, in->size, in->block_coffset, in->block_clen, ustart.data()};
+  uint64_t stream_total = 0;
+  for (uint32_t b = 0; b < nb; ++b) stream_total += in->block_isize[b];
   const uint64_t lim = shard_mem_limit();
   // shards after this context's first are expected to be sized like it (on one GPU: like shard 0)
   const bool later = k > s.first;
   const uint64_t n0 = later ? s.store[s.first].n_prim : 0, iv0 = later ? s.store[s.first].n_iv : 0;
-  uint64_t at = in->records_at, tail = SLICE_TAIL_BYTES, max_slice = 0;
-  uint32_t n_slices = 0;
-  float ms_inflate = 0, ms_chain = 0, ms_extract = 0, ms_grow = 0;
-  int halvings = 0;
-  uint32_t cap_end = nb;  // a slice end forced lower by a failed allocation (cleared once a slice decodes)
-  while (at < ustart[nb]) {
-    // ---- the slice: from the block holding `at`, as many blocks as the budget allows
-    const uint32_t b0 = (uint32_t)(std::upper_bound(ustart.begin(), ustart.end(), at) - ustart.begin()) - 1;
+  float ms_grow = 0;
+  auto budget = [&](uint64_t at) -> uint64_t {
     const uint64_t need_now = shard_need(c, k, st.n_prim, st.n_iv);
     // What the sample is still expected to need: this shard's rest, the later shards' stores like shard 0's, and the sorted
     // winners (at most one record per primary of a shard, 60 B each with an interval slot).  Shard 0's first slice has no
@@ -2251,59 +2362,20 @@ int decode_shard(cmb_ctx* c, const cmb_bgzf_input* in, cmb_bgzf_result* out, uin
       expect = 37 * (n0 > st.n_prim ? n0 - st.n_prim : 0) + 8 * (iv0 > st.n_iv ? iv0 - st.n_iv : 0) + (s.last - 1 - k) * (37 * n0 + 8 * iv0) +
                60 * n0;
     } else if (at > in->records_at) {  // the first shard: scaled by the inflated bytes its slices so far held
-      const double scale = (double)(ustart[nb] - in->records_at) / (double)(at - in->records_at);
+      const double scale = (double)(stream_total - in->records_at) / (double)(at - in->records_at);
       const double total = need_now * scale, store = (37.0 * st.n_prim + 8.0 * st.n_iv) * scale, winners = 60.0 * st.n_prim * scale;
       expect = (uint64_t)(total - need_now + store * (s.last - 1 - k) + winners);
     }
     const uint64_t room = shard_room(c), held = need_now + expect;
-    uint64_t budget = room > held ? room - held : 0;
-    budget = std::max(budget, lim ? lim / 64 : SLICE_MIN_BYTES);
-    bool over = false;
-    uint32_t b1 = std::min(slice_end(blocks, b0, budget, tail, &over), std::max(cap_end, b0 + 1));
-    // ---- decode it: halved when its buffers do not fit, the tail doubled when a record runs past it
-    cmb_bgzf_input si = *in;
-    si.ranged = 1; si.records_at = at; si.walk_begin_block = b0; si.walk_end_block = b1;
-    si.own_tid_begin = INT_MIN; si.own_tid_end = INT_MAX; si.own_unplaced = 1; si.excl_end_block = b1;
-    cmb_bgzf_result r{};
-    BgzfCall j{c, d, &si, &r, true, nb};
-    j.tail_bytes = tail;
-    int rc = j.prepare();
-    if (!rc && !j.nothing_to_decode && !(rc = j.copy_inflate()) && !(rc = j.declined()) && !(rc = j.chain())) rc = j.extract();
-    if (rc == CMB_E_NOMEM) {
-      release_decode(c);
-      if (b1 - b0 > 1 && halvings < SLICE_HALVINGS) {
-        ++halvings;
-        cap_end = b0 + (b1 - b0) / 2;
-        continue;
-      }
-      return fail(c, CMB_E_NOMEM, "shard %u: not enough device memory to decode blocks %u..%u (%llu bytes); the sharded sample holds %llu bytes", k, b0, b1,
-                  (unsigned long long)slice_bytes(blocks, b0, b1, tail), (unsigned long long)need_now);
-    }
-    if (rc == CMB_E_DECLINED && j.tail_short) {
-      tail *= 2;
-      continue;
-    }
-    if (rc == CMB_E_DECLINED) return fail(c, CMB_E_DECLINED, "shard %u: the device decoder declined it (%s); sharded input is decoded on the device only", k, c->err.c_str());
-    if (rc) return rc;
-    if (j.nothing_to_decode) break;
-    CU_TRY(c, cudaEventSynchronize(d.ev[4]));
-    cudaEventElapsedTime(&r.ms_total, d.ev[0], d.ev[4]);
-    cudaEventElapsedTime(&r.ms_copy_inflate, d.ev[0], d.ev[2]);
-    cudaEventElapsedTime(&r.ms_chain, d.ev[2], d.ev[3]);
-    cudaEventElapsedTime(&r.ms_extract, d.ev[3], d.ev[4]);
+    const uint64_t budget = room > held ? room - held : 0;
+    return std::max(budget, lim ? lim / 64 : SLICE_MIN_BYTES);
+  };
+  auto step = [&](BgzfCall& j, cmb_bgzf_result&, uint64_t*) -> int {
     const uint64_t n_rec = j.n_rec;
-    if (!n_rec || j.exit_off <= at) return fail(c, CMB_E_DECLINED, "shard %u: the slice from block %u decoded no record", k, b0);
     // ---- which records are primaries, and where their tuples and intervals go
     CU_TRY(c, cudaEventRecord(s.ev[0], c->stream));
-    if ((rc = s.d_scan.ensure(c, n_rec + 1, with_slack(n_rec + 1))) == CMB_E_NOMEM) {  // part of the slice: halve it like its other buffers
-      release_decode(c);
-      if (b1 - b0 > 1 && halvings < SLICE_HALVINGS) {
-        ++halvings;
-        cap_end = b0 + (b1 - b0) / 2;
-        continue;
-      }
-      return fail(c, CMB_E_NOMEM, "shard %u: not enough device memory to scan the records of blocks %u..%u", k, b0, b1);
-    }
+    int rc = s.d_scan.ensure(c, n_rec + 1, with_slack(n_rec + 1));
+    if (rc == CMB_E_NOMEM) return SLICE_HALVE;  // part of the slice: halve it like its other buffers
     if (rc) return rc;
     ShardScanArgs a{};
     a.data = d.last_infl_base; a.rec_off = d.d_rec_off; a.n_records = n_rec; a.scan = s.d_scan;
@@ -2320,7 +2392,7 @@ int decode_shard(cmb_ctx* c, const cmb_bgzf_input* in, cmb_bgzf_result* out, uin
     // ---- room for them in the store, the AS scratch and (shard 0) the name hashes; without the decode buffers the slice is
     // decoded again
     // The expected totals: shard 0's, for shard k > 0; for shard 0, its slices so far scaled by the inflated bytes they cover
-    const double scale = (double)(ustart[nb] - in->records_at) / (double)(j.exit_off - in->records_at);
+    const double scale = (double)(stream_total - in->records_at) / (double)(j.exit_off - in->records_at);
     const uint64_t hint_prim = later ? n0 : (uint64_t)(n_prim * scale), hint_iv = later ? iv0 : (uint64_t)(n_iv * scale);
     bool released = false;
     const auto g0 = std::chrono::steady_clock::now();
@@ -2337,7 +2409,7 @@ int decode_shard(cmb_ctx* c, const cmb_bgzf_input* in, cmb_bgzf_result* out, uin
     };
     if ((rc = shard_alloc(c, shard_need(c, k, n_prim, n_iv), grow))) return rc;
     ms_grow += std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - g0).count();
-    if (released) continue;
+    if (released) return SLICE_AGAIN;
     a.st = st.view; a.prim_base = st.n_prim; a.iv_base = (uint32_t)st.n_iv;
     a.as_val = s.group ? st.as_val.p : s.d_as_val.p; a.as_state = s.group ? st.as_state.p : s.d_as_state.p; a.hash0 = s.d_hash0; a.n0 = k ? s.store[0].n_prim : 0;
     if (k && s.group) a.names = st.names;
@@ -2350,22 +2422,135 @@ int decode_shard(cmb_ctx* c, const cmb_bgzf_input* in, cmb_bgzf_result* out, uin
     s.ms_choose += ms;
     st.n_prim = n_prim;
     st.n_iv = n_iv;
-    // ---- the slice's result into the shard's
-    out->n_records += r.n_records; out->n_primary += r.n_primary; out->n_intervals += r.n_intervals;
-    out->n_blocks_host += r.n_blocks_host; out->chain_repairs += r.chain_repairs; out->n_launches += r.n_launches;
-    out->n_blocks_second_pass += r.n_blocks_second_pass; out->h2d_bytes += r.h2d_bytes;
-    out->ms_copy_enqueue_wall += r.ms_copy_enqueue_wall; out->ms_total += r.ms_total;
-    ms_inflate += r.ms_copy_inflate; ms_chain += r.ms_chain; ms_extract += r.ms_extract;
-    max_slice = std::max(max_slice, (j.byte_hi - j.byte_lo) + (j.total - j.u_lo));
-    ++n_slices;
-    at = j.exit_off;
-    cap_end = nb;
-    halvings = 0;
-  }
+    return CMB_OK;
+  };
+  auto nomem = [&](const ShardBlocks& blocks, uint32_t b0, uint32_t b1, uint64_t tail) {
+    return fail(c, CMB_E_NOMEM, "shard %u: not enough device memory to decode blocks %u..%u (%llu bytes); the sharded sample holds %llu bytes", k, b0, b1,
+                (unsigned long long)slice_bytes(blocks, b0, b1, tail), (unsigned long long)shard_need(c, k, st.n_prim, st.n_iv));
+  };
+  SliceStats ss;
+  const int rc = decode_in_slices(c, in, out, ss, budget, step, nomem);
+  if (rc == CMB_E_DECLINED) return fail(c, CMB_E_DECLINED, "shard %u: the device decoder declined it (%s); sharded input is decoded on the device only", k, c->err.c_str());
+  if (rc) return rc;
   if (getenv("CMB_PIPELINE_STATS"))
     fprintf(stderr, "#shard_slices\tshard=%u\tslices=%u\tmax_slice_bytes=%llu\tcopy_inflate_ms=%.1f\tchain_ms=%.1f\textract_ms=%.1f\tgrow_ms=%.1f\n", k,
-            n_slices, (unsigned long long)max_slice, ms_inflate, ms_chain, ms_extract, ms_grow);
-  c->dec.last_valid = false;  // the tuples are a slice's, not a sample's: cmb_last_bgzf_batch must not hand them out
+            ss.n_slices, (unsigned long long)ss.max_slice, ss.ms_inflate, ss.ms_chain, ss.ms_extract, ms_grow);
+  return CMB_OK;
+}
+
+// cmb_submit_bgzf when the whole-stream buffers do not fit: the stream (a rank's block range in a group) in block slices, each
+// submitted to K1 as one batch at the sample's running interval base -- in pair mode after its mates are matched, and only
+// up to its cut (cmb_decode_slices.hpp).  A decline leaves the sample as cmb_begin_sample left it, for the host decoder.
+int decode_sliced(cmb_ctx* c, const cmb_bgzf_input* in, cmb_bgzf_result* out) {
+  auto& d = c->dec;
+  *out = cmb_bgzf_result{};
+  auto decline = [&](int rc) {
+    cudaGetLastError();
+    release_decode(c);
+    if (int e = reset_sample(c)) return e;
+    return rc;
+  };
+  // Room for the decode buffers and the sample's event list: the limit under CMB_DECODE_MEM_LIMIT_MB, else free memory plus
+  // the decode buffers held
+  auto room = [&]() -> uint64_t {
+    if (const uint64_t lim = shard_mem_limit()) return lim;
+    size_t free_b = 0, total_b = 0;
+    cudaMemGetInfo(&free_b, &total_b);
+    cudaGetLastError();
+    return free_b + decode_bytes(c);
+  };
+  if (room() < SLICE_MIN_BYTES) return decline(fail(c, CMB_E_DECLINED, "cmb_submit_bgzf: not enough device memory for device-side decode"));
+  uint64_t stream_end = 0;  // end of the inflated bytes whose records are walked
+  const uint32_t walk_end = in->ranged ? std::min(in->walk_end_block, in->n_blocks) : in->n_blocks;
+  for (uint32_t b = 0; b < walk_end; ++b) stream_end += in->block_isize[b];
+  const uint64_t iv0 = c->n_intervals;
+  double side = 0;       // the last slice's other buffers per compressed + inflated byte
+  uint32_t carry = 0;    // pair mode: the largest eligible tid of the slices so far
+  uint64_t cut_records = 0;
+  auto budget = [&](uint64_t at) -> uint64_t {
+    const uint64_t done = at > in->records_at ? at - in->records_at : 0;
+    const uint64_t total = stream_end > in->records_at ? stream_end - in->records_at : 0;
+    return decode_slice_budget(room(), !c->gene_mode, c->d_events.bytes(), done, total, c->n_intervals - iv0, side);
+  };
+  auto step = [&](BgzfCall& j, cmb_bgzf_result& r, uint64_t* next) -> int {
+    const uint32_t n = (uint32_t)j.n_rec;
+    uint32_t n_sub = n, iv_sub = (uint32_t)j.n_cig;
+    cmb_read_batch tb;
+    carve_batch(d.d_tuple_slab, n, (uint32_t)j.n_cig, &tb);
+    const int32_t* mate = nullptr;
+    uint32_t largest = carry;
+    int rc;
+    if (c->mode.filter_pairs) {
+      // words 12..14 of d_cnt: the slice's largest eligible tid, then the cut's `after` and n - cut (zeroed by copy_inflate)
+      uint32_t* w = d.d_cnt + 12;
+      rc = match_mates(c, d.last_infl_base, n, true, "cmb_submit_bgzf", carry, w);
+      if (rc == CMB_E_NOMEM) return SLICE_HALVE;
+      if (rc) return rc;
+      r.n_launches += 5;
+      if (j.walk_end < walk_end) {  // not the last slice: hold the trailing run of its last eligible tid back for the next one
+        const uint32_t g = (n + 255) / 256;
+        kd_pair_cut_after<<<g, 256, 0, c->stream>>>(d.d_pair_key, tb.tid, n, w, w + 1);
+        kd_pair_cut_at<<<g, 256, 0, c->stream>>>(d.d_pair_key, tb.tid, n, w, w + 1, w + 2);
+        CU_TRY(c, cudaGetLastError());
+        r.n_launches += 2;
+      }
+      uint32_t h[3] = {0, 0, 0};
+      CU_TRY(c, cudaMemcpyAsync(h, w, 12, cudaMemcpyDeviceToHost, c->stream));
+      CU_TRY(c, cudaStreamSynchronize(c->stream));
+      largest = h[0];
+      const uint32_t cut = n - h[2];
+      if (cut == 0)
+        return fail(c, CMB_E_DECLINED, "cmb_submit_bgzf: the proper-pair records of reference %d do not fit in one decode slice; mates are "
+                    "matched on the host", (int32_t)largest);
+      if (cut < n) {  // the next slice starts at record `cut`; its records leave this slice's counters
+        uint64_t off = 0;
+        CU_TRY(c, cudaMemcpyAsync(&off, d.d_rec_off + cut, 8, cudaMemcpyDeviceToHost, c->stream));
+        CU_TRY(c, cudaMemcpyAsync(&iv_sub, tb.iv_begin + cut, 4, cudaMemcpyDeviceToHost, c->stream));
+        CU_TRY(c, cudaMemsetAsync(d.d_cnt + 16, 0, 16, c->stream));
+        kd_count_held<<<(n - cut + 255) / 256, 256, 0, c->stream>>>(tb.tid, tb.flag, cut, n, j.in->own_tid_begin, j.in->own_tid_end, j.in->own_unplaced,
+                                                                   (unsigned long long*)(d.d_cnt + 16), (unsigned long long*)(d.d_cnt + 18));
+        CU_TRY(c, cudaGetLastError());
+        uint64_t held[2] = {0, 0};
+        CU_TRY(c, cudaMemcpyAsync(held, d.d_cnt + 16, 16, cudaMemcpyDeviceToHost, c->stream));
+        CU_TRY(c, cudaStreamSynchronize(c->stream));
+        r.n_primary -= held[0];
+        r.n_records -= held[1];
+        r.n_intervals = iv_sub;
+        r.n_launches += 1;
+        *next = off;
+        n_sub = cut;
+        cut_records += n - cut;
+      }
+      mate = d.d_pair_mate;
+    }
+    if (k1_active(c)) {
+      uint32_t excl = 0;
+      if ((rc = j.excl_n(&excl))) return rc;
+      rc = launch_k1(c, tb, n_sub, iv_sub, excl, mate);
+      if (rc == CMB_E_NOMEM) return SLICE_HALVE;  // the event list did not grow: nothing of the slice was accumulated
+      if (rc) return rc;
+    }
+    carry = largest;
+    uint64_t other = d.d_tuple_slab.bytes() + d.d_rec_off.bytes();
+    if (c->mode.filter_pairs)
+      other += d.d_pair_key.bytes() + d.d_pair_mate.bytes() + d.d_pair_next.bytes() + d.d_pair_tag.bytes() + d.d_pair_head.bytes();
+    side = (double)other / (double)std::max<uint64_t>(1, (j.byte_hi - j.byte_lo) + (j.total - j.u_lo));
+    return CMB_OK;
+  };
+  auto nomem = [&](const ShardBlocks&, uint32_t, uint32_t, uint64_t) {
+    return fail(c, CMB_E_DECLINED, "cmb_submit_bgzf: not enough device memory for device-side decode");
+  };
+  SliceStats ss;
+  const int rc = decode_in_slices(c, in, out, ss, budget, step, nomem);
+  if (rc == CMB_E_DECLINED) return decline(rc);
+  if (rc) return rc;
+  release_decode(c);  // the end of the sample needs the room; a sliced sample has no resident tuples to hand out
+  out->ms_copy_inflate = ss.ms_inflate;
+  out->ms_chain = ss.ms_chain;
+  out->ms_extract = ss.ms_extract;
+  if (getenv("CMB_PIPELINE_STATS"))
+    fprintf(stderr, "#decode_slices\tslices=%u\tmax_slice_bytes=%llu\thalvings=%u\tpair_cut_records=%llu\n", ss.n_slices,
+            (unsigned long long)ss.max_slice, ss.halvings, (unsigned long long)cut_records);
   return CMB_OK;
 }
 

@@ -26,6 +26,7 @@
 // eligible tids are non-decreasing), so the sortedness check (contig.rs:129-132) over the kept records in file order fails
 // exactly when it fails over the emitted stream.
 #pragma once
+#include "cmb_decode_slices.hpp"
 
 struct PairArgs {
   const uint8_t* data;       // inflated stream
@@ -98,25 +99,29 @@ __global__ void __launch_bounds__(256) kd_pair_order(const PairArgs a) {
   if (down) atomicOr(a.flags, DEC_ERR_PAIR_ORDER);
 }
 
-// Across chunks (one CTA): chunk c's first eligible tid must be >= the last eligible tid of every chunk before it.
-__global__ void __launch_bounds__(1024) kd_pair_order_fold(const uint2* order, uint32_t n_chunks, uint32_t* flags) {
+// Across chunks (one CTA): chunk c's first eligible tid must be >= the last eligible tid of every chunk before it and >= `carry`,
+// the largest eligible tid of the earlier slices of a sliced decode (0: none).  `largest` (when given) receives the largest
+// eligible tid so far, carry included: the next slice's carry.
+__global__ void __launch_bounds__(1024) kd_pair_order_fold(const uint2* order, uint32_t n_chunks, uint32_t* flags, uint32_t carry,
+                                                           uint32_t* largest) {
   __shared__ uint32_t s_max[1024];
   const uint32_t t = threadIdx.x;
   const uint32_t per = (n_chunks + 1023) / 1024;
   const uint32_t c0 = min(n_chunks, t * per), c1 = min(n_chunks, c0 + per);
-  uint32_t lmax = 0;
+  uint32_t lmax = carry;
   bool bad = false;
   for (uint32_t c = c0; c < c1; ++c) {
     const uint2 r = order[c];
-    bad = bad || r.x < lmax;
+    bad = bad || pair_order_drop(r.x, lmax);
     lmax = max(lmax, r.y);
   }
   s_max[t] = lmax;
   __syncthreads();
-  uint32_t before = 0;
+  uint32_t before = carry;
   for (uint32_t k = 0; k < t; ++k) before = max(before, s_max[k]);
-  for (uint32_t c = c0; c < c1 && !bad; ++c) bad = order[c].x < before;
+  for (uint32_t c = c0; c < c1 && !bad; ++c) bad = pair_order_drop(order[c].x, before);
   if (bad) atomicOr(flags, DEC_ERR_PAIR_ORDER);
+  if (largest && t == 1023) *largest = max(before, lmax);
 }
 
 __global__ void __launch_bounds__(256) kd_pair_insert(const PairArgs a) {
@@ -191,3 +196,22 @@ __global__ void __launch_bounds__(256) kd_pair_resolve(const PairArgs a) {
     }
   }
 }
+
+#ifdef __CUDACC__
+// The pair-mode cut of a slice (cmb_decode_slices.hpp) over its n records, `last` = its largest eligible tid
+// (kd_pair_order_fold): *after = max of pair_cut_after, then *cut_back = n - min of pair_cut_at (0: no record is held back).
+__global__ void __launch_bounds__(256) kd_pair_cut_after(const uint64_t* key, const int32_t* tid, uint32_t n, const uint32_t* last,
+                                                         uint32_t* after) {
+  const uint32_t i = blockIdx.x * 256 + threadIdx.x;
+  if (i >= n) return;
+  const uint32_t v = pair_cut_after(key[i] != 0, (uint32_t)tid[i], *last, i);
+  if (v) atomicMax(after, v);
+}
+__global__ void __launch_bounds__(256) kd_pair_cut_at(const uint64_t* key, const int32_t* tid, uint32_t n, const uint32_t* last,
+                                                      const uint32_t* after, uint32_t* cut_back) {
+  const uint32_t i = blockIdx.x * 256 + threadIdx.x;
+  if (i >= n) return;
+  const uint32_t v = pair_cut_at(key[i] != 0, (uint32_t)tid[i], *last, *after, i, n);
+  if (v < n) atomicMax(cut_back, n - v);
+}
+#endif

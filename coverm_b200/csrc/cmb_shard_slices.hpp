@@ -1,4 +1,5 @@
-// Sharded input: the block slices a shard is decoded in (cmb_shard_add).  Host-only, so that tests can check the plan natively.
+// The block slices a sliced device decode walks: a shard of sharded input (cmb_shard_add), or an ordinary stream whose whole
+// decode does not fit (cmb_submit_bgzf).  Host-only, so that tests can check the plan natively.
 //
 // A slice decodes the records that START in blocks [b0, b1).  Its device footprint is what a ranged decode uploads and inflates:
 // the compressed bytes of blocks [b0, data_end) and their inflated bytes, where data_end extends b1 by the following blocks that
@@ -44,7 +45,7 @@ inline uint32_t slice_end(const ShardBlocks& f, uint32_t b0, uint64_t budget, ui
 }
 
 // The slices of blocks [first, nb) under a fixed budget, in order; *n_over counts the slices of one block that exceed it.  For
-// tests only: the device loop (decode_shard) calls slice_end itself, with a budget recomputed before every slice, each slice
+// tests only: the device loop (decode_in_slices) calls slice_end itself, with a budget recomputed before every slice, each slice
 // starting at the block that holds the previous slice's exit offset (past the planned end when a record spans whole blocks),
 // its end lowered when its buffers fail to allocate and its tail doubled for a long record.
 inline std::vector<std::pair<uint32_t, uint32_t>> plan_slices(const ShardBlocks& f, uint32_t first, uint64_t budget, uint64_t tail,

@@ -51,8 +51,10 @@ extern "C" {
 #define CMB_E_NM (-5)        /* NM aux missing / wrong type where the reference calls nm()  (lib.rs:138-158 panic) */
 #define CMB_E_BOUNDS (-6)    /* an aligned block starts at/after the contig end (contig.rs:178 index panic) */
 #define CMB_E_CAPACITY (-7)  /* a device-side buffer (histogram bin pool or pairs) overflowed */
-#define CMB_E_DECLINED (-8)  /* cmb_submit_bgzf: the device decoder cannot vouch for this stream; nothing was
-                                accumulated -- decode on the host instead                    */
+#define CMB_E_DECLINED (-8)  /* cmb_submit_bgzf: the device decoder cannot vouch for this stream; the sample is
+                                reset to the state cmb_begin_sample left it in (also when a
+                                late slice of a sliced decode declines) -- decode on the host
+                                instead                                                      */
 
 typedef struct cmb_ctx cmb_ctx;
 
@@ -246,9 +248,10 @@ int cmb_end_sample_device(cmb_ctx* ctx, const cmb_contig_stats** dev_stats);
  * inflates the blocks, finds the record boundaries, extracts the tuples and runs the same filter/delta kernel.
  * Call it between cmb_begin_sample and cmb_end_sample INSTEAD of the acquire/submit loop, and only when
  * cmb_filter_mode.filter_pairs == 0 (mate matching needs read names, which never reach the device).
- * Returns CMB_E_DECLINED -- with nothing accumulated -- when the device path cannot vouch for the stream (malformed
- * deflate data, an inconsistent record chain, an unknown aux type ...): the caller then decodes on the host, which
- * raises the reference's error if there is one.  `data` may be pageable (staged through pinned buffers by
+ * A stream whose whole decode does not fit in device memory is decoded in block slices, each submitted as one batch.
+ * Returns CMB_E_DECLINED -- with the sample reset to its empty state -- when the device path cannot vouch for the stream
+ * (malformed deflate data, an inconsistent record chain, an unknown aux type, too little device memory even for slices
+ * ...): the caller then decodes on the host, which raises the reference's error if there is one.  `data` may be pageable (staged through pinned buffers by
  * `copy_threads` host threads) or pinned / registered memory (copied directly). */
 typedef struct cmb_bgzf_input {
   const uint8_t* data;            /* host pointer: the whole BAM file                                  */
