@@ -71,6 +71,17 @@ __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commi
 template <int N>
 __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
 
+// Little-endian loads of BAM fields at any byte offset
+__device__ __forceinline__ uint32_t ldu32(const uint8_t* p) {
+  const uintptr_t a = (uintptr_t)p;
+  const uint32_t* q = (const uint32_t*)(a & ~(uintptr_t)3);
+  const uint32_t sh = (uint32_t)(a & 3) * 8;
+  const uint32_t lo = q[0];
+  if (sh == 0) return lo;
+  return __funnelshift_r(lo, q[1], sh);
+}
+__device__ __forceinline__ uint32_t ldu16(const uint8_t* p) { return (uint32_t)p[0] | ((uint32_t)p[1] << 8); }
+
 __device__ __forceinline__ uint64_t warp_sum_u64(uint64_t v) {
 #pragma unroll
   for (int d = 16; d > 0; d >>= 1) v += __shfl_xor_sync(FULL, v, d);

@@ -466,16 +466,6 @@ constexpr uint64_t WALK_UNKNOWN = ~0ull;      // no guess / no valid exit
 constexpr uint32_t GUESS_SCAN_LIMIT = 1u << 20;  // bytes scanned for a first record boundary
 constexpr uint32_t DEC_ERR_CHAIN = 1u, DEC_ERR_RECORD = 2u, DEC_ERR_AUX = 4u;
 
-__device__ __forceinline__ uint32_t ldu32(const uint8_t* p) {
-  const uintptr_t a = (uintptr_t)p;
-  const uint32_t* q = (const uint32_t*)(a & ~(uintptr_t)3);
-  const uint32_t sh = (uint32_t)(a & 3) * 8;
-  const uint32_t lo = q[0];
-  if (sh == 0) return lo;
-  return __funnelshift_r(lo, q[1], sh);
-}
-__device__ __forceinline__ uint32_t ldu16(const uint8_t* p) { return (uint32_t)p[0] | ((uint32_t)p[1] << 8); }
-
 struct WalkArgs {
   const uint8_t* data;   // inflated stream (>= 8 readable bytes after `total`)
   uint64_t total;
@@ -788,7 +778,7 @@ __global__ void __launch_bounds__(256) kd_extract(const ExtractArgs a) {
   if (err && (threadIdx.x & 31) == 0) atomicOr(a.flags, err);
 }
 
-// A pair-mode slice of a sliced decode holds records [i0, n) back for the next slice (cmb_decode_slices.hpp): their share of
+// A pair-mode slice of a sliced decode holds records [i0, n) back for the next slice (cmb_slices.hpp): their share of
 // kd_extract's n_primary and n_owned, which the slice's result gives back (same ownership rule as kd_extract)
 __global__ void __launch_bounds__(256) kd_count_held(const int32_t* tid, const uint16_t* flag, uint32_t i0, uint32_t n, int32_t own_lo,
                                                      int32_t own_hi, uint32_t own_unplaced, unsigned long long* n_primary,

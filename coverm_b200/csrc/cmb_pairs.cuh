@@ -26,7 +26,7 @@
 // eligible tids are non-decreasing), so the sortedness check (contig.rs:129-132) over the kept records in file order fails
 // exactly when it fails over the emitted stream.
 #pragma once
-#include "cmb_decode_slices.hpp"
+#include "cmb_slices.hpp"
 
 struct PairArgs {
   const uint8_t* data;       // inflated stream
@@ -198,7 +198,7 @@ __global__ void __launch_bounds__(256) kd_pair_resolve(const PairArgs a) {
 }
 
 #ifdef __CUDACC__
-// The pair-mode cut of a slice (cmb_decode_slices.hpp) over its n records, `last` = its largest eligible tid
+// The pair-mode cut of a slice (cmb_slices.hpp) over its n records, `last` = its largest eligible tid
 // (kd_pair_order_fold): *after = max of pair_cut_after, then *cut_back = n - min of pair_cut_at (0: no record is held back).
 __global__ void __launch_bounds__(256) kd_pair_cut_after(const uint64_t* key, const int32_t* tid, uint32_t n, const uint32_t* last,
                                                          uint32_t* after) {

@@ -1,6 +1,6 @@
 // Sharded input (ReadSortedShardedBamReader, src/shard_bam_reader.rs): the per-record scan of one shard's decoded stream, the
-// per-pair choice of the best shard, and the counting sort of the winners by tid.  Included from cmb_device.cu after
-// cmb_decode.cuh (ldu32 / ldu16).
+// per-pair choice of the best shard, and the counting sort of the winners by tid.  Included from cmb_shard_input.cu; the plain
+// structs the context stores (ShardStore, PairState) are in cmb_context.cuh.
 //
 // Errors are not traps: each kernel folds what it finds into one 64-bit key with atomicMin, ordered like the reference's serial
 // loop meets them -- the primary-set index first (the reference reads set s of every shard, then decides pair s/2 after its second
@@ -21,10 +21,6 @@ __device__ __forceinline__ unsigned long long sh_key(uint64_t set, uint32_t phas
 // info byte of a stored primary: bits 0-1 NM tag (0 absent, 1 type C, 2 another type), bit 2 n_cigar > 0
 constexpr uint8_t SHI_NM_MASK = 3, SHI_HAS_CIGAR = 4;
 // AS state of a stored primary (aux_as, lib.rs:160-178): 0 absent, 1 type C or S, else the tag's type character
-struct ShardStore {
-  cmb_read_batch b;  // device pointers; tids already shifted into the concatenated layout
-  uint8_t* info;
-};
 
 // One block slice of a shard (cmb_shard_add): its records are scanned and their primaries appended to the shard's store at
 // prim_base / iv_base, so that every index below (the store's, hash0's, the error keys') counts from the shard's first record.
@@ -137,14 +133,6 @@ __global__ void __launch_bounds__(256) ks_compact(const ShardScanArgs a) {
   else if (a.names) a.names[j] = h;
   else if (j < a.n0 && a.hash0[j] != h) atomicMin(a.err, sh_key(j, a.shard, SHE_NAME, 0));
 }
-
-// Running choice of every pair (shard_bam_reader.rs:210-262).  best = highest score so far, winner = its shard, ties = how many
-// candidates share it.
-struct PairState {
-  long long best;
-  uint32_t winner;
-  uint32_t ties;
-};
 
 struct ShardPairArgs {
   ShardStore st;

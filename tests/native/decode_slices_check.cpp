@@ -1,4 +1,4 @@
-// The ordinary sliced decode's rules (coverm_b200/csrc/cmb_decode_slices.hpp) compiled as plain C++.
+// The ordinary sliced decode's rules (coverm_b200/csrc/cmb_slices.hpp) compiled as plain C++.
 //
 // Pair cut: random tid / eligibility streams, sorted and unsorted, walked in slices of random record counts the way
 // decode_sliced walks them -- every slice but the last submits the records before its cut and the next slice starts at the
@@ -16,7 +16,7 @@
 #include <random>
 #include <vector>
 
-#include "cmb_decode_slices.hpp"
+#include "cmb_slices.hpp"
 
 namespace {
 int failures = 0;

@@ -1,10 +1,10 @@
-// The sharded decode's slice planner (coverm_b200/csrc/cmb_shard_slices.hpp) on random block tables: the slices cover the
+// The sliced decode's slice planner (coverm_b200/csrc/cmb_slices.hpp) on random block tables: the slices cover the
 // record blocks exactly once and in order, each fits the budget unless it is one block that alone exceeds it, each is as long as
 // the budget allows, and a budget below one block is reported slice by slice instead of looping.  Prints "ok <cases>".
 #include <cstdio>
 #include <random>
 
-#include "cmb_shard_slices.hpp"
+#include "cmb_slices.hpp"
 
 static int fails = 0;
 #define CHECK(cond, ...)                        \
@@ -34,7 +34,7 @@ int main() {
       o += 18 + clen[b] + 8;
       ustart[b + 1] = ustart[b] + isize;
     }
-    const ShardBlocks f{nb, o, coff.data(), clen.data(), ustart.data()};
+    const SliceBlocks f{nb, o, coff.data(), clen.data(), ustart.data()};
     const uint32_t first = (uint32_t)(rng() % nb);
     const uint64_t tail = rng() % 3 == 0 ? 0 : 1 + rng() % 200000;
     const uint64_t whole = slice_bytes(f, first, nb, tail);

@@ -1,4 +1,4 @@
-"""`--sharded` input decoded in block slices (cmb_shard_add, coverm_b200/csrc/cmb_shard_slices.hpp).
+"""`--sharded` input decoded in block slices (cmb_shard_add, coverm_b200/csrc/cmb_slices.hpp).
 
 CPU: the slice planner's invariants on random block tables (tests/native/shard_slices_check.cpp).  GPU (-m gpu): with
 CMB_DECODE_MEM_LIMIT_MB low enough that the shards after the first are decoded in many slices (the first, like a whole-shard

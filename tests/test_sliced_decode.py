@@ -1,5 +1,5 @@
 """The ordinary device decode in block slices (cmb_submit_bgzf when the whole-stream buffers do not fit;
-coverm_b200/csrc/cmb_decode_slices.hpp).
+coverm_b200/csrc/cmb_slices.hpp).
 
 CPU: the pair-mode cut and the slice budget against a brute-force walk (tests/native/decode_slices_check.cpp).  GPU (-m gpu):
 with CMB_DECODE_MEM_LIMIT_MB low enough for four or more slices, `coverm` prints what the unlimited run and the oracle print,
