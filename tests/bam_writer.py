@@ -44,6 +44,20 @@ def bgzf(stream, level=6, block_sizes=None, eof=True, empty_block_every=0, seed=
     return b"".join(out)
 
 
+def bgzf_cuts(stream, cuts, level=6, eof=True):
+    """Cut `stream` into BGZF blocks that end at each offset of the sorted list `cuts` (a repeated offset gives an empty
+    block there), then into blocks of 0xff00 bytes after the last cut."""
+    out, o = [], 0
+    for c in list(cuts) + list(range(cuts[-1] + 0xFF00 if cuts else 0xFF00, len(stream), 0xFF00)) + [len(stream)]:
+        assert o <= c <= len(stream), (o, c)
+        if c > o or (c == o and out and c < len(stream)):
+            out.append(bgzf_block(stream[o:c], level))
+        o = c
+    if eof:
+        out.append(BGZF_EOF)
+    return b"".join(out)
+
+
 def aux_bytes(tags):
     """tags: list of (tag, type, value); type in AcCsSiIfZHB (B takes (subtype, [values]))."""
     out = bytearray()
@@ -65,15 +79,18 @@ def aux_bytes(tags):
 
 
 def record(tid, pos, cigar, flag=0, mapq=60, qname="r", l_seq=None, mtid=-1, mpos=-1, tlen=0, tags=(("NM", "C", 0),), seq_byte=0x11,
-           qual_byte=30, rng=None):
-    """cigar: list of (op_char, len)."""
+           qual_byte=30, rng=None, qual=None):
+    """cigar: list of (op_char, len).  qual: the QUAL bytes (l_seq of them) instead of `qual_byte` repeated."""
     ops = [(CIGAR_OPS.index(c), n) for c, n in cigar]
     if l_seq is None:
         l_seq = sum(n for o, n in ops if o in (0, 1, 4, 7, 8))
     name = qname.encode() + b"\0"
     body = struct.pack("<iiBBHHHIiii", tid, pos, len(name), mapq, 4680, len(ops), flag, l_seq, mtid, mpos, tlen)
     body += name + b"".join(struct.pack("<I", (n << 4) | o) for o, n in ops)
-    if rng is None:
+    if qual is not None:
+        assert len(qual) == l_seq
+        body += bytes([seq_byte]) * ((l_seq + 1) // 2) + bytes(qual)
+    elif rng is None:
         body += bytes([seq_byte]) * ((l_seq + 1) // 2) + bytes([qual_byte]) * l_seq
     else:  # incompressible-ish SEQ, QUAL from a 40-letter alphabet
         body += rng.randbytes((l_seq + 1) // 2) + bytes(b % 40 for b in rng.randbytes(l_seq))
