@@ -1,6 +1,6 @@
 // libcoverm_b200 -- device-side BAM decode behind cmb_submit_bgzf / cmb_decode_bgzf (cmb_decode*.cuh): the staged call
 // (BgzfCall), the decode in block slices when the whole stream does not fit (decode_sliced), mate matching (cmb_pairs.cuh)
-// and `coverm filter` over the resident sample (cmb_filter.cuh).
+// and `coverm filter` (cmb_filter.cuh) over the resident sample or, through cmb_filter_bgzf, slice by slice.
 #include <algorithm>
 #include <atomic>
 #include <chrono>
@@ -37,6 +37,9 @@ size_t dec_window_bytes() {  // CMB_DECODE_WINDOW_KB: testing aid, lets a small 
   return v;
 }
 constexpr size_t DEC_SLACK = 1024;
+// the reference's panic in nm() (CMB_E_NM)
+constexpr const char* NM_PANIC = "Mapping record encountered that does not have an 'NM' auxiliary tag in the SAM/BAM format. This is "
+                                 "required to work out some coverage statistics";
 constexpr size_t DEC_FRONT = 256;              // readable bytes in front of the first uploaded block (the bit readers align down)
 
 // First-pass inflate kernel: 0 = kd_inflate_t1 (a thread per block + kd_crc32), 1 = kd_inflate_g8 (four blocks per warp), 2 =
@@ -837,8 +840,7 @@ extern "C" int cmb_filter_plan(cmb_ctx* c, int inverse, uint64_t* n_records, uin
   CU_TRY(c, cudaMemcpyAsync(h, d.d_cnt + 12, 16, cudaMemcpyDeviceToHost, c->stream));
   CU_TRY(c, cudaMemcpyAsync(&total, d.d_filter_anchor + n, 8, cudaMemcpyDeviceToHost, c->stream));
   CU_TRY(c, cudaStreamSynchronize(c->stream));
-  if (h[0] & ERR_NM)
-    return fail(c, CMB_E_NM, "Mapping record encountered that does not have an 'NM' auxiliary tag in the SAM/BAM format. This is required to work out some coverage statistics");
+  if (h[0] & ERR_NM) return fail(c, CMB_E_NM, "%s", NM_PANIC);
   unsigned long long n_emit;
   memcpy(&n_emit, h + 2, 8);
   if ((rc = d.d_filter_out.ensure(c, total, (size_t)total + (size_t)total / 8 + 4096))) return rc;
@@ -860,4 +862,208 @@ extern "C" int cmb_filter_fetch(cmb_ctx* c, uint8_t* records, uint64_t n_bytes) 
   if (n_bytes) CU_TRY(c, cudaMemcpyAsync(records, d.d_filter_out, n_bytes, cudaMemcpyDeviceToHost, c->stream));
   CU_TRY(c, cudaStreamSynchronize(c->stream));
   return CMB_OK;
+}
+
+// ------------------------------------------------------------------------------------------------ coverm filter, streamed
+namespace {
+
+using Clock = std::chrono::steady_clock;
+constexpr uint64_t FILTER_PIECE_BYTES = 64u << 20;  // most bytes per sink call, and the size of each pinned staging buffer
+double ms_since(Clock::time_point t0) { return std::chrono::duration<double, std::milli>(Clock::now() - t0).count(); }
+
+// One cmb_filter_bgzf call: the filter over the records of the resident decode (the whole stream, or one slice), and the
+// hand-over of what it returns to the sink.
+struct FilterCall {
+  cmb_ctx* c;
+  int inverse;
+  cmb_filter_sink sink;
+  void* user;
+  cmb_filter_result* out;
+  bool pair_path;  // filter.rs:117-233 (mates matched), else the singles path (filter.rs:88-116)
+
+  // The filter kernels over records [0, n) of the last decode (its mates matched on the pair path), then the returned records
+  // to the sink in pieces of at most FILTER_PIECE_BYTES, each through the next staging buffer.  Every allocation comes before
+  // the first sink call: CMB_E_NOMEM means nothing was handed over.
+  int filter(uint32_t n) {
+    auto& d = c->dec;
+    const auto t0 = Clock::now();
+    int rc;
+    if ((rc = d.d_filter_anchor.ensure(c, (size_t)n + 1, with_slack(n))) || (rc = d.d_filter_role.ensure(c, (size_t)n + 1, with_slack(n))))
+      return rc;
+    cmb_read_batch tb;
+    carve_batch(d.d_tuple_slab, d.last_n_rec, d.last_n_cig, &tb);
+    FilterArgs a{};
+    a.data = d.last_infl_base; a.rec_off = d.d_rec_off; a.n = n; a.flag = tb.flag; a.mapq = tb.mapq; a.nm_state = tb.nm_state; a.nm = tb.nm;
+    a.l_seq = tb.l_seq; a.aligned = tb.aligned; a.del = tb.del; a.mate = pair_path ? d.last_mate : nullptr; a.p = c->params;
+    a.filter_single = c->mode.filter_single_reads; a.pair_path = pair_path; a.filter_out = inverse ? 0 : 1;
+    a.anchor_bytes = d.d_filter_anchor; a.role = d.d_filter_role; a.error_flags = d.d_cnt + 12; a.n_emit = (unsigned long long*)(d.d_cnt + 14);
+    CU_TRY(c, cudaMemsetAsync(d.d_cnt + 12, 0, 16, c->stream));
+    kf_decide<<<(n + 255) / 256, 256, 0, c->stream>>>(a);
+    kf_scan<<<1, 1024, 0, c->stream>>>(d.d_filter_anchor, n);
+    CU_TRY(c, cudaGetLastError());
+    uint32_t h[4];
+    unsigned long long total = 0, n_emit = 0;
+    CU_TRY(c, cudaMemcpyAsync(h, d.d_cnt + 12, 16, cudaMemcpyDeviceToHost, c->stream));
+    CU_TRY(c, cudaMemcpyAsync(&total, d.d_filter_anchor + n, 8, cudaMemcpyDeviceToHost, c->stream));
+    CU_TRY(c, cudaStreamSynchronize(c->stream));
+    if (h[0] & ERR_NM) return fail(c, CMB_E_NM, "%s", NM_PANIC);
+    memcpy(&n_emit, h + 2, 8);
+    if (total) {
+      if ((rc = d.d_filter_out.ensure(c, total, (size_t)total + (size_t)total / 8 + 4096))) return rc;
+      a.out = d.d_filter_out;
+      kf_gather<<<(n + 7) / 8, 256, 0, c->stream>>>(a);
+      CU_TRY(c, cudaGetLastError());
+    }
+    CU_TRY(c, cudaStreamSynchronize(c->stream));
+    out->ms_filter += (float)ms_since(t0);
+    if (!total) return CMB_OK;
+    // Both staging buffers have their fixed size once allocated, so that none is freed while the caller still reads it
+    for (auto& stage : d.filter_stage)
+      if ((rc = stage.ensure(c, FILTER_PIECE_BYTES))) return rc;
+    for (uint64_t o = 0; o < total; o += FILTER_PIECE_BYTES) {
+      // sink call k - 1's bytes are in the other buffer, which its caller may still be reading
+      const auto t1 = Clock::now();
+      const uint64_t len = std::min<uint64_t>(FILTER_PIECE_BYTES, total - o);
+      uint8_t* stage = d.filter_stage[out->n_sink_calls & 1];
+      CU_TRY(c, cudaMemcpyAsync(stage, d.d_filter_out + o, len, cudaMemcpyDeviceToHost, c->stream));
+      CU_TRY(c, cudaStreamSynchronize(c->stream));
+      out->ms_d2h += (float)ms_since(t1);
+      if (const int s = sink(user, stage, len)) return fail(c, CMB_E_ARG, "cmb_filter_bgzf: the sink returned %d", s);
+      out->n_sink_calls += 1;
+      out->n_bytes += len;
+    }
+    out->n_records += n_emit;
+    return CMB_OK;
+  }
+
+  // Device bytes the filter holds beside the decode buffers: they count as room, since they are reused or freed to grow
+  uint64_t held() const {
+    const auto& d = c->dec;
+    uint64_t b = decode_bytes(c) + d.d_filter_anchor.bytes() + d.d_filter_role.bytes() + d.d_filter_out.bytes();
+    if (pair_path) b += d.d_pair_key.bytes() + d.d_pair_mate.bytes() + d.d_pair_next.bytes() + d.d_pair_tag.bytes() + d.d_pair_head.bytes();
+    return b;
+  }
+  void release_filter() {
+    auto& d = c->dec;
+    d.d_filter_anchor.release();
+    d.d_filter_role.release();
+    d.d_filter_out.release();
+  }
+
+  // The whole stream when its buffers fit; else slices
+  int whole(const cmb_bgzf_input* in) {
+    auto& d = c->dec;
+    d.last_valid = false;
+    d.filter_planned = false;
+    cmb_bgzf_result br{};
+    int rc = submit_bgzf_impl(c, in, &br, true);
+    if (!rc && d.last_valid) {
+      out->ms_decode = br.ms_total;
+      const uint32_t n = d.last_n_rec;
+      const auto t0 = Clock::now();
+      if (pair_path && n) rc = match_mates(c, d.last_infl_base, n, !inverse, "cmb_filter_bgzf");
+      out->ms_filter += (float)ms_since(t0);
+      if (!rc && n) rc = filter(n);
+    }
+    if (rc != CMB_E_NOMEM) return rc;
+    release_filter();  // nothing was handed over: every buffer is allocated before the sink call
+    release_decode(c);
+    return sliced(in);
+  }
+
+  // The stream in block slices (decode_in_slices), each filtered up to its cut and handed to the sink
+  int sliced(const cmb_bgzf_input* in) {
+    auto& d = c->dec;
+    auto decline = [&](int rc) {
+      release_decode(c);
+      return rc;
+    };
+    auto room = [&] { return device_room(held()); };
+    if (room() < SLICE_MIN_BYTES) return decline(fail(c, CMB_E_DECLINED, "cmb_filter_bgzf: not enough device memory for device-side decode"));
+    uint64_t stream_end = 0;
+    for (uint32_t b = 0; b < in->n_blocks; ++b) stream_end += in->block_isize[b];
+    double side = 0;     // the last slice's other buffers per compressed + inflated byte
+    uint32_t carry = 0;  // pair path: the largest eligible tid of the slices so far
+    auto budget = [&](uint64_t at) -> uint64_t {
+      const uint64_t done = at > in->records_at ? at - in->records_at : 0;
+      const uint64_t total = stream_end > in->records_at ? stream_end - in->records_at : 0;
+      return decode_slice_budget(room(), false, 0, done, total, 0, side);
+    };
+    auto step = [&](BgzfCall& j, cmb_bgzf_result&, uint64_t* next) -> int {
+      const uint32_t n = (uint32_t)j.n_rec;
+      uint32_t cut = n, largest = carry;
+      uint64_t held_back = 0;
+      int rc;
+      const auto t0 = Clock::now();
+      if (pair_path) {
+        // words 12..14 of d_cnt: the slice's largest eligible tid, then the cut's `after` and n - cut (zeroed by copy_inflate)
+        uint32_t* w = d.d_cnt + 12;
+        rc = match_mates(c, d.last_infl_base, n, !inverse, "cmb_filter_bgzf", carry, w);
+        if (rc == CMB_E_NOMEM) return SLICE_HALVE;
+        if (rc) return rc;
+        if (j.walk_end < in->n_blocks) {  // not the last slice: hold the trailing run of its last eligible tid back for the next one
+          cmb_read_batch tb;
+          carve_batch(d.d_tuple_slab, n, (uint32_t)j.n_cig, &tb);
+          const uint32_t g = (n + 255) / 256;
+          kd_pair_cut_after<<<g, 256, 0, c->stream>>>(d.d_pair_key, tb.tid, n, w, w + 1);
+          kd_pair_cut_at<<<g, 256, 0, c->stream>>>(d.d_pair_key, tb.tid, n, w, w + 1, w + 2);
+          CU_TRY(c, cudaGetLastError());
+        }
+        uint32_t h[3] = {0, 0, 0};
+        CU_TRY(c, cudaMemcpyAsync(h, w, 12, cudaMemcpyDeviceToHost, c->stream));
+        CU_TRY(c, cudaStreamSynchronize(c->stream));
+        largest = h[0];
+        cut = n - h[2];
+        if (cut == 0)
+          return fail(c, CMB_E_DECLINED, "cmb_filter_bgzf: the proper-pair records of reference %d do not fit in one decode slice; the "
+                      "filter runs on the host", (int32_t)largest);
+        if (cut < n) {  // the next slice starts at record `cut`
+          uint64_t off = 0;
+          CU_TRY(c, cudaMemcpy(&off, d.d_rec_off + cut, 8, cudaMemcpyDeviceToHost));
+          *next = off;
+          held_back = n - cut;
+        }
+      }
+      out->ms_filter += (float)ms_since(t0);
+      rc = filter(cut);
+      if (rc == CMB_E_NOMEM) {
+        release_filter();
+        return SLICE_HALVE;
+      }
+      if (rc) return rc;
+      carry = largest;
+      out->pair_cut_records += held_back;
+      const uint64_t other = held() - d.d_comp.bytes() - d.d_inflated.bytes();
+      side = (double)other / (double)std::max<uint64_t>(1, (j.byte_hi - j.byte_lo) + (j.total - j.u_lo));
+      return CMB_OK;
+    };
+    auto nomem = [&](const SliceBlocks&, uint32_t, uint32_t, uint64_t) {
+      return fail(c, CMB_E_DECLINED, "cmb_filter_bgzf: not enough device memory for device-side decode");
+    };
+    SliceStats ss;
+    cmb_bgzf_result r{};
+    const int rc = decode_in_slices(c, in, &r, ss, budget, step, nomem);
+    release_decode(c);  // the next input needs the room; a sliced decode has no resident stream to keep
+    out->n_slices = ss.n_slices;  // on a decline: the slices handed over before it
+    out->halvings = ss.halvings;
+    if (rc) return rc;
+    out->ms_decode = ss.ms_inflate + ss.ms_chain + ss.ms_extract;
+    if (getenv("CMB_PIPELINE_STATS"))
+      fprintf(stderr, "#filter_slices\tslices=%u\tmax_slice_bytes=%llu\thalvings=%u\tpair_cut_records=%llu\n", ss.n_slices,
+              (unsigned long long)ss.max_slice, ss.halvings, (unsigned long long)out->pair_cut_records);
+    return CMB_OK;
+  }
+};
+
+}  // namespace
+
+extern "C" int cmb_filter_bgzf(cmb_ctx* c, const cmb_bgzf_input* in, int inverse, cmb_filter_sink sink, void* user, cmb_filter_result* out) {
+  NvtxRange nvtx("cmb_filter_bgzf");
+  if (!c || !in || !sink || !out) return fail(c, CMB_E_ARG, "cmb_filter_bgzf: null argument");
+  *out = cmb_filter_result{};
+  if (!c->have_params || c->in_sample) return fail(c, CMB_E_ARG, "cmb_filter_bgzf: set the parameters first; not inside a sample");
+  if (c->n_acquired) return fail(c, CMB_E_ARG, "cmb_filter_bgzf: a staging batch is still acquired");
+  CU_TRY(c, cudaSetDevice(c->device));
+  FilterCall f{c, inverse, sink, user, out, !(c->mode.filter_single_reads && !c->mode.filter_pairs)};
+  return f.whole(in);
 }

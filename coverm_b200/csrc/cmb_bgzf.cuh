@@ -1,6 +1,7 @@
 // The device decode as the rest of the library drives it (cmb_bgzf.cu): one staged decode call (BgzfCall), the memory its
-// buffers take, and the loop that decodes a stream in block slices.  Ordinary streams that do not fit (decode_sliced) and the
-// shards of sharded input (decode_shard, cmb_shard_input.cu) each drive that loop with their own budget and per-slice step.
+// buffers take, and the loop that decodes a stream in block slices.  Ordinary streams that do not fit (decode_sliced), `coverm
+// filter` over such a stream (cmb_filter_bgzf) and the shards of sharded input (decode_shard, cmb_shard_input.cu) each drive
+// that loop with their own budget and per-slice step.
 #pragma once
 #include <algorithm>
 #include <climits>

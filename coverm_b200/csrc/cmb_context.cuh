@@ -221,6 +221,7 @@ struct cmb_ctx {
     Buf<uint8_t> d_filter_out;
     uint64_t filter_bytes = 0;
     bool filter_planned = false;
+    PinnedBuf<uint8_t> filter_stage[2];  // cmb_filter_bgzf: sink call k's bytes are in filter_stage[k & 1]; 64 MB each
     std::vector<PinnedBuf<uint8_t>> pinned;  // two copy slots per copy stream
     std::vector<cudaStream_t> streams;
     std::vector<cudaEvent_t> slot_events, done_events;

@@ -390,16 +390,15 @@ inline CliResult run_cli_rank(const std::vector<std::string>& args, const std::v
         in.path = o.bam_files[k];
         for (auto& m : memory_inputs)
           if (m.path == in.path) in = m;
-        const FilterRun run = filter_one_input(*session, in, fp, o.inverse);
-        if (o.timing) err << "#filter\tsample=" << k << "\trecords_out=" << run.n_records << "\tdevice=" << (run.on_device ? 1 : 0) << '\n';
-        if (o.sub == "filter-names") {
-          for (size_t off = 0; off + 4 <= run.records.size(); off += 4 + (size_t)rd_u32(run.records.data() + off)) out << bam_qname(run.records.data() + off) << '\n';
+        if (o.sub == "filter-names") {  // printed once the input is done: an input that ends in an error prints nothing of it
+          RecordsSink names;
+          const FilterRun run = filter_one_input(*session, in, fp, o.inverse, names);
+          if (o.timing) err << "#filter\tsample=" << k << "\trecords_out=" << run.n_records << "\tdevice=" << (run.on_device ? 1 : 0) << '\n';
+          for (size_t off = 0; off + 4 <= names.bytes.size(); off += 4 + (size_t)rd_u32(names.bytes.data() + off)) out << bam_qname(names.bytes.data() + off) << '\n';
         } else {
-          std::ofstream bam(o.output_bam_files[k], std::ios::binary);
-          if (!bam) throw Panic("Failed to write BAM file " + o.output_bam_files[k]);
-          write_bgzf(bam, {run.header_bytes.data(), run.records.data()}, {run.header_bytes.size(), run.records.size()}, session->pool());
-          bam.flush();
-          if (!bam) throw Panic("Failed to write BAM record");
+          BamFileSink bam(o.output_bam_files[k], session->pool());
+          const FilterRun run = filter_one_input(*session, in, fp, o.inverse, bam);
+          if (o.timing) err << "#filter\tsample=" << k << "\trecords_out=" << run.n_records << "\tdevice=" << (run.on_device ? 1 : 0) << '\n';
         }
       }
       out.flush();

@@ -1,15 +1,24 @@
 // `coverm filter` (src/bin/coverm.rs:408-472): ReferenceSortedBamFilter (src/filter.rs:36-234) used as a record sink --
 // every record the filter returns is written, in the order it returns them, into a new BAM file with the input's header.
 //
-// Fast path: the sample is decoded on the GPU (cmb_decode_bgzf), the device decides and orders the returned records
-// (cmb_filter_plan, cmb_filter.cuh) and hands their bytes back; this file then only compresses and writes.  Fallback (SAM /
-// uncompressed input, a stream the device declines): FilterOnHost below runs the reference's loop on the host.
+// Fast path: the sample is decoded on the GPU (cmb_filter_bgzf: whole, or in block slices when it does not fit), the device
+// decides and orders the returned records (cmb_filter.cuh) and hands their bytes back piece by piece; this file compresses and
+// writes each piece while the device works on the next (BgzfWriter).  Fallback (SAM / uncompressed input, a stream the device
+// declines): filter_on_host below runs the reference's loop on the host.
 // `filter-names` prints the returned records' names instead of writing a BAM: the form in which the reference's unit tests
 // (filter.rs:342-844) state their expectations.
 #pragma once
+#include <cstdio>
+#include <exception>
 #include <fstream>
 
+#include "bgzf_writer.hpp"
 #include "sample_processor.hpp"
+
+// Referenced weakly: the host code also links against stand-ins of the device library without it (the CPU emulator of the ABI),
+// where every input takes the host loop.  libcoverm_b200 always defines it.
+extern "C" int cmb_filter_bgzf(cmb_ctx* ctx, const cmb_bgzf_input* in, int inverse, cmb_filter_sink sink, void* user,
+                               cmb_filter_result* out) __attribute__((weak));
 
 namespace cmbh {
 
@@ -80,71 +89,112 @@ inline void filter_on_host(const uint8_t* recs, size_t n_bytes, const HostFilter
   });
 }
 
-// BGZF writer: `data` cut into blocks of at most 0xff00 bytes, deflated on all threads, followed by the EOF marker.
-inline void write_bgzf(std::ostream& os, const std::vector<const uint8_t*>& parts, const std::vector<size_t>& sizes, ThreadPool& pool) {
-  // flatten the parts into block jobs (a block may span parts: assemble per job)
-  size_t total = 0;
-  for (size_t s : sizes) total += s;
-  const size_t BLOCK = 0xff00;
-  const size_t n_blocks = (total + BLOCK - 1) / BLOCK;
-  std::vector<size_t> part_start(parts.size() + 1, 0);
-  for (size_t i = 0; i < parts.size(); ++i) part_start[i + 1] = part_start[i] + sizes[i];
-  auto copy_range = [&](size_t from, size_t len, uint8_t* dst) {
-    size_t i = (size_t)(std::upper_bound(part_start.begin(), part_start.end(), from) - part_start.begin()) - 1;
-    while (len) {
-      const size_t in_part = from - part_start[i];
-      const size_t take = std::min(len, sizes[i] - in_part);
-      memcpy(dst, parts[i] + in_part, take);
-      dst += take;
-      from += take;
-      len -= take;
-      ++i;
+// Where `coverm filter` sends one input's output: the header bytes, then the returned records in the reference's order, in
+// as many pieces as they arrive.  A piece's bytes stay valid until the next call into the sink returns; after the last piece
+// the caller calls finish() or restart() before they go.
+struct FilterSink {
+  virtual ~FilterSink() = default;
+  virtual void header(const uint8_t* p, size_t n) = 0;
+  virtual void records(const uint8_t* p, size_t n) = 0;
+  // Forget everything received (the input is filtered again from its start, or it ended in an error); nothing received is
+  // read after this returns.  Does not throw.
+  virtual void restart() noexcept = 0;
+  virtual void finish() = 0;  // the input is done: nothing of it is still being written after this returns
+};
+
+// `coverm filter`'s output BAM, compressed and written while the device works.  The file is created by the first piece and
+// removed again unless finish() is reached: an input that ends in an error leaves no output file.
+class BamFileSink : public FilterSink {
+ public:
+  BamFileSink(std::string path, ThreadPool& pool) : path_(std::move(path)), pool_(pool) {}
+  ~BamFileSink() override {
+    if (done_ || !created_) return;
+    writer_.reset();
+    if (file_.is_open()) file_.close();
+    std::remove(path_.c_str());
+  }
+  void header(const uint8_t* p, size_t n) override { open().feed(p, n); }
+  void records(const uint8_t* p, size_t n) override { open().feed(p, n); }
+  void restart() noexcept override {
+    writer_.reset();  // waits for the blocks being deflated, and drops their error
+    if (file_.is_open()) file_.close();  // the next piece truncates it
+  }
+  void finish() override {
+    open().finish();
+    file_.flush();
+    if (!file_) throw Panic("Failed to write BAM record");
+    done_ = true;
+  }
+
+ private:
+  BgzfWriter& open() {
+    if (!writer_) {
+      file_.open(path_, std::ios::binary | std::ios::trunc);
+      if (!file_) throw Panic("Failed to write BAM file " + path_);
+      created_ = true;
+      writer_ = std::make_unique<BgzfWriter>(file_, pool_);
     }
-  };
-  const size_t GROUP = 64;  // blocks per task, written in order group by group
-  std::vector<std::vector<uint8_t>> done((n_blocks + GROUP - 1) / GROUP);
-  pool.parallel_for(done.size(), [&](size_t g, int) {
-    std::vector<uint8_t> raw(BLOCK), comp(BLOCK + 1024);
-    z_stream zs;
-    memset(&zs, 0, sizeof zs);
-    if (deflateInit2(&zs, Z_DEFAULT_COMPRESSION, Z_DEFLATED, -15, 8, Z_DEFAULT_STRATEGY) != Z_OK) throw ExitError(1, "zlib init failed");
-    std::vector<uint8_t>& outb = done[g];
-    for (size_t b = g * GROUP; b < std::min(n_blocks, (g + 1) * GROUP); ++b) {
-      const size_t from = b * BLOCK, len = std::min(BLOCK, total - from);
-      copy_range(from, len, raw.data());
-      deflateReset(&zs);
-      zs.next_in = raw.data();
-      zs.avail_in = (uInt)len;
-      zs.next_out = comp.data();
-      zs.avail_out = (uInt)comp.size();
-      if (deflate(&zs, Z_FINISH) != Z_STREAM_END) throw ExitError(1, "deflate failed");
-      const size_t clen = zs.total_out;
-      const uint32_t bsize = (uint32_t)(12 + 6 + clen + 8 - 1);
-      const uint8_t head[18] = {0x1f, 0x8b, 8, 4, 0, 0, 0, 0, 0, 0xff, 6, 0, 'B', 'C', 2, 0, (uint8_t)(bsize & 0xff), (uint8_t)(bsize >> 8)};
-      outb.insert(outb.end(), head, head + 18);
-      outb.insert(outb.end(), comp.data(), comp.data() + clen);
-      const uint32_t crc = (uint32_t)crc32(0, raw.data(), (uInt)len), isz = (uint32_t)len;
-      uint8_t tail[8];
-      memcpy(tail, &crc, 4);
-      memcpy(tail + 4, &isz, 4);
-      outb.insert(outb.end(), tail, tail + 8);
-    }
-    deflateEnd(&zs);
-  });
-  for (auto& b : done) os.write((const char*)b.data(), (std::streamsize)b.size());
-  static const uint8_t eof[28] = {0x1f, 0x8b, 8, 4, 0, 0, 0, 0, 0, 0xff, 6, 0, 0x42, 0x43, 2, 0, 0x1b, 0, 3, 0, 0, 0, 0, 0, 0, 0, 0, 0};
-  os.write((const char*)eof, sizeof eof);
-}
+    return *writer_;
+  }
+  std::string path_;
+  ThreadPool& pool_;
+  std::ofstream file_;
+  std::unique_ptr<BgzfWriter> writer_;
+  bool created_ = false, done_ = false;
+};
+
+// `filter-names`: the returned records, kept until the input is done
+struct RecordsSink : FilterSink {
+  std::vector<uint8_t> bytes;
+  void header(const uint8_t*, size_t) override {}
+  void records(const uint8_t* p, size_t n) override { bytes.insert(bytes.end(), p, p + n); }
+  void restart() noexcept override { bytes.clear(); }
+  void finish() override {}
+};
 
 struct FilterRun {
-  std::vector<uint8_t> header_bytes;  // the uncompressed BAM header block: magic .. last reference entry
-  std::vector<uint8_t> records;       // returned records, back to back
   uint64_t n_records = 0;
   bool on_device = false;
 };
 
-// One input through the filter.  `params`: thresholds + flag includes with filtering = 1; inverse = --inverse.
-inline FilterRun filter_one_input(DeviceSession& session, const InputSpec& in, const cmb_params& params, bool inverse) {
+// cmb_filter_bgzf's sink: the pieces to a FilterSink, whose first error is kept for the caller to rethrow
+struct DeviceSinkCall {
+  FilterSink* sink = nullptr;
+  std::exception_ptr error;
+  static int piece(void* user, const uint8_t* p, uint64_t n) {
+    auto* s = static_cast<DeviceSinkCall*>(user);
+    try {
+      s->sink->records(p, n);
+      return 0;
+    } catch (...) {
+      s->error = std::current_exception();
+      return 1;
+    }
+  }
+};
+
+// Restarts the sink on every exit but a finished one: the pieces it was fed from buffers that go with the caller's frame are not
+// read after they are gone.
+class SinkSettle {
+ public:
+  explicit SinkSettle(FilterSink& sink) : sink_(sink) {}
+  ~SinkSettle() {
+    if (!finished_) sink_.restart();
+  }
+  SinkSettle(const SinkSettle&) = delete;
+  SinkSettle& operator=(const SinkSettle&) = delete;
+  void finish() {
+    sink_.finish();
+    finished_ = true;
+  }
+
+ private:
+  FilterSink& sink_;
+  bool finished_ = false;
+};
+
+// One input through the filter into `sink`.  `params`: thresholds + flag includes with filtering = 1; inverse = --inverse.
+inline FilterRun filter_one_input(DeviceSession& session, const InputSpec& in, const cmb_params& params, bool inverse, FilterSink& sink) {
   FilterRun run;
   const BamInput input(in);
   cmb_ctx* ctx = session.ctx();
@@ -154,25 +204,32 @@ inline FilterRun filter_one_input(DeviceSession& session, const InputSpec& in, c
   InflateStream stream(input.data(), input.size(), session.pool(), 1u << 20);
   std::vector<uint8_t> buf;
   const BamHeader h = read_bam_header(stream, buf, in.path);
-  run.header_bytes.assign(buf.begin(), buf.begin() + (ptrdiff_t)h.records_at);
+  const std::vector<uint8_t> header(buf.begin(), buf.begin() + (ptrdiff_t)h.records_at);  // magic .. last reference entry
+  std::vector<uint8_t> records;  // the host loop's output
+  SinkSettle settle(sink);       // after `header` and `records`: gone before them
   const BlockIndex& bx = stream.index();
-  if (bx.bgzf && !getenv("CMB_HOST_DECODE")) {
+  if (bx.bgzf && cmb_filter_bgzf && !getenv("CMB_HOST_DECODE")) {
+    sink.header(header.data(), header.size());  // written on the pool while the device decodes, which does not use it
     const BgzfInput bi(bx, (uint32_t)h.header->names.size(), h.records_at, session.pool().size());
-    cmb_bgzf_result br{};
-    rc = cmb_decode_bgzf(ctx, &bi.in, &br);
-    uint64_t n_rec = 0, n_bytes = 0;
-    // the plan declines a stream whose mates the device cannot match in file order (cmb_pairs.cuh): the host loop takes it
-    if (rc == CMB_OK) rc = cmb_filter_plan(ctx, inverse ? 1 : 0, &n_rec, &n_bytes);
+    DeviceSinkCall sc;
+    sc.sink = &sink;
+    cmb_filter_result fr{};
+    rc = cmb_filter_bgzf(ctx, &bi.in, inverse ? 1 : 0, &DeviceSinkCall::piece, &sc, &fr);
+    if (sc.error) std::rethrow_exception(sc.error);
     if (rc == CMB_OK) {
-      run.records.resize(n_bytes);
-      rc = cmb_filter_fetch(ctx, run.records.data(), n_bytes);
-      if (rc) throw_device_error(ctx, rc);
-      run.n_records = n_rec;
+      settle.finish();
+      run.n_records = fr.n_records;
       run.on_device = true;
       return run;
     }
+    // the device declines a stream whose mates it cannot match in file order (cmb_pairs.cuh), among others: the host loop
+    // takes it from the start, whatever was handed over already
     if (rc != CMB_E_DECLINED) throw_device_error(ctx, rc);
-    if (getenv("CMB_PIPELINE_STATS")) fprintf(stderr, "#device_decode\tdeclined: %s\n", cmb_last_error(ctx));
+    if (getenv("CMB_PIPELINE_STATS")) {
+      fprintf(stderr, "#device_decode\tdeclined: %s\n", cmb_last_error(ctx));
+      fprintf(stderr, "#filter_declined\tslices_before=%u\tsink_calls=%u\n", fr.n_slices, fr.n_sink_calls);
+    }
+    sink.restart();  // the writer is idle after this: the host decoder below needs the pool
   }
   // host fallback: the whole record stream in memory, then the reference's loop
   while (stream.fill(buf)) {
@@ -182,7 +239,10 @@ inline FilterRun filter_one_input(DeviceSession& session, const InputSpec& in, c
   f.filter_single = mode.filter_single_reads;
   f.filter_pairs = mode.filter_pairs;
   f.filter_out = !inverse;
-  filter_on_host(buf.data() + h.records_at, buf.size() - h.records_at, f, run.records, run.n_records);
+  filter_on_host(buf.data() + h.records_at, buf.size() - h.records_at, f, records, run.n_records);
+  sink.header(header.data(), header.size());
+  sink.records(records.data(), records.size());
+  settle.finish();
   return run;
 }
 

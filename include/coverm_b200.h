@@ -376,6 +376,30 @@ int cmb_shard_choose(cmb_ctx* ctx, uint64_t* err_key);
 int cmb_shard_finish_group(cmb_ctx* ctx, uint64_t err_key, cmb_shard_result* out);
 int cmb_filter_plan(cmb_ctx* ctx, int inverse, uint64_t* n_records, uint64_t* n_bytes);
 int cmb_filter_fetch(cmb_ctx* ctx, uint8_t* records, uint64_t n_bytes);
+/* ---- `coverm filter` over a stream of any size ----
+ * cmb_filter_bgzf hands the records the filter returns to `sink`, in the reference's order, as consecutive byte ranges of at
+ * most 64 MB (each record with its 4-byte block_size; a range may end inside a record).  When the whole-stream decode fits, it
+ * is cmb_decode_bgzf + cmb_filter_plan with what cmb_filter_fetch would copy handed to the sink.  When it does not
+ * (CMB_E_NOMEM), the stream is decoded in block slices and filtered slice by slice, each slice's records handed over before the
+ * next slice is decoded.  In pair mode a slice that is not the last holds back the trailing run of its last eligible reference
+ * id for the next slice, so that every pair lies in one slice.  The bytes of sink call k lie in one of two pinned staging
+ * buffers of the context (64 MB each) and stay valid until sink call k + 1 returns -- the last call's until the context's next
+ * cmb_filter_bgzf or cmb_destroy: the caller may keep working on them (compressing them) while the device goes on.  A sink
+ * returning non-zero stops the call with CMB_E_ARG.
+ * CMB_E_DECLINED (the stream is not BGZF, a CG:B placeholder, a corrupt block, proper pairs out of reference-id order, one
+ * reference's proper pairs larger than a slice, too little device memory) may come after some sink calls: the caller then
+ * discards what it received and runs the filter on the host.  CMB_E_NM (the reference's panic in nm()) is raised in the slice
+ * that meets it, before that slice's first sink call.  A sliced call gives its decode buffers back when it ends. */
+typedef int (*cmb_filter_sink)(void* user, const uint8_t* bytes, uint64_t n_bytes);
+typedef struct cmb_filter_result {
+  uint64_t n_records, n_bytes;  /* returned records and their bytes, summed over the sink calls              */
+  uint32_t n_slices;            /* block slices decoded (on CMB_E_DECLINED: before it); 0: the whole stream fit */
+  uint32_t halvings;            /* slices halved because their buffers did not fit                           */
+  uint64_t pair_cut_records;    /* pair mode: records held back at slice ends (each decoded twice)           */
+  uint32_t n_sink_calls;
+  float ms_decode, ms_filter, ms_d2h; /* device decode (CUDA events), mate matching + filter kernels, staging copies (host clock) */
+} cmb_filter_result;
+int cmb_filter_bgzf(cmb_ctx* ctx, const cmb_bgzf_input* in, int inverse, cmb_filter_sink sink, void* user, cmb_filter_result* out);
 
 /* The tuples the last successful cmb_submit_bgzf extracted, still resident in device memory (valid until the next
  * cmb_submit_bgzf / cmb_destroy): DEVICE pointers laid out as cmb_read_batch, ready for cmb_submit_device_batch.
