@@ -176,6 +176,12 @@ uint64_t cmb::device_room(uint64_t held) {
 
 // ------------------------------------------------------------------------------------------------ the stages of one call
 
+int BgzfCall::run() {
+  int rc = prepare();
+  if (!rc && !nothing_to_decode && !(rc = copy_inflate()) && !(rc = declined()) && !(rc = chain())) rc = extract();
+  return rc;
+}
+
 // Stage 1: the block table, the blocks this call decodes, its copy windows, and every buffer, stream and copy slot it needs.
 int BgzfCall::prepare() {
   ustart.assign((size_t)nb + 1, 0);
@@ -592,6 +598,15 @@ int BgzfCall::excl_n(uint32_t* n) {
   return CMB_OK;
 }
 
+int BgzfCall::stage_times() {
+  CU_TRY(c, cudaEventSynchronize(d.ev[4]));
+  cudaEventElapsedTime(&out->ms_copy_inflate, d.ev[0], d.ev[2]);
+  cudaEventElapsedTime(&out->ms_chain, d.ev[2], d.ev[3]);
+  cudaEventElapsedTime(&out->ms_extract, d.ev[3], d.ev[4]);
+  cudaEventElapsedTime(&out->ms_total, d.ev[0], d.ev[4]);
+  return CMB_OK;
+}
+
 // ------------------------------------------------------------------------------------------------ mate matching
 int cmb::match_mates(cmb_ctx* c, const uint8_t* infl_base, uint32_t n_rec, bool filter_out, const char* who, uint32_t carry,
                      uint32_t* largest) {
@@ -653,123 +668,162 @@ int submit_bgzf_impl(cmb_ctx* c, const cmb_bgzf_input* in, cmb_bgzf_result* out,
   if (in->n_blocks == 0) return CMB_OK;
   CU_TRY(c, cudaSetDevice(c->device));
   BgzfCall j{c, c->dec, in, out, decode_only, in->n_blocks};
-  int rc;
-  if ((rc = j.prepare()) || j.nothing_to_decode) return rc;
-  if ((rc = j.copy_inflate()) || (rc = j.declined()) || (rc = j.chain()) || (rc = j.extract())) return rc;
-  auto& d = c->dec;
-  CU_TRY(c, cudaEventSynchronize(d.ev[4]));
-  cudaEventElapsedTime(&out->ms_copy_inflate, d.ev[0], d.ev[2]);
-  cudaEventElapsedTime(&out->ms_chain, d.ev[2], d.ev[3]);
-  cudaEventElapsedTime(&out->ms_extract, d.ev[3], d.ev[4]);
-  cudaEventElapsedTime(&out->ms_total, d.ev[0], d.ev[4]);
+  const int rc = j.run();
+  if (rc || j.nothing_to_decode) return rc;
+  return j.stage_times();
+}
+
+// A whole-stream call that ran out of device memory did so before anything was accumulated (K1) or handed over (the filter's
+// sink): its buffers go back, so that the rest has room, and slices() takes the stream instead.
+template <class Slices>
+int whole_or_slices(cmb_ctx* c, int rc, Slices slices) {
+  if (rc != CMB_E_NOMEM) return rc;
+  release_decode(c);
+  return slices();
+}
+
+// Device bytes of the mate-matching buffers
+uint64_t pair_bytes(const cmb_ctx* c) {
+  const auto& d = c->dec;
+  return d.d_pair_key.bytes() + d.d_pair_mate.bytes() + d.d_pair_next.bytes() + d.d_pair_tag.bytes() + d.d_pair_head.bytes();
+}
+
+// Pair mode: the mates of the slice j decoded, matched after the slices before it (`carry`: their largest eligible tid), and
+// unless it is the stream's `last` slice, the trailing run of its last eligible tid held back for the next one (cmb_slices.hpp).
+// *largest: the slice's largest eligible tid; *cut: the records it keeps, and when that is fewer than it decoded, *next: record
+// `cut`'s offset, where the next slice starts.  A run that is the whole slice declines, the message naming the entry point
+// (`who`) and where the stream goes instead (`host_route`).  SLICE_HALVE when mate matching runs out of memory.
+int pair_cut(BgzfCall& j, bool filter_out, uint32_t carry, bool last, const char* who, const char* host_route, uint32_t* largest,
+             uint32_t* cut, uint64_t* next) {
+  cmb_ctx* c = j.c;
+  auto& d = j.d;
+  const uint32_t n = (uint32_t)j.n_rec;
+  // words 12..14 of d_cnt: the slice's largest eligible tid, then the cut's `after` and n - cut (zeroed by copy_inflate)
+  uint32_t* w = d.d_cnt + 12;
+  const int rc = match_mates(c, d.last_infl_base, n, filter_out, who, carry, w);
+  if (rc == CMB_E_NOMEM) return SLICE_HALVE;
+  if (rc) return rc;
+  j.out->n_launches += 5;
+  if (!last) {
+    cmb_read_batch tb;
+    carve_batch(d.d_tuple_slab, n, (uint32_t)j.n_cig, &tb);
+    const uint32_t g = (n + 255) / 256;
+    kd_pair_cut_after<<<g, 256, 0, c->stream>>>(d.d_pair_key, tb.tid, n, w, w + 1);
+    kd_pair_cut_at<<<g, 256, 0, c->stream>>>(d.d_pair_key, tb.tid, n, w, w + 1, w + 2);
+    CU_TRY(c, cudaGetLastError());
+    j.out->n_launches += 2;
+  }
+  uint32_t h[3] = {0, 0, 0};
+  CU_TRY(c, cudaMemcpyAsync(h, w, 12, cudaMemcpyDeviceToHost, c->stream));
+  CU_TRY(c, cudaStreamSynchronize(c->stream));
+  *largest = h[0];
+  *cut = n - h[2];
+  if (*cut == 0)
+    return fail(c, CMB_E_DECLINED, "%s: the proper-pair records of reference %d do not fit in one decode slice; %s", who, (int32_t)h[0],
+                host_route);
+  if (*cut < n) {
+    CU_TRY(c, cudaMemcpyAsync(next, d.d_rec_off + *cut, 8, cudaMemcpyDeviceToHost, c->stream));
+    CU_TRY(c, cudaStreamSynchronize(c->stream));
+  }
   return CMB_OK;
 }
 
-// cmb_submit_bgzf when the whole-stream buffers do not fit: the stream (a rank's block range in a group) in block slices, each
-// submitted to K1 as one batch at the sample's running interval base -- in pair mode after its mates are matched, and only
-// up to its cut (cmb_slices.hpp).  A decline leaves the sample as cmb_begin_sample left it, for the host decoder.
-int decode_sliced(cmb_ctx* c, const cmb_bgzf_input* in, cmb_bgzf_result* out) {
-  auto& d = c->dec;
-  *out = cmb_bgzf_result{};
-  auto decline = [&](int rc) {
+// An ordinary stream (the whole stream, or a rank's block range in a group) in block slices (decode_in_slices), for the
+// sliced decode (decode_sliced) and the sliced filter (FilterCall::sliced): in `pair` mode each slice is cut (pair_cut), then
+// work(j, r, cut) takes its records [0, cut).
+//   held()  device bytes the caller holds that count as room, since they are reused or freed to grow
+//   events  K1 appends to the sample's event list: the budget keeps room for its growth
+//   other() bytes the last slice needed beside its compressed and inflated bytes (the budget's `side`, per byte of those)
+// CMB_PIPELINE_STATS prints #<stats>_slices.  Every exit releases the decode buffers: what comes next needs the room, and a
+// sliced decode has no resident stream to keep.
+template <class Held, class Other, class Work>
+int stream_in_slices(cmb_ctx* c, const cmb_bgzf_input* in, cmb_bgzf_result* out, SliceStats& ss, const char* who, const char* host_route,
+                     const char* stats, bool pair, bool filter_out, bool events, Held held, Other other, Work work) {
+  auto room = [&] { return device_room(held()); };
+  if (room() < SLICE_MIN_BYTES) {
+    const int rc = fail(c, CMB_E_DECLINED, "%s: not enough device memory for device-side decode", who);
     release_decode(c);
-    if (int e = reset_sample(c)) return e;
     return rc;
-  };
-  // Room for the decode buffers and the sample's event list: the decode buffers held count as room
-  auto room = [&] { return device_room(decode_bytes(c)); };
-  if (room() < SLICE_MIN_BYTES) return decline(fail(c, CMB_E_DECLINED, "cmb_submit_bgzf: not enough device memory for device-side decode"));
-  uint64_t stream_end = 0;  // end of the inflated bytes whose records are walked
+  }
   const uint32_t walk_end = in->ranged ? std::min(in->walk_end_block, in->n_blocks) : in->n_blocks;
+  uint64_t stream_end = 0;  // end of the inflated bytes whose records are walked
   for (uint32_t b = 0; b < walk_end; ++b) stream_end += in->block_isize[b];
   const uint64_t iv0 = c->n_intervals;
-  double side = 0;       // the last slice's other buffers per compressed + inflated byte
-  uint32_t carry = 0;    // pair mode: the largest eligible tid of the slices so far
-  uint64_t cut_records = 0;
+  double side = 0;     // the last slice's other buffers per compressed + inflated byte
+  uint32_t carry = 0;  // pair mode: the largest eligible tid of the slices so far
   auto budget = [&](uint64_t at) -> uint64_t {
     const uint64_t done = at > in->records_at ? at - in->records_at : 0;
     const uint64_t total = stream_end > in->records_at ? stream_end - in->records_at : 0;
-    return decode_slice_budget(room(), !c->gene_mode, c->d_events.bytes(), done, total, c->n_intervals - iv0, side);
+    return decode_slice_budget(room(), events, c->d_events.bytes(), done, total, c->n_intervals - iv0, side);
   };
   auto step = [&](BgzfCall& j, cmb_bgzf_result& r, uint64_t* next) -> int {
     const uint32_t n = (uint32_t)j.n_rec;
-    uint32_t n_sub = n, iv_sub = (uint32_t)j.n_cig;
-    cmb_read_batch tb;
-    carve_batch(d.d_tuple_slab, n, (uint32_t)j.n_cig, &tb);
-    const int32_t* mate = nullptr;
-    uint32_t largest = carry;
+    uint32_t cut = n, largest = carry;
     int rc;
-    if (c->mode.filter_pairs) {
-      // words 12..14 of d_cnt: the slice's largest eligible tid, then the cut's `after` and n - cut (zeroed by copy_inflate)
-      uint32_t* w = d.d_cnt + 12;
-      rc = match_mates(c, d.last_infl_base, n, true, "cmb_submit_bgzf", carry, w);
-      if (rc == CMB_E_NOMEM) return SLICE_HALVE;
-      if (rc) return rc;
-      r.n_launches += 5;
-      if (j.walk_end < walk_end) {  // not the last slice: hold the trailing run of its last eligible tid back for the next one
-        const uint32_t g = (n + 255) / 256;
-        kd_pair_cut_after<<<g, 256, 0, c->stream>>>(d.d_pair_key, tb.tid, n, w, w + 1);
-        kd_pair_cut_at<<<g, 256, 0, c->stream>>>(d.d_pair_key, tb.tid, n, w, w + 1, w + 2);
-        CU_TRY(c, cudaGetLastError());
-        r.n_launches += 2;
-      }
-      uint32_t h[3] = {0, 0, 0};
-      CU_TRY(c, cudaMemcpyAsync(h, w, 12, cudaMemcpyDeviceToHost, c->stream));
-      CU_TRY(c, cudaStreamSynchronize(c->stream));
-      largest = h[0];
-      const uint32_t cut = n - h[2];
-      if (cut == 0)
-        return fail(c, CMB_E_DECLINED, "cmb_submit_bgzf: the proper-pair records of reference %d do not fit in one decode slice; mates are "
-                    "matched on the host", (int32_t)largest);
-      if (cut < n) {  // the next slice starts at record `cut`; its records leave this slice's counters
-        uint64_t off = 0;
-        CU_TRY(c, cudaMemcpyAsync(&off, d.d_rec_off + cut, 8, cudaMemcpyDeviceToHost, c->stream));
-        CU_TRY(c, cudaMemcpyAsync(&iv_sub, tb.iv_begin + cut, 4, cudaMemcpyDeviceToHost, c->stream));
-        CU_TRY(c, cudaMemsetAsync(d.d_cnt + 16, 0, 16, c->stream));
-        kd_count_held<<<(n - cut + 255) / 256, 256, 0, c->stream>>>(tb.tid, tb.flag, cut, n, j.in->own_tid_begin, j.in->own_tid_end, j.in->own_unplaced,
-                                                                   (unsigned long long*)(d.d_cnt + 16), (unsigned long long*)(d.d_cnt + 18));
-        CU_TRY(c, cudaGetLastError());
-        uint64_t held[2] = {0, 0};
-        CU_TRY(c, cudaMemcpyAsync(held, d.d_cnt + 16, 16, cudaMemcpyDeviceToHost, c->stream));
-        CU_TRY(c, cudaStreamSynchronize(c->stream));
-        r.n_primary -= held[0];
-        r.n_records -= held[1];
-        r.n_intervals = iv_sub;
-        r.n_launches += 1;
-        *next = off;
-        n_sub = cut;
-        cut_records += n - cut;
-      }
-      mate = d.d_pair_mate;
+    if (pair) {
+      const auto t0 = std::chrono::steady_clock::now();
+      if ((rc = pair_cut(j, filter_out, carry, j.walk_end >= walk_end, who, host_route, &largest, &cut, next))) return rc;
+      ss.ms_mates += std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count();
     }
-    if (k1_active(c)) {
-      uint32_t excl = 0;
-      if ((rc = j.excl_n(&excl))) return rc;
-      rc = launch_k1(c, tb, n_sub, iv_sub, excl, mate);
-      if (rc == CMB_E_NOMEM) return SLICE_HALVE;  // the event list did not grow: nothing of the slice was accumulated
-      if (rc) return rc;
-    }
+    if ((rc = work(j, r, cut))) return rc;
     carry = largest;
-    uint64_t other = d.d_tuple_slab.bytes() + d.d_rec_off.bytes();
-    if (c->mode.filter_pairs)
-      other += d.d_pair_key.bytes() + d.d_pair_mate.bytes() + d.d_pair_next.bytes() + d.d_pair_tag.bytes() + d.d_pair_head.bytes();
-    side = (double)other / (double)std::max<uint64_t>(1, (j.byte_hi - j.byte_lo) + (j.total - j.u_lo));
+    ss.pair_cut_records += n - cut;
+    side = (double)other() / (double)std::max<uint64_t>(1, (j.byte_hi - j.byte_lo) + (j.total - j.u_lo));
     return CMB_OK;
   };
   auto nomem = [&](const SliceBlocks&, uint32_t, uint32_t, uint64_t) {
-    return fail(c, CMB_E_DECLINED, "cmb_submit_bgzf: not enough device memory for device-side decode");
+    return fail(c, CMB_E_DECLINED, "%s: not enough device memory for device-side decode", who);
+  };
+  const int rc = decode_in_slices(c, in, out, ss, budget, step, nomem);
+  release_decode(c);
+  if (rc) return rc;
+  if (getenv("CMB_PIPELINE_STATS"))
+    fprintf(stderr, "#%s_slices\tslices=%u\tmax_slice_bytes=%llu\thalvings=%u\tpair_cut_records=%llu\n", stats, ss.n_slices,
+            (unsigned long long)ss.max_slice, ss.halvings, (unsigned long long)ss.pair_cut_records);
+  return CMB_OK;
+}
+
+// cmb_submit_bgzf when the whole-stream buffers do not fit: each slice submitted to K1 as one batch at the sample's running
+// interval base, in pair mode only up to its cut.  A decline leaves the sample as cmb_begin_sample left it, for the host decoder.
+int decode_sliced(cmb_ctx* c, const cmb_bgzf_input* in, cmb_bgzf_result* out) {
+  auto& d = c->dec;
+  *out = cmb_bgzf_result{};
+  const bool pair = c->mode.filter_pairs;
+  auto work = [&](BgzfCall& j, cmb_bgzf_result& r, uint32_t cut) -> int {
+    const uint32_t n = (uint32_t)j.n_rec;
+    uint32_t iv_sub = (uint32_t)j.n_cig;
+    cmb_read_batch tb;
+    carve_batch(d.d_tuple_slab, n, (uint32_t)j.n_cig, &tb);
+    if (cut < n) {  // records [cut, n) start the next slice: they leave this slice's counters
+      CU_TRY(c, cudaMemcpyAsync(&iv_sub, tb.iv_begin + cut, 4, cudaMemcpyDeviceToHost, c->stream));
+      CU_TRY(c, cudaMemsetAsync(d.d_cnt + 16, 0, 16, c->stream));
+      kd_count_held<<<(n - cut + 255) / 256, 256, 0, c->stream>>>(tb.tid, tb.flag, cut, n, j.in->own_tid_begin, j.in->own_tid_end, j.in->own_unplaced,
+                                                                 (unsigned long long*)(d.d_cnt + 16), (unsigned long long*)(d.d_cnt + 18));
+      CU_TRY(c, cudaGetLastError());
+      uint64_t held[2] = {0, 0};
+      CU_TRY(c, cudaMemcpyAsync(held, d.d_cnt + 16, 16, cudaMemcpyDeviceToHost, c->stream));
+      CU_TRY(c, cudaStreamSynchronize(c->stream));
+      r.n_primary -= held[0];
+      r.n_records -= held[1];
+      r.n_intervals = iv_sub;
+      r.n_launches += 1;
+    }
+    if (!k1_active(c)) return CMB_OK;
+    uint32_t excl = 0;
+    if (int rc = j.excl_n(&excl)) return rc;
+    const int rc = launch_k1(c, tb, cut, iv_sub, excl, pair ? d.d_pair_mate.p : nullptr);
+    return rc == CMB_E_NOMEM ? SLICE_HALVE : rc;  // the event list did not grow: nothing of the slice was accumulated
   };
   SliceStats ss;
-  const int rc = decode_in_slices(c, in, out, ss, budget, step, nomem);
-  if (rc == CMB_E_DECLINED) return decline(rc);
+  const int rc = stream_in_slices(
+      c, in, out, ss, "cmb_submit_bgzf", "mates are matched on the host", "decode", pair, true, !c->gene_mode, [&] { return decode_bytes(c); },
+      [&] { return d.d_tuple_slab.bytes() + d.d_rec_off.bytes() + (pair ? pair_bytes(c) : 0); }, work);
+  if (rc == CMB_E_DECLINED)
+    if (int e = reset_sample(c)) return e;
   if (rc) return rc;
-  release_decode(c);  // the end of the sample needs the room; a sliced sample has no resident tuples to hand out
   out->ms_copy_inflate = ss.ms_inflate;
   out->ms_chain = ss.ms_chain;
   out->ms_extract = ss.ms_extract;
-  if (getenv("CMB_PIPELINE_STATS"))
-    fprintf(stderr, "#decode_slices\tslices=%u\tmax_slice_bytes=%llu\thalvings=%u\tpair_cut_records=%llu\n", ss.n_slices,
-            (unsigned long long)ss.max_slice, ss.halvings, (unsigned long long)cut_records);
   return CMB_OK;
 }
 
@@ -779,14 +833,44 @@ int bgzf_entry(cmb_ctx* c, const cmb_bgzf_input* in, cmb_bgzf_result* out, bool 
     c->dec.filter_planned = false;
   }
   const auto t_call0 = std::chrono::steady_clock::now();
-  int rc = submit_bgzf_impl(c, in, out, decode_only);
-  if (rc == CMB_E_NOMEM) {
-    release_decode(c);  // give the big buffers back so that the rest of the sample has room
-    // nothing was accumulated: the whole-stream call allocates every buffer before K1
-    rc = decode_only ? fail(c, CMB_E_DECLINED, "cmb_submit_bgzf: not enough device memory for device-side decode") : decode_sliced(c, in, out);
-  }
+  const int rc = whole_or_slices(c, submit_bgzf_impl(c, in, out, decode_only), [&] {
+    return decode_only ? fail(c, CMB_E_DECLINED, "cmb_submit_bgzf: not enough device memory for device-side decode") : decode_sliced(c, in, out);
+  });
   if (out) out->ms_host_wall = (float)std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_call0).count();
   return rc;
+}
+
+// The filter kernels over records [0, n) of the resident decode, its mates matched on the pair path (filter.rs:117-233; else
+// the singles path, filter.rs:88-116): kf_decide, kf_scan, and kf_gather of the *total bytes of the *n_emit returned records
+// into d_filter_out.
+int filter_kernels(cmb_ctx* c, bool pair_path, int inverse, uint32_t n, uint64_t* total, uint64_t* n_emit) {
+  auto& d = c->dec;
+  int rc;
+  if ((rc = d.d_filter_anchor.ensure(c, (size_t)n + 1, with_slack(n))) || (rc = d.d_filter_role.ensure(c, (size_t)n + 1, with_slack(n))))
+    return rc;
+  cmb_read_batch tb;
+  carve_batch(d.d_tuple_slab, d.last_n_rec, d.last_n_cig, &tb);
+  FilterArgs a{};
+  a.data = d.last_infl_base; a.rec_off = d.d_rec_off; a.n = n; a.flag = tb.flag; a.mapq = tb.mapq; a.nm_state = tb.nm_state; a.nm = tb.nm;
+  a.l_seq = tb.l_seq; a.aligned = tb.aligned; a.del = tb.del; a.mate = pair_path ? d.last_mate : nullptr; a.p = c->params;
+  a.filter_single = c->mode.filter_single_reads; a.pair_path = pair_path; a.filter_out = inverse ? 0 : 1;
+  a.anchor_bytes = d.d_filter_anchor; a.role = d.d_filter_role; a.error_flags = d.d_cnt + 12; a.n_emit = (unsigned long long*)(d.d_cnt + 14);
+  CU_TRY(c, cudaMemsetAsync(d.d_cnt + 12, 0, 16, c->stream));
+  kf_decide<<<(n + 255) / 256, 256, 0, c->stream>>>(a);
+  kf_scan<<<1, 1024, 0, c->stream>>>(d.d_filter_anchor, n);
+  CU_TRY(c, cudaGetLastError());
+  uint32_t h[4];
+  CU_TRY(c, cudaMemcpyAsync(h, d.d_cnt + 12, 16, cudaMemcpyDeviceToHost, c->stream));
+  CU_TRY(c, cudaMemcpyAsync(total, d.d_filter_anchor + n, 8, cudaMemcpyDeviceToHost, c->stream));
+  CU_TRY(c, cudaStreamSynchronize(c->stream));
+  if (h[0] & ERR_NM) return fail(c, CMB_E_NM, "%s", NM_PANIC);
+  memcpy(n_emit, h + 2, 8);
+  if (!*total) return CMB_OK;
+  if ((rc = d.d_filter_out.ensure(c, *total, (size_t)*total + (size_t)*total / 8 + 4096))) return rc;
+  a.out = d.d_filter_out;
+  kf_gather<<<(n + 7) / 8, 256, 0, c->stream>>>(a);
+  CU_TRY(c, cudaGetLastError());
+  return CMB_OK;
 }
 }  // namespace
 
@@ -822,31 +906,8 @@ extern "C" int cmb_filter_plan(cmb_ctx* c, int inverse, uint64_t* n_records, uin
   const bool pair_path = !(c->mode.filter_single_reads && !c->mode.filter_pairs);
   int rc;
   if (pair_path && (rc = match_mates(c, d.last_infl_base, n, !inverse, "cmb_filter_plan"))) return rc;
-  if ((rc = d.d_filter_anchor.ensure(c, (size_t)n + 1, with_slack(n))) || (rc = d.d_filter_role.ensure(c, (size_t)n + 1, with_slack(n))))
-    return rc;
-  cmb_read_batch tb;
-  carve_batch(d.d_tuple_slab, d.last_n_rec, d.last_n_cig, &tb);
-  FilterArgs a{};
-  a.data = d.last_infl_base; a.rec_off = d.d_rec_off; a.n = n; a.flag = tb.flag; a.mapq = tb.mapq; a.nm_state = tb.nm_state; a.nm = tb.nm;
-  a.l_seq = tb.l_seq; a.aligned = tb.aligned; a.del = tb.del; a.mate = pair_path ? d.last_mate : nullptr; a.p = c->params;
-  a.filter_single = c->mode.filter_single_reads; a.pair_path = pair_path; a.filter_out = inverse ? 0 : 1;
-  a.anchor_bytes = d.d_filter_anchor; a.role = d.d_filter_role; a.error_flags = d.d_cnt + 12; a.n_emit = (unsigned long long*)(d.d_cnt + 14);
-  CU_TRY(c, cudaMemsetAsync(d.d_cnt + 12, 0, 16, c->stream));
-  kf_decide<<<(n + 255) / 256, 256, 0, c->stream>>>(a);
-  kf_scan<<<1, 1024, 0, c->stream>>>(d.d_filter_anchor, n);
-  CU_TRY(c, cudaGetLastError());
-  uint32_t h[4];
-  unsigned long long total = 0;
-  CU_TRY(c, cudaMemcpyAsync(h, d.d_cnt + 12, 16, cudaMemcpyDeviceToHost, c->stream));
-  CU_TRY(c, cudaMemcpyAsync(&total, d.d_filter_anchor + n, 8, cudaMemcpyDeviceToHost, c->stream));
-  CU_TRY(c, cudaStreamSynchronize(c->stream));
-  if (h[0] & ERR_NM) return fail(c, CMB_E_NM, "%s", NM_PANIC);
-  unsigned long long n_emit;
-  memcpy(&n_emit, h + 2, 8);
-  if ((rc = d.d_filter_out.ensure(c, total, (size_t)total + (size_t)total / 8 + 4096))) return rc;
-  a.out = d.d_filter_out;
-  kf_gather<<<(n + 7) / 8, 256, 0, c->stream>>>(a);
-  CU_TRY(c, cudaGetLastError());
+  uint64_t total = 0, n_emit = 0;
+  if ((rc = filter_kernels(c, pair_path, inverse, n, &total, &n_emit))) return rc;
   d.filter_bytes = total;
   d.filter_planned = true;
   *n_records = n_emit;
@@ -881,39 +942,15 @@ struct FilterCall {
   cmb_filter_result* out;
   bool pair_path;  // filter.rs:117-233 (mates matched), else the singles path (filter.rs:88-116)
 
-  // The filter kernels over records [0, n) of the last decode (its mates matched on the pair path), then the returned records
-  // to the sink in pieces of at most FILTER_PIECE_BYTES, each through the next staging buffer.  Every allocation comes before
-  // the first sink call: CMB_E_NOMEM means nothing was handed over.
+  // filter_kernels over records [0, n) of the last decode (its mates matched on the pair path), then the returned records to
+  // the sink in pieces of at most FILTER_PIECE_BYTES, each through the next staging buffer.  Every allocation comes before the
+  // first sink call: CMB_E_NOMEM means nothing was handed over.
   int filter(uint32_t n) {
     auto& d = c->dec;
     const auto t0 = Clock::now();
+    uint64_t total = 0, n_emit = 0;
     int rc;
-    if ((rc = d.d_filter_anchor.ensure(c, (size_t)n + 1, with_slack(n))) || (rc = d.d_filter_role.ensure(c, (size_t)n + 1, with_slack(n))))
-      return rc;
-    cmb_read_batch tb;
-    carve_batch(d.d_tuple_slab, d.last_n_rec, d.last_n_cig, &tb);
-    FilterArgs a{};
-    a.data = d.last_infl_base; a.rec_off = d.d_rec_off; a.n = n; a.flag = tb.flag; a.mapq = tb.mapq; a.nm_state = tb.nm_state; a.nm = tb.nm;
-    a.l_seq = tb.l_seq; a.aligned = tb.aligned; a.del = tb.del; a.mate = pair_path ? d.last_mate : nullptr; a.p = c->params;
-    a.filter_single = c->mode.filter_single_reads; a.pair_path = pair_path; a.filter_out = inverse ? 0 : 1;
-    a.anchor_bytes = d.d_filter_anchor; a.role = d.d_filter_role; a.error_flags = d.d_cnt + 12; a.n_emit = (unsigned long long*)(d.d_cnt + 14);
-    CU_TRY(c, cudaMemsetAsync(d.d_cnt + 12, 0, 16, c->stream));
-    kf_decide<<<(n + 255) / 256, 256, 0, c->stream>>>(a);
-    kf_scan<<<1, 1024, 0, c->stream>>>(d.d_filter_anchor, n);
-    CU_TRY(c, cudaGetLastError());
-    uint32_t h[4];
-    unsigned long long total = 0, n_emit = 0;
-    CU_TRY(c, cudaMemcpyAsync(h, d.d_cnt + 12, 16, cudaMemcpyDeviceToHost, c->stream));
-    CU_TRY(c, cudaMemcpyAsync(&total, d.d_filter_anchor + n, 8, cudaMemcpyDeviceToHost, c->stream));
-    CU_TRY(c, cudaStreamSynchronize(c->stream));
-    if (h[0] & ERR_NM) return fail(c, CMB_E_NM, "%s", NM_PANIC);
-    memcpy(&n_emit, h + 2, 8);
-    if (total) {
-      if ((rc = d.d_filter_out.ensure(c, total, (size_t)total + (size_t)total / 8 + 4096))) return rc;
-      a.out = d.d_filter_out;
-      kf_gather<<<(n + 7) / 8, 256, 0, c->stream>>>(a);
-      CU_TRY(c, cudaGetLastError());
-    }
+    if ((rc = filter_kernels(c, pair_path, inverse, n, &total, &n_emit))) return rc;
     CU_TRY(c, cudaStreamSynchronize(c->stream));
     out->ms_filter += (float)ms_since(t0);
     if (!total) return CMB_OK;
@@ -939,9 +976,7 @@ struct FilterCall {
   // Device bytes the filter holds beside the decode buffers: they count as room, since they are reused or freed to grow
   uint64_t held() const {
     const auto& d = c->dec;
-    uint64_t b = decode_bytes(c) + d.d_filter_anchor.bytes() + d.d_filter_role.bytes() + d.d_filter_out.bytes();
-    if (pair_path) b += d.d_pair_key.bytes() + d.d_pair_mate.bytes() + d.d_pair_next.bytes() + d.d_pair_tag.bytes() + d.d_pair_head.bytes();
-    return b;
+    return decode_bytes(c) + d.d_filter_anchor.bytes() + d.d_filter_role.bytes() + d.d_filter_out.bytes() + (pair_path ? pair_bytes(c) : 0);
   }
   void release_filter() {
     auto& d = c->dec;
@@ -965,92 +1000,32 @@ struct FilterCall {
       out->ms_filter += (float)ms_since(t0);
       if (!rc && n) rc = filter(n);
     }
-    if (rc != CMB_E_NOMEM) return rc;
-    release_filter();  // nothing was handed over: every buffer is allocated before the sink call
-    release_decode(c);
-    return sliced(in);
+    return whole_or_slices(c, rc, [&] {
+      release_filter();
+      return sliced(in);
+    });
   }
 
-  // The stream in block slices (decode_in_slices), each filtered up to its cut and handed to the sink
+  // The stream in block slices, each filtered up to its cut and handed to the sink
   int sliced(const cmb_bgzf_input* in) {
     auto& d = c->dec;
-    auto decline = [&](int rc) {
-      release_decode(c);
-      return rc;
-    };
-    auto room = [&] { return device_room(held()); };
-    if (room() < SLICE_MIN_BYTES) return decline(fail(c, CMB_E_DECLINED, "cmb_filter_bgzf: not enough device memory for device-side decode"));
-    uint64_t stream_end = 0;
-    for (uint32_t b = 0; b < in->n_blocks; ++b) stream_end += in->block_isize[b];
-    double side = 0;     // the last slice's other buffers per compressed + inflated byte
-    uint32_t carry = 0;  // pair path: the largest eligible tid of the slices so far
-    auto budget = [&](uint64_t at) -> uint64_t {
-      const uint64_t done = at > in->records_at ? at - in->records_at : 0;
-      const uint64_t total = stream_end > in->records_at ? stream_end - in->records_at : 0;
-      return decode_slice_budget(room(), false, 0, done, total, 0, side);
-    };
-    auto step = [&](BgzfCall& j, cmb_bgzf_result&, uint64_t* next) -> int {
-      const uint32_t n = (uint32_t)j.n_rec;
-      uint32_t cut = n, largest = carry;
-      uint64_t held_back = 0;
-      int rc;
-      const auto t0 = Clock::now();
-      if (pair_path) {
-        // words 12..14 of d_cnt: the slice's largest eligible tid, then the cut's `after` and n - cut (zeroed by copy_inflate)
-        uint32_t* w = d.d_cnt + 12;
-        rc = match_mates(c, d.last_infl_base, n, !inverse, "cmb_filter_bgzf", carry, w);
-        if (rc == CMB_E_NOMEM) return SLICE_HALVE;
-        if (rc) return rc;
-        if (j.walk_end < in->n_blocks) {  // not the last slice: hold the trailing run of its last eligible tid back for the next one
-          cmb_read_batch tb;
-          carve_batch(d.d_tuple_slab, n, (uint32_t)j.n_cig, &tb);
-          const uint32_t g = (n + 255) / 256;
-          kd_pair_cut_after<<<g, 256, 0, c->stream>>>(d.d_pair_key, tb.tid, n, w, w + 1);
-          kd_pair_cut_at<<<g, 256, 0, c->stream>>>(d.d_pair_key, tb.tid, n, w, w + 1, w + 2);
-          CU_TRY(c, cudaGetLastError());
-        }
-        uint32_t h[3] = {0, 0, 0};
-        CU_TRY(c, cudaMemcpyAsync(h, w, 12, cudaMemcpyDeviceToHost, c->stream));
-        CU_TRY(c, cudaStreamSynchronize(c->stream));
-        largest = h[0];
-        cut = n - h[2];
-        if (cut == 0)
-          return fail(c, CMB_E_DECLINED, "cmb_filter_bgzf: the proper-pair records of reference %d do not fit in one decode slice; the "
-                      "filter runs on the host", (int32_t)largest);
-        if (cut < n) {  // the next slice starts at record `cut`
-          uint64_t off = 0;
-          CU_TRY(c, cudaMemcpy(&off, d.d_rec_off + cut, 8, cudaMemcpyDeviceToHost));
-          *next = off;
-          held_back = n - cut;
-        }
-      }
-      out->ms_filter += (float)ms_since(t0);
-      rc = filter(cut);
-      if (rc == CMB_E_NOMEM) {
-        release_filter();
-        return SLICE_HALVE;
-      }
-      if (rc) return rc;
-      carry = largest;
-      out->pair_cut_records += held_back;
-      const uint64_t other = held() - d.d_comp.bytes() - d.d_inflated.bytes();
-      side = (double)other / (double)std::max<uint64_t>(1, (j.byte_hi - j.byte_lo) + (j.total - j.u_lo));
-      return CMB_OK;
-    };
-    auto nomem = [&](const SliceBlocks&, uint32_t, uint32_t, uint64_t) {
-      return fail(c, CMB_E_DECLINED, "cmb_filter_bgzf: not enough device memory for device-side decode");
+    auto work = [&](BgzfCall&, cmb_bgzf_result&, uint32_t cut) {
+      const int rc = filter(cut);
+      if (rc != CMB_E_NOMEM) return rc;
+      release_filter();
+      return SLICE_HALVE;
     };
     SliceStats ss;
     cmb_bgzf_result r{};
-    const int rc = decode_in_slices(c, in, &r, ss, budget, step, nomem);
-    release_decode(c);  // the next input needs the room; a sliced decode has no resident stream to keep
+    const int rc = stream_in_slices(
+        c, in, &r, ss, "cmb_filter_bgzf", "the filter runs on the host", "filter", pair_path, !inverse, false, [&] { return held(); },
+        [&] { return held() - d.d_comp.bytes() - d.d_inflated.bytes(); }, work);
     out->n_slices = ss.n_slices;  // on a decline: the slices handed over before it
     out->halvings = ss.halvings;
+    out->pair_cut_records = ss.pair_cut_records;
+    out->ms_filter += ss.ms_mates;
     if (rc) return rc;
     out->ms_decode = ss.ms_inflate + ss.ms_chain + ss.ms_extract;
-    if (getenv("CMB_PIPELINE_STATS"))
-      fprintf(stderr, "#filter_slices\tslices=%u\tmax_slice_bytes=%llu\thalvings=%u\tpair_cut_records=%llu\n", ss.n_slices,
-              (unsigned long long)ss.max_slice, ss.halvings, (unsigned long long)out->pair_cut_records);
     return CMB_OK;
   }
 };

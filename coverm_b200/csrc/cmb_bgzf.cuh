@@ -1,7 +1,7 @@
 // The device decode as the rest of the library drives it (cmb_bgzf.cu): one staged decode call (BgzfCall), the memory its
-// buffers take, and the loop that decodes a stream in block slices.  Ordinary streams that do not fit (decode_sliced), `coverm
-// filter` over such a stream (cmb_filter_bgzf) and the shards of sharded input (decode_shard, cmb_shard_input.cu) each drive
-// that loop with their own budget and per-slice step.
+// buffers take, and the loop that decodes a stream in block slices.  An ordinary stream that does not fit goes through that
+// loop by one driver in cmb_bgzf.cu (stream_in_slices), decoded for K1 (decode_sliced) or filtered for `coverm filter`
+// (cmb_filter_bgzf); the shards of sharded input (decode_shard, cmb_shard_input.cu) drive it with their own budget and step.
 #pragma once
 #include <algorithm>
 #include <climits>
@@ -43,11 +43,13 @@ struct BgzfCall {
   bool tail_short = false;               // ranged: a record runs past the tail (a longer tail may decode it)
   uint64_t exit_off = 0;                 // end of the last record that starts in the range: the next range's records_at
 
+  int run();  // prepare, then the four stages unless there is nothing to decode
   int prepare();
   int copy_inflate();
   int declined();
   int chain();
   int extract();
+  int stage_times();  // waits for the extract; out's ms_copy_inflate, ms_chain, ms_extract and ms_total from the stage events
   int excl_n(uint32_t* n);
 };
 
@@ -77,6 +79,8 @@ struct SliceStats {
   uint32_t halvings = 0;  // over the whole decode
   uint64_t max_slice = 0;  // compressed + inflated bytes of the largest slice
   float ms_inflate = 0, ms_chain = 0, ms_extract = 0;
+  uint64_t pair_cut_records = 0;  // pair mode (stream_in_slices): records held back at the ends of the slices
+  float ms_mates = 0;             // pair mode (stream_in_slices): host clock of mate matching and the cuts
 };
 constexpr int SLICE_HALVE = 1;  // a slice step's verdict: a buffer of the slice did not fit, halve it
 constexpr int SLICE_AGAIN = 2;  // a slice step's verdict: decode the same slice again (the step released the decode buffers)
@@ -113,16 +117,11 @@ int decode_in_slices(cmb_ctx* c, const cmb_bgzf_input* in, cmb_bgzf_result* out,
     cmb_bgzf_result r{};
     BgzfCall j{c, d, &si, &r, true, nb};
     j.tail_bytes = tail;
-    int rc = j.prepare();
-    if (!rc && !j.nothing_to_decode && !(rc = j.copy_inflate()) && !(rc = j.declined()) && !(rc = j.chain())) rc = j.extract();
+    int rc = j.run();
     if (rc == CMB_E_NOMEM) rc = SLICE_HALVE;
     uint64_t next = j.exit_off;
     if (!rc && !j.nothing_to_decode) {
-      CU_TRY(c, cudaEventSynchronize(d.ev[4]));
-      cudaEventElapsedTime(&r.ms_total, d.ev[0], d.ev[4]);
-      cudaEventElapsedTime(&r.ms_copy_inflate, d.ev[0], d.ev[2]);
-      cudaEventElapsedTime(&r.ms_chain, d.ev[2], d.ev[3]);
-      cudaEventElapsedTime(&r.ms_extract, d.ev[3], d.ev[4]);
+      if (int e = j.stage_times()) return e;
       if (!j.n_rec || j.exit_off <= at) return fail(c, CMB_E_DECLINED, "the slice from block %u decoded no record", b0);
       rc = step(j, r, &next);
     }

@@ -199,7 +199,7 @@ struct cmb_ctx {
     Buf<uint32_t> d_block_window;
     PinnedBuf<uint32_t> h_ones;  // source of the arrival flags
     Buf<uint32_t> d_cnt;  // 20 words: [0] inflate failures [1] decode error bits [2] chain changed [4..5] n_primary [6..9] totals
-                          // [10..11] n_owned; sliced decode: [12..14] pair cut (decode_sliced), [16..19] held-back counts
+                          // [10..11] n_owned; sliced decode: [12..14] pair cut (pair_cut), [16..19] held-back counts
     Buf<uint64_t> d_rec_off;
     Buf<uint8_t> d_tuple_slab;
     uint32_t last_n_rec = 0, last_n_cig = 0;  // tuples of the last successful cmb_submit_bgzf (cmb_last_bgzf_batch)
