@@ -104,6 +104,7 @@ class HostResult(C.Structure):
 DEVICE_SYMBOLS = ["cmb_abi_version", "cmb_create", "cmb_destroy", "cmb_last_error", "cmb_set_reference",
                   "cmb_set_params", "cmb_begin_sample", "cmb_acquire_batch", "cmb_submit_batch",
                   "cmb_submit_device_batch", "cmb_submit_bgzf", "cmb_decode_bgzf", "cmb_filter_plan", "cmb_filter_fetch", "cmb_filter_bgzf", "cmb_set_genes",
+                  "cmb_deflate_begin", "cmb_deflate_feed", "cmb_deflate_finish", "cmb_filter_bgzf_deflate",
                   "cmb_set_genes_range", "cmb_fetch_gene_extras", "cmb_grow_buffers", "cmb_last_bgzf_batch", "cmb_end_sample", "cmb_comm_unique_id",
                   "cmb_comm_init", "cmb_comm_init_local", "cmb_comm_destroy", "cmb_comm_allgather", "cmb_allgather_stats", "cmb_kept_tid_range", "cmb_fetch_pairs", "cmb_end_sample_device",
                   "cmb_get_timing", "cmb_stream", "cmb_host_alloc", "cmb_host_free", "cmb_nvtx_push", "cmb_nvtx_pop",

@@ -941,6 +941,7 @@ struct FilterCall {
   void* user;
   cmb_filter_result* out;
   bool pair_path;  // filter.rs:117-233 (mates matched), else the singles path (filter.rs:88-116)
+  bool deflate;    // the returned records to the deflate stream (cmb_filter_bgzf_deflate), not to the staging buffers
 
   // filter_kernels over records [0, n) of the last decode (its mates matched on the pair path), then the returned records to
   // the sink in pieces of at most FILTER_PIECE_BYTES, each through the next staging buffer.  Every allocation comes before the
@@ -954,6 +955,12 @@ struct FilterCall {
     CU_TRY(c, cudaStreamSynchronize(c->stream));
     out->ms_filter += (float)ms_since(t0);
     if (!total) return CMB_OK;
+    if (deflate) {  // cmb_filter_bgzf_deflate: the records go to the context's deflate stream from device memory
+      if ((rc = deflate_feed_device(c, d.d_filter_out, total, sink, user, &out->n_sink_calls))) return rc;
+      out->n_bytes += total;
+      out->n_records += n_emit;
+      return CMB_OK;
+    }
     // Both staging buffers have their fixed size once allocated, so that none is freed while the caller still reads it
     for (auto& stage : d.filter_stage)
       if ((rc = stage.ensure(c, FILTER_PIECE_BYTES))) return rc;
@@ -1032,13 +1039,26 @@ struct FilterCall {
 
 }  // namespace
 
-extern "C" int cmb_filter_bgzf(cmb_ctx* c, const cmb_bgzf_input* in, int inverse, cmb_filter_sink sink, void* user, cmb_filter_result* out) {
-  NvtxRange nvtx("cmb_filter_bgzf");
+namespace {
+int filter_entry(cmb_ctx* c, const cmb_bgzf_input* in, int inverse, cmb_filter_sink sink, void* user, cmb_filter_result* out, bool deflate) {
   if (!c || !in || !sink || !out) return fail(c, CMB_E_ARG, "cmb_filter_bgzf: null argument");
   *out = cmb_filter_result{};
   if (!c->have_params || c->in_sample) return fail(c, CMB_E_ARG, "cmb_filter_bgzf: set the parameters first; not inside a sample");
   if (c->n_acquired) return fail(c, CMB_E_ARG, "cmb_filter_bgzf: a staging batch is still acquired");
+  if (deflate && !c->dfl.active) return fail(c, CMB_E_ARG, "cmb_filter_bgzf_deflate: no stream begun (cmb_deflate_begin first)");
   CU_TRY(c, cudaSetDevice(c->device));
-  FilterCall f{c, inverse, sink, user, out, !(c->mode.filter_single_reads && !c->mode.filter_pairs)};
+  FilterCall f{c, inverse, sink, user, out, !(c->mode.filter_single_reads && !c->mode.filter_pairs), deflate};
   return f.whole(in);
+}
+}  // namespace
+
+extern "C" int cmb_filter_bgzf(cmb_ctx* c, const cmb_bgzf_input* in, int inverse, cmb_filter_sink sink, void* user, cmb_filter_result* out) {
+  NvtxRange nvtx("cmb_filter_bgzf");
+  return filter_entry(c, in, inverse, sink, user, out, false);
+}
+
+extern "C" int cmb_filter_bgzf_deflate(cmb_ctx* c, const cmb_bgzf_input* in, int inverse, cmb_filter_sink sink, void* user,
+                                       cmb_filter_result* out) {
+  NvtxRange nvtx("cmb_filter_bgzf_deflate");
+  return filter_entry(c, in, inverse, sink, user, out, true);
 }

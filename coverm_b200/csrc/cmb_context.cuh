@@ -270,6 +270,23 @@ struct cmb_ctx {
     cudaEvent_t ev[4]{};
     float ms_choose = 0, ms_decode = 0;
   } sh;
+  // the BGZF output stream deflated on the device (cmb_deflate_*; cmb_deflate.cu); buffers allocated by cmb_deflate_begin
+  struct Deflate {
+    Buf<uint8_t> d_raw;     // the stream's bytes not yet deflated: the carry (< one block) first, then what a feed appends
+    Buf<uint8_t> d_blocks;  // one DFL_MAX_OUT slot per block of the piece
+    Buf<uint32_t> d_size;   // per block: its BGZF size | DFL_STORED_FLAG when stored
+    Buf<uint8_t> d_packed;  // the piece's blocks back to back
+    PinnedBuf<uint8_t> stage[2];  // sink call k's bytes are in stage[k & 1]
+    PinnedBuf<uint32_t> h_size;
+    uint64_t carry = 0;
+    bool active = false;
+    cmb_deflate_stats stats{};
+    cudaEvent_t ev[2]{};
+    ~Deflate() {
+      for (auto e : ev)
+        if (e) cudaEventDestroy(e);
+    }
+  } dfl;
 };
 #pragma GCC diagnostic pop
 
@@ -370,6 +387,9 @@ int reset_sample(cmb_ctx* c);
 // decode passes the largest eligible tid of the slices before it (`carry`) and gets its own largest in *largest (device).
 int match_mates(cmb_ctx* c, const uint8_t* infl_base, uint32_t n_rec, bool filter_out, const char* who, uint32_t carry = 0,
                 uint32_t* largest = nullptr);
+// cmb_deflate.cu: d_src[0, n) (device memory) fed to the context's deflate stream, as cmb_deflate_feed feeds host bytes;
+// *n_calls counts the sink calls made
+int deflate_feed_device(cmb_ctx* c, const uint8_t* d_src, uint64_t n, cmb_filter_sink sink, void* user, uint32_t* n_calls);
 // kf_scan (cmb_filter.cuh) on the context stream: v[0, n) exclusively scanned in place, v[n] = the total
 void launch_scan(cmb_ctx* c, unsigned long long* v, uint32_t n);
 

@@ -356,49 +356,7 @@ __device__ uint32_t inf_block(InfWarpSmem& S, const uint8_t* in, uint32_t in_len
   return INF_OK;
 }
 
-// ---- CRC-32 (ISO-HDLC, the gzip/BGZF checksum; reflected polynomial 0xEDB88320) of a block's output, by the whole warp:
-// every lane checksums a 2 KB slice with slicing-by-4 tables, then the slices are combined through the linearity of the
-// CRC: crc(A||B) = crc(A) * x^(8|B|) mod P  xor  crc(B)  (polynomial arithmetic over GF(2), bit 31 = x^0).
-constexpr uint32_t CRC_POLY = 0xedb88320u;
-constexpr uint32_t CRC_SLICE = 2048;
-constexpr uint32_t INF_CRC_TABLE_BYTES = 4 * 256 * 4;
-
-__device__ __forceinline__ uint32_t gf2_mulmod(uint32_t a, uint32_t b) {  // a(x) * b(x) mod P(x)
-  uint32_t p = 0;
-  for (uint32_t m = 1u << 31; m; m >>= 1) {
-    if (a & m) p ^= b;
-    b = (b & 1) ? (b >> 1) ^ CRC_POLY : b >> 1;
-  }
-  return p;
-}
-__device__ uint32_t gf2_x_pow_8n(uint32_t n_bytes) {  // x^(8 n) mod P by square and multiply
-  uint32_t sq = 0x00800000u;  // x^8: x^0 is bit 31, x^k is bit 31-k
-  uint32_t r = 1u << 31;
-  while (n_bytes) {
-    if (n_bytes & 1) r = gf2_mulmod(sq, r);
-    sq = gf2_mulmod(sq, sq);
-    n_bytes >>= 1;
-  }
-  return r;
-}
-__device__ uint32_t warp_crc32(const uint8_t* data, uint32_t n, const uint32_t* T, uint32_t lane) {
-  const uint32_t b0 = min(n, lane * CRC_SLICE), b1 = min(n, (lane + 1) * CRC_SLICE);
-  uint32_t c = 0;
-  if (b1 > b0) {
-    const uint8_t* p = data + b0;
-    const uint8_t* e = data + b1;
-    c = 0xffffffffu;
-    while (p < e && ((uintptr_t)p & 3)) c = T[(c ^ __ldcg(p++)) & 0xff] ^ (c >> 8);
-    for (; p + 4 <= e; p += 4) {
-      c ^= __ldcg(reinterpret_cast<const uint32_t*>(p));
-      c = T[768 + (c & 0xff)] ^ T[512 + ((c >> 8) & 0xff)] ^ T[256 + ((c >> 16) & 0xff)] ^ T[c >> 24];
-    }
-    while (p < e) c = T[(c ^ __ldcg(p++)) & 0xff] ^ (c >> 8);
-    c = ~c;
-    c = gf2_mulmod(gf2_x_pow_8n(n - b1), c);
-  }
-  return __reduce_xor_sync(FULL, c);
-}
+#include "cmb_crc32.cuh"
 
 __global__ void __launch_bounds__(INF_WARPS * 32, 2) kd_inflate(const InflateArgs a) {
   extern __shared__ __align__(16) uint8_t inf_smem[];

@@ -27,6 +27,7 @@ struct CliOptions {
   std::string sub;
   std::vector<std::string> bam_files, methods, output_bam_files;
   bool inverse = false;
+  bool device_deflate = false;  // `filter --device-deflate`: the output BAM compressed on the GPU (cmb_deflate_*)
   std::optional<uint32_t> min_read_aligned_length, min_read_aligned_length_pair;
   std::optional<float> min_read_percent_identity, min_read_aligned_percent, min_read_percent_identity_pair,
       min_read_aligned_percent_pair;
@@ -90,6 +91,7 @@ inline CliOptions parse_cli(const std::vector<std::string>& args) {
     if (a == "-b" || a == "--bam-files") list = &o.bam_files;
     else if (filter_sub && (a == "-o" || a == "--output-bam-files")) list = &o.output_bam_files;
     else if (filter_sub && a == "--inverse") o.inverse = true;
+    else if (o.sub == "filter" && a == "--device-deflate") o.device_deflate = true;
     else if (a == "-m" || a == "--methods" || a == "--method") {
       if (!methods_given) o.methods.clear();
       methods_given = true;
@@ -395,6 +397,16 @@ inline CliResult run_cli_rank(const std::vector<std::string>& args, const std::v
           const FilterRun run = filter_one_input(*session, in, fp, o.inverse, names);
           if (o.timing) err << "#filter\tsample=" << k << "\trecords_out=" << run.n_records << "\tdevice=" << (run.on_device ? 1 : 0) << '\n';
           for (size_t off = 0; off + 4 <= names.bytes.size(); off += 4 + (size_t)rd_u32(names.bytes.data() + off)) out << bam_qname(names.bytes.data() + off) << '\n';
+        } else if (o.device_deflate) {
+          DeviceDeflateBamSink bam(o.output_bam_files[k], session->ctx());
+          const FilterRun run = filter_one_input(*session, in, fp, o.inverse, bam);
+          if (o.timing) {
+            const cmb_deflate_stats& z = bam.stats();
+            err << "#filter\tsample=" << k << "\trecords_out=" << run.n_records << "\tdevice=" << (run.on_device ? 1 : 0) << '\n';
+            err << "#deflate\tsample=" << k << "\traw_bytes=" << z.raw_bytes << "\tbgzf_bytes=" << z.bgzf_bytes << "\tblocks=" << z.blocks
+                << "\tstored_blocks=" << z.stored_blocks << "\tsink_calls=" << z.sink_calls << "\tdeflate_ms=" << z.ms_deflate
+                << "\td2h_ms=" << z.ms_d2h << '\n';
+          }
         } else {
           BamFileSink bam(o.output_bam_files[k], session->pool());
           const FilterRun run = filter_one_input(*session, in, fp, o.inverse, bam);

@@ -3,7 +3,8 @@
 //
 // Fast path: the sample is decoded on the GPU (cmb_filter_bgzf: whole, or in block slices when it does not fit), the device
 // decides and orders the returned records (cmb_filter.cuh) and hands their bytes back piece by piece; this file compresses and
-// writes each piece while the device works on the next (BgzfWriter).  Fallback (SAM / uncompressed input, a stream the device
+// writes each piece while the device works on the next (BgzfWriter).  With --device-deflate the records are compressed on the
+// device instead (cmb_filter_bgzf_deflate) and only BGZF bytes come back; the host loop's output goes through the same encoder.  Fallback (SAM / uncompressed input, a stream the device
 // declines): filter_on_host below runs the reference's loop on the host.
 // `filter-names` prints the returned records' names instead of writing a BAM: the form in which the reference's unit tests
 // (filter.rs:342-844) state their expectations.
@@ -11,6 +12,7 @@
 #include <cstdio>
 #include <exception>
 #include <fstream>
+#include <utility>
 
 #include "bgzf_writer.hpp"
 #include "sample_processor.hpp"
@@ -19,6 +21,11 @@
 // where every input takes the host loop.  libcoverm_b200 always defines it.
 extern "C" int cmb_filter_bgzf(cmb_ctx* ctx, const cmb_bgzf_input* in, int inverse, cmb_filter_sink sink, void* user,
                                cmb_filter_result* out) __attribute__((weak));
+extern "C" int cmb_filter_bgzf_deflate(cmb_ctx* ctx, const cmb_bgzf_input* in, int inverse, cmb_filter_sink sink, void* user,
+                                       cmb_filter_result* out) __attribute__((weak));
+extern "C" int cmb_deflate_begin(cmb_ctx* ctx) __attribute__((weak));
+extern "C" int cmb_deflate_feed(cmb_ctx* ctx, const uint8_t* bytes, uint64_t n_bytes, cmb_filter_sink sink, void* user) __attribute__((weak));
+extern "C" int cmb_deflate_finish(cmb_ctx* ctx, cmb_filter_sink sink, void* user, cmb_deflate_stats* stats) __attribute__((weak));
 
 namespace cmbh {
 
@@ -100,6 +107,10 @@ struct FilterSink {
   // read after this returns.  Does not throw.
   virtual void restart() noexcept = 0;
   virtual void finish() = 0;  // the input is done: nothing of it is still being written after this returns
+  // true: the sink's BGZF stream is the device's (cmb_deflate_*), and the device path hands it compressed bytes through
+  // compressed() instead of records through records()
+  virtual bool device_deflate() const { return false; }
+  virtual void compressed(const uint8_t*, size_t) {}
 };
 
 // `coverm filter`'s output BAM, compressed and written while the device works.  The file is created by the first piece and
@@ -143,6 +154,75 @@ class BamFileSink : public FilterSink {
   bool created_ = false, done_ = false;
 };
 
+// `coverm filter --device-deflate`'s output BAM: the header and the host loop's records are fed to the context's deflate
+// stream, the device path's records reach it on the device, and the stream's BGZF bytes are written as they arrive.  Restarting
+// truncates the file and begins the stream again.  Like BamFileSink, it leaves no file unless finish() is reached.
+class DeviceDeflateBamSink : public FilterSink {
+ public:
+  DeviceDeflateBamSink(std::string path, cmb_ctx* ctx) : path_(std::move(path)), ctx_(ctx) {
+    if (!cmb_deflate_begin || !cmb_deflate_feed || !cmb_deflate_finish || !cmb_filter_bgzf_deflate)
+      throw ExitError(1, "--device-deflate: this build of the device library has no deflate encoder");
+  }
+  ~DeviceDeflateBamSink() override {
+    if (done_ || !created_) return;
+    if (file_.is_open()) file_.close();
+    std::remove(path_.c_str());
+  }
+  void header(const uint8_t* p, size_t n) override { feed(p, n); }
+  void records(const uint8_t* p, size_t n) override { feed(p, n); }
+  void compressed(const uint8_t* p, size_t n) override {
+    open();
+    file_.write((const char*)p, (std::streamsize)n);
+    if (!file_) throw Panic("Failed to write BAM record");
+  }
+  void restart() noexcept override {
+    if (file_.is_open()) file_.close();  // the next piece truncates it and begins the stream again
+  }
+  void finish() override {
+    open();
+    const int rc = cmb_deflate_finish(ctx_, &piece, this, &stats_);
+    settle(rc);
+    file_.flush();
+    if (!file_) throw Panic("Failed to write BAM record");
+    done_ = true;
+  }
+  bool device_deflate() const override { return true; }
+  const cmb_deflate_stats& stats() const { return stats_; }
+
+ private:
+  void open() {
+    if (file_.is_open()) return;
+    file_.open(path_, std::ios::binary | std::ios::trunc);
+    if (!file_) throw Panic("Failed to write BAM file " + path_);
+    created_ = true;
+    if (const int rc = cmb_deflate_begin(ctx_)) throw_device_error(ctx_, rc);
+  }
+  void feed(const uint8_t* p, size_t n) {
+    open();
+    settle(cmb_deflate_feed(ctx_, p, n, &piece, this));
+  }
+  void settle(int rc) {  // the sink's own error first, then the library's
+    if (error_) std::rethrow_exception(std::exchange(error_, nullptr));
+    if (rc) throw_device_error(ctx_, rc);
+  }
+  static int piece(void* user, const uint8_t* p, uint64_t n) {
+    auto* s = static_cast<DeviceDeflateBamSink*>(user);
+    try {
+      s->compressed(p, n);
+      return 0;
+    } catch (...) {
+      s->error_ = std::current_exception();
+      return 1;
+    }
+  }
+  std::string path_;
+  cmb_ctx* ctx_;
+  std::ofstream file_;
+  std::exception_ptr error_;
+  cmb_deflate_stats stats_{};
+  bool created_ = false, done_ = false;
+};
+
 // `filter-names`: the returned records, kept until the input is done
 struct RecordsSink : FilterSink {
   std::vector<uint8_t> bytes;
@@ -164,7 +244,8 @@ struct DeviceSinkCall {
   static int piece(void* user, const uint8_t* p, uint64_t n) {
     auto* s = static_cast<DeviceSinkCall*>(user);
     try {
-      s->sink->records(p, n);
+      if (s->sink->device_deflate()) s->sink->compressed(p, n);
+      else s->sink->records(p, n);
       return 0;
     } catch (...) {
       s->error = std::current_exception();
@@ -209,12 +290,13 @@ inline FilterRun filter_one_input(DeviceSession& session, const InputSpec& in, c
   SinkSettle settle(sink);       // after `header` and `records`: gone before them
   const BlockIndex& bx = stream.index();
   if (bx.bgzf && cmb_filter_bgzf && !getenv("CMB_HOST_DECODE")) {
-    sink.header(header.data(), header.size());  // written on the pool while the device decodes, which does not use it
+    sink.header(header.data(), header.size());  // written on the pool while the device decodes, which does not use it (or
+                                                // fed to the device's deflate stream)
     const BgzfInput bi(bx, (uint32_t)h.header->names.size(), h.records_at, session.pool().size());
     DeviceSinkCall sc;
     sc.sink = &sink;
     cmb_filter_result fr{};
-    rc = cmb_filter_bgzf(ctx, &bi.in, inverse ? 1 : 0, &DeviceSinkCall::piece, &sc, &fr);
+    rc = (sink.device_deflate() ? cmb_filter_bgzf_deflate : cmb_filter_bgzf)(ctx, &bi.in, inverse ? 1 : 0, &DeviceSinkCall::piece, &sc, &fr);
     if (sc.error) std::rethrow_exception(sc.error);
     if (rc == CMB_OK) {
       settle.finish();

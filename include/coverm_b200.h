@@ -401,6 +401,36 @@ typedef struct cmb_filter_result {
 } cmb_filter_result;
 int cmb_filter_bgzf(cmb_ctx* ctx, const cmb_bgzf_input* in, int inverse, cmb_filter_sink sink, void* user, cmb_filter_result* out);
 
+/* ---- BGZF output compressed on the device (`coverm filter --device-deflate`) ----
+ * The context holds one output stream.  Everything fed to it is cut into blocks of 0xff00 bytes counted from the stream's
+ * start (the last one shorter), each block is deflated alone on the GPU (LZ77 inside the block, dynamic Huffman codes, or a
+ * stored block when that is not larger) into one complete BGZF block, and cmb_deflate_finish closes the stream with the
+ * 28-byte EOF block.  A block depends only on its own bytes, so the stream's BGZF bytes are the same however it was fed.
+ * The BGZF bytes go to `sink` (cmb_filter_sink) in pieces of at most 64 MB, each in one of two pinned staging buffers of the
+ * context: the bytes of sink call k stay valid until sink call k + 1 returns (the last call's until the next cmb_deflate_*
+ * call or cmb_destroy).  A sink returning non-zero stops the call with CMB_E_ARG, and the stream must be begun again.
+ *
+ * cmb_deflate_begin starts a new stream and drops whatever the last one held; it allocates the stream's buffers (about
+ * 200 MB of device memory and 128 MB of pinned memory, kept for later streams): CMB_E_NOMEM when they do not fit.
+ * cmb_deflate_feed appends host bytes (the BAM header, or records filtered on the host); the blocks they complete are
+ * handed to the sink before it returns.  cmb_deflate_finish deflates the partial last block and hands it with the EOF block
+ * to the sink, fills *stats and ends the stream.  cmb_filter_bgzf_deflate is cmb_filter_bgzf with the returned records fed
+ * to the context's stream from device memory (they are not copied to the host raw): the sink receives BGZF bytes, and
+ * out->n_bytes counts the raw record bytes fed.  Its CMB_E_DECLINED and CMB_E_NM come as cmb_filter_bgzf's do, possibly
+ * after some sink calls: the caller discards what it received and begins the stream again.  All need a begun stream
+ * (CMB_E_ARG otherwise). */
+typedef struct cmb_deflate_stats {
+  uint64_t raw_bytes, bgzf_bytes; /* fed to the stream; handed to the sink, EOF block included           */
+  uint64_t blocks, stored_blocks; /* BGZF blocks holding data (EOF block excluded); those stored verbatim  */
+  uint32_t sink_calls;
+  float ms_deflate, ms_d2h;       /* deflate + pack kernels (CUDA events); BGZF bytes to the host (host clock) */
+} cmb_deflate_stats;
+int cmb_deflate_begin(cmb_ctx* ctx);
+int cmb_deflate_feed(cmb_ctx* ctx, const uint8_t* bytes, uint64_t n_bytes, cmb_filter_sink sink, void* user);
+int cmb_deflate_finish(cmb_ctx* ctx, cmb_filter_sink sink, void* user, cmb_deflate_stats* stats);
+int cmb_filter_bgzf_deflate(cmb_ctx* ctx, const cmb_bgzf_input* in, int inverse, cmb_filter_sink sink, void* user,
+                            cmb_filter_result* out);
+
 /* The tuples the last successful cmb_submit_bgzf extracted, still resident in device memory (valid until the next
  * cmb_submit_bgzf / cmb_destroy): DEVICE pointers laid out as cmb_read_batch, ready for cmb_submit_device_batch.
  * Lets a caller re-run the filter/scan/reduce kernels over an already decoded sample (device-only timing, parameter sweeps). */

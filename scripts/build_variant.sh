@@ -7,7 +7,7 @@
 set -e
 cd "$(dirname "$0")/../coverm_b200/csrc"
 name=$1; shift
-others="build/cmb_comm.o build/cmb_bgzf.o build/cmb_shard_input.o build/host_api.o"
+others="build/cmb_comm.o build/cmb_bgzf.o build/cmb_shard_input.o build/cmb_deflate.o build/host_api.o"
 mkdir -p ../../variants build
 make $others
 nvcc -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC $* -c cmb_device.cu -o build/cmb_device_$name.o
